@@ -47,7 +47,14 @@ def parse_args():
     ap.add_argument("--config2-samples", type=int, default=4096)
     ap.add_argument("--ops", action="store_true", help="also time index_max / ball_query (config 3)")
     ap.add_argument("--ops-only", action="store_true", help="only time index_max / ball_query and print that JSON")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step of the headline run returned as DIR/<name>.npy (float64): rank "
+                         "0's register_batch arrays and, with --gpus > 1, the all-gathered poses and costs of every rank "
+                         "(gathered_P, gathered_cost); not available with --impl reference or --ops-only")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.ops_only):
+        ap.error("--dump-outputs needs the GPU registration path: not with --impl reference or --ops-only")
+    return args
 
 
 def workload_shape(args):
@@ -64,43 +71,7 @@ def load_measured_peaks():
                 return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def load_traffic(S_local, n_inits, is_2d):
-    """DRAM bytes (read + write) of ONE launch of the dominant kernel, from the committed ncu --set full capture
-    (profiles/r01_traffic.json, written by scripts/ncu_traffic.py) -- only if it was taken on this workload."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    try:
-        with open(p) as f:
-            t = json.load(f)
-        if t["samples_per_gpu"] == S_local and t["inits"] == n_inits and bool(t["is_2d"]) == bool(is_2d):
-            return t["dram_bytes_read"] + t["dram_bytes_write"]
-    except Exception:  # noqa: BLE001
-        pass
-    return None
-
-
-def load_ncu_fractions(S_local, n_inits, is_2d):
-    """What the committed ncu --set full capture of the dominant kernel says about its limiter (SURVEY 8d asks for the
-    FP64-ALU fraction next to the bandwidth fraction; VERDICT r1 for l2 / issue / dram as well); None when the capture
-    is of another workload."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    try:
-        with open(p) as f:
-            t = json.load(f)
-        if t["samples_per_gpu"] == S_local and t["inits"] == n_inits and bool(t["is_2d"]) == bool(is_2d):
-            secs = t["gpu_time_ns"] * 1e-9
-            l2_bytes = t.get("lts_t_bytes") or ((t.get("l2_read_sectors_from_l1") or 0) * 32.0)
-            return {"issue_frac": (t.get("issue_active_pct") or 0) / 100.0, "fp64_frac": (t.get("fp64_pipe_active_pct") or 0) / 100.0,
-                    "dram_frac": (t.get("dram_throughput_pct") or 0) / 100.0,
-                    "l2_to_l1_GBps": l2_bytes / secs / 1e9 if secs > 0 else None,
-                    "warps_active_frac": (t.get("warps_active_pct") or 0) / 100.0,
-                    "lts_t_bytes": t.get("lts_t_bytes"), "dram_bytes": t["dram_bytes_read"] + t["dram_bytes_write"],
-                    "source": "profiles/r02_traffic.json (%s)" % t.get("source")}
-    except Exception:  # noqa: BLE001
-        pass
-    return None
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 class ClockSampler:
@@ -407,7 +378,7 @@ def main():
     pred_d = pred_pin.to(dev)
     K_d = torch.as_tensor(Kmat, dtype=torch.float64).reshape(1, 9).expand(S_local, 9).contiguous().to(dev)
     n_total = S_local * world
-    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
 
     def flush_l2():
         flush_buf.fill_(1)
@@ -499,6 +470,11 @@ def main():
     sampler2.mark_begin()
     ms_total = timed_overlapped(args.steps)
     sampler2.mark_end()
+    if args.dump_outputs and rank == 0:
+        last = dict(outs[(args.steps - 1) % n_bufs])
+        if world > 1:                                    # equal shards: the gathered buffer holds every rank's records
+            last["gathered_P"], last["gathered_cost"] = sharding.unpack_records(gathered[(args.steps - 1) & 1])
+        dump_outputs(args.dump_outputs, last)
     clocks_overlapped = sampler2.stop() if rank == 0 else None
     ms_per_step = ms_total / args.steps
     value = n_total / (ms_per_step * 1e-3)
@@ -590,7 +566,6 @@ def main():
             dist.destroy_process_group()
         return
 
-    ncu = load_ncu_fractions(S_local, n_inits, is_2d)
     line = {
         "metric": "registrations/sec", "value": value, "unit": "registrations/s", "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True,
@@ -604,7 +579,7 @@ def main():
                                  "`configs` sub-records of this line",
             "l2": "value and e2e: %d steps issued back to back on two alternating streams inside ONE event bracket (the tail of "
                   "one step's persistent kernel overlaps the head of the next); no flush between them -- each step streams "
-                  "136 MB of inputs + a 168 MB packed copy, more than the 126 MB L2; `serial` = the same steps one at a time "
+                  "136 MB of inputs + a 168 MB packed copy, more than the 50 MB L2; `serial` = the same steps one at a time "
                   "with an L2 flush before each" % args.steps,
             "step": "ONE C-ABI call frustum_register_batch_f32 = prepare (initial guess + front filter + Morton sort + "
                     "Philox inits) + boxes + order + LM solve + arg-min/degenerate rule"
@@ -621,9 +596,9 @@ def main():
                            "summed, max over ranks; the roofline block below is measured on these steps"},
         "roofline": {
             "bound": "issue",
-            "bound_note": "limiter per ncu = instruction issue / dependent fp64 latency (profiles/); DRAM moves ~1.3x the "
-                          "compulsory bytes. achieved/peak/frac below are SURVEY 8d's streamed-model HBM-equivalent: 13 B x "
-                          "points x cloud passes, divided by the measured copy bandwidth",
+            "bound_note": "not HBM: the box cull and the L2 serve most of the streamed bytes (frac can exceed 1), the "
+                          "limiter is instruction issue / dependent fp64 latency (DESIGN.md 4.4). achieved/peak/frac below "
+                          "are SURVEY 8d's streamed-model HBM-equivalent: 13 B x points x cloud passes, divided by peak",
             "kernel": "frustum_solve_kernel<float,%d>" % (4 if is_2d else 6),
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
             "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": k_ms, "kernel_ms_all": kern_ms,
@@ -638,8 +613,6 @@ def main():
             "point_evals_per_s": pts_evals / args.steps / (k_ms * 1e-3),
             "mean_cloud_passes_per_solve": passes_mean, "mean_lm_iterations_per_solve": iters_mean,
             "compulsory_bytes_per_launch": compulsory,
-            "traffic": load_traffic(S_local, n_inits, is_2d),
-            "secondary": ncu,
         },
     }
 
@@ -688,6 +661,27 @@ def main():
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, res):
+    """Output arrays (first axis = sample) as float64 .npy files.  Beyond DUMP_LIMIT_BYTES a fixed, seeded subset of
+    the samples (rows of every array; of every rank's for the gathered ones) is written, with the chosen ids of the
+    local samples in sample_index.npy."""
+    arrays = {k: v.detach().cpu().numpy().astype(np.float64) for k, v in sorted(res.items())}
+    S = res["P"].shape[0]
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        world = next((a.shape[0] for k, a in arrays.items() if k.startswith("gathered_")), S) // max(S, 1)
+        keep = np.sort(np.random.default_rng(0).choice(S, int(S * DUMP_LIMIT_BYTES // (total + 8 * S)), replace=False))
+        rows = np.concatenate([r * S + keep for r in range(world)])
+        arrays = {k: a[rows] if k.startswith("gathered_") else a[keep] for k, a in arrays.items()}
+        arrays["sample_index"] = keep.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
 
 
 def bench_config1(torch, frustum, lib, dev, n_points, is_2d, flush, peak, smi_index):
@@ -797,7 +791,7 @@ def cpu_and_parity(torch, frustum, dev, args, xyz_d, pred_d, n_points, K_d, H, W
     res = {"cpu_baseline": {
         "value": count / dt, "unit": "registrations/s", "cores": cores, "kind": "port",
         "sample": "%d registrations x %d inits of the same workload (first samples of the GPU batch, device-made inits), oracle "
-                  "port of the Ceres path (Ceres is installed neither here nor on the GPU box: profiles/r02_probe_ceres_gpu_box.txt), "
+                  "port of the Ceres path (Ceres is not installed), "
                   "all solves spread over %d threads, best of %d runs" % (count, n_inits, cores, len(dts)),
         "spread": {"runs_s": dts, "min_value": count / max(dts), "max_value": count / min(dts)}},
         "parity": {
@@ -810,14 +804,14 @@ def cpu_and_parity(torch, frustum, dev, args, xyz_d, pred_d, n_points, K_d, H, W
         "registrations": count, "registrations_within_gate": reg_ok,
         "registrations_gpu_cost_le_oracle": cost_le,
         "best_of_I_max_rot_err_rad": worst_r, "best_of_I_max_trans_err_m": worst_t,
-        "note": "trajectories are chaotic at rounding level; every out-of-gate solve of a 1440-solve run is traced to its first "
-                "divergent evaluation in profiles/r02_trace_divergence.md"}}
+        "note": "trajectories are chaotic at rounding level (DESIGN.md 3.1); tests/tools/trace_divergence.py traces an "
+                "out-of-gate solve to its first divergent evaluation"}}
     return res
 
 
 def bench_ops(torch, dev, peak):
     """BASELINE config 3: index_max + ball_query forward, B=64, C=M=64, N=16384, K=64.
-    Inputs are 2 x 268 MB per op (> 126 MB L2) and the timed iterations alternate between two
+    Inputs are 2 x 268 MB per op (> 50 MB L2) and the timed iterations alternate between two
     distinct input sets, so every byte comes from HBM and no dirty flush lines compete with it."""
     from deepi2p_b200 import point_ops
     B, C, N, K = 64, 64, 16384, 64

@@ -1,4 +1,4 @@
-"""deepi2p_b200 -- B200-native (sm_100a) inverse-camera-projection registration path of DeepI2P.
+"""deepi2p_b200 -- H100-native (sm_90a) inverse-camera-projection registration path of DeepI2P.
 
 Scope (SURVEY.md section 8): the Ceres-backed solver FrustumRegistration.solvePGivenK and the
 multi-start loop around it, plus the two CUDA ops of the classifier (index_max, ball_query),
@@ -15,7 +15,7 @@ _DROPIN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "dropin")
 
 def install_dropins():
     """Make `import FrustumRegistration`, `import index_max`, `import ball_query` resolve to the
-    B200 implementations (prepends deepi2p_b200/dropin to sys.path)."""
+    CUDA implementations (prepends deepi2p_b200/dropin to sys.path)."""
     if _DROPIN_DIR not in sys.path:
         sys.path.insert(0, _DROPIN_DIR)
     return _DROPIN_DIR

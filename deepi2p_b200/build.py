@@ -1,4 +1,4 @@
-"""Build the sm_100a CUDA library in-tree: deepi2p_b200/lib/libdeepi2p_b200.so.
+"""Build the sm_90a (H100) CUDA library in-tree: deepi2p_b200/lib/libdeepi2p_b200.so.
 
     python -m deepi2p_b200.build [--force] [--verbose]
 
@@ -16,7 +16,7 @@ LIB = os.path.join(LIBDIR, "libdeepi2p_b200.so")
 SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "ball_query_xyz.cu", "cluster_assign.cu"]
 HEADERS = ["common.cuh", os.path.join("..", "..", "include", "deepi2p_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
     "--fmad=true",

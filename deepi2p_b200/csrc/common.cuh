@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels: error plumbing for the C ABI and thin PTX wrappers
+// Shared helpers for the sm_90a kernels: error plumbing for the C ABI and thin PTX wrappers
 // for the mbarrier + 1-D bulk-copy (TMA engine, SASS UBLKCP) staging used by the solver.
 #pragma once
 #include <cuda_runtime.h>

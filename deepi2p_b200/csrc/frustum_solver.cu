@@ -1,5 +1,5 @@
 // Batched robust bounded Levenberg-Marquardt solver for the inverse-camera-projection
-// ("frustum") registration problem, written for sm_100a.
+// ("frustum") registration problem, written for sm_90a (H100).
 //
 // Replaces FrustumRegistration.solvePGivenK (evaluation/frustum_reg/src/registration.cpp:9-186)
 // and the multi-start loop around it (evaluation/registration_lsq.py:127-186).
@@ -46,10 +46,9 @@ void set_error(const char* fmt, ...) {
 // Team shape: warps per CTA (= the help domain: warps that can take slices of each other's passes) x CTAs per SM
 // (= problems in flight per SM / warps per CTA).  The register budget decides the product: 20 warps x 32 lanes x 96
 // registers for the 4-DoF solver, 14 for 6-DoF (128 registers) and for the f64 record (rings twice as large); shared
-// memory (rings + accumulators + per-problem state, ~10.6 KB per 4-DoF warp) is checked below.  Measured on B200, 512 x
-// 60 problems (profiles/r02_sweep_schedule.jsonl): 20 x 1: 77.5 ms, 10 x 2: 76.8, 5 x 4: 76.5, 4 x 5: 76.7 -- smaller
-// CTAs leave the SM earlier at the end of a launch (the next launch's CTAs start there); 10 x 2 keeps a help domain of
-// 10 warps, which is what a small batch's 10 slices per pass can use.
+// memory (rings + accumulators + per-problem state, ~10.6 KB per 4-DoF warp) is checked below.  An H100 SM has 64 K
+// registers and 228 KB of shared memory.  Smaller CTAs leave the SM earlier at the end of a launch (the next launch's
+// CTAs start there); 10 x 2 keeps a help domain of 10 warps, which is what a small batch's 10 slices per pass can use.
 #ifndef DIB_WARPS_F4
 #define DIB_WARPS_F4 10
 #endif
@@ -778,9 +777,8 @@ __device__ __forceinline__ void eval_slice(WarpScratch<CT, P>& ws, const ProbCtx
     };
 #pragma unroll 1
     do {
-      // (issuing the NEXT step's loads before this step is classified -- a register software pipeline -- measured
-      // 12 % slower on B200, 87.1 vs 77.6 ms per 512 x 60 problems: the registers it needs cost more than the latency
-      // it hides; profiles/r02_sweep_schedule.jsonl)
+      // (issuing the NEXT step's loads before this step is classified -- a register software pipeline -- is not done:
+      // the registers it needs cost more than the latency it hides)
       CT gx[DIB_GPS], gy[DIB_GPS], gz[DIB_GPS];
       int glab[DIB_GPS];
       bool all_sure = true;
@@ -1928,7 +1926,7 @@ static thread_local void* g_ev_stop = nullptr;
 
 // Per-device launch configuration of a solver instantiation, looked up once (cudaFuncSetAttribute and the
 // occupancy query cost tens of microseconds per call, which the single-problem drop-in path would pay every time).
-struct LaunchCfg { int sms = 0, per_sm = 0; };
+struct LaunchCfg { int sms = 0, per_sm = 0, l2_bytes = 0; };
 template <typename CT, int P>
 static int solver_launch_cfg(LaunchCfg* out) {
   static LaunchCfg cache[64];
@@ -1940,6 +1938,7 @@ static int solver_launch_cfg(LaunchCfg* out) {
   LaunchCfg c;
   DIB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   DIB_CHECK_CUDA(cudaDeviceGetAttribute(&c.sms, cudaDevAttrMultiProcessorCount, dev));
+  DIB_CHECK_CUDA(cudaDeviceGetAttribute(&c.l2_bytes, cudaDevAttrL2CacheSize, dev));
   DIB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c.per_sm, kern, Cfg<CT, P>::kWarps * 32, smem));
   if (c.per_sm < 1) { set_error("solver kernel does not fit an SM (%zu B shared memory)", smem); return DIB_ECUDA; }
   if (dev >= 0 && dev < 64) cache[dev] = c;
@@ -1977,12 +1976,16 @@ static int launch_solve(const SolveArgs& a_in, cudaStream_t st) {
   if (grid > total) grid = total;
   // scheduling chunk: the queue walks chunks of samples rank-major (longest-predicted inits of every sample of the
   // chunk first).  Larger chunks start the long solves earlier (shorter tail); smaller chunks keep the packed clouds
-  // of the concurrently running problems inside the 126 MB L2.  Measured on B200, 512 x 60 problems, this kernel
-  // (profiles/r02_sweep_schedule.jsonl): 64 samples 90.5 ms, 98 (32 MB) 90.4, 128 89.5, 171 88.8, 256 (84 MB) 87.2,
-  // 512 (no chunking, 167 MB) 88.7 -> aim at ~80 MB of packed clouds per chunk, at least ~2x the resident problems.
+  // of the concurrently running problems inside the L2.  H100 (50 MB L2), 512 x 60 problems of 20480 points, chunk set
+  // with DIB_CHUNK_SAMPLES (DESIGN.md 4.3.3): at a 700 W power limit, bench.py's headline (4 steps back to back on two
+  // streams, alternating runs) gives 6077-6090 reg/s at 86 samples (28 MB of packed clouds), 6012-6057 at 256 (84 MB),
+  // 5950 at 512 (no chunking); at a 400 W limit, 8 steps back to back per value, three interleaved repetitions:
+  // 86 samples 107.9 ms per step, 128 (42 MB) 109.2, 171 (56 MB) 111.5, 256 115.5, 512 120.9.  -> aim at 5/8 of the L2
+  // per chunk, at least ~2x the resident problems.
   long long chunk = (2 * grid * kW + a.I - 1) / a.I;
   const long long bytes_per_sample = (long long)a.rounds_max * kRoundPoints * (long long)sizeof(Entry<CT>);
-  if (bytes_per_sample > 0 && chunk < (80ll << 20) / bytes_per_sample) chunk = (80ll << 20) / bytes_per_sample;
+  const long long chunk_bytes = (long long)cfg.l2_bytes * 5 / 8;
+  if (bytes_per_sample > 0 && chunk < chunk_bytes / bytes_per_sample) chunk = chunk_bytes / bytes_per_sample;
   if (const char* e = getenv("DIB_CHUNK_SAMPLES")) chunk = atoll(e);   // tuning knob
   if (chunk < 1) chunk = 1;
   if (chunk > a.S) chunk = a.S;

@@ -1,4 +1,4 @@
-// index_max (segmented arg-max) and ball_query (first-K-within-radius) for sm_100a.
+// index_max (segmented arg-max) and ball_query (first-K-within-radius) for sm_90a.
 //
 // index_max replaces models/index_max_ext/index_max_cuda.cu:30-62 (one thread per (b,c) scanning
 // N floats with stride C*N between neighbouring threads).  Here a CTA owns (b, a group of

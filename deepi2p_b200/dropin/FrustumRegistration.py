@@ -1,6 +1,6 @@
 """Drop-in for the reference's pybind11 module `FrustumRegistration`
 (evaluation/frustum_reg/src/registration.cpp:190-213): same module name, same function name,
-same keyword names, same return tuple -- backed by the sm_100a batched solver instead of Ceres.
+same keyword names, same return tuple -- backed by the sm_90a batched solver instead of Ceres.
 
     import deepi2p_b200; deepi2p_b200.install_dropins()
     import FrustumRegistration

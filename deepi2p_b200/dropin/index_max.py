@@ -1,6 +1,6 @@
 """Drop-in for the reference's torch extension `index_max` (models/index_max_ext/index_max.cpp:154-159).
 
-forward_cuda and forward_cuda_shared_mem run the sm_100a segmented-argmax kernel on CUDA tensors.  The reference's
+forward_cuda and forward_cuda_shared_mem run the sm_90a segmented-argmax kernel on CUDA tensors.  The reference's
 CPU entry points (forward_cpu, forward_multi_thread_cpu; index_max.cpp:73-112) take and return CPU tensors; this
 framework has no CPU compute path, so they keep that CONTRACT (CPU tensors in, int32 CPU tensor out, identical
 indices) but compute on the GPU: host -> device copy, the same kernel, device -> host copy.  Without a CUDA device

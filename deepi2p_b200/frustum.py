@@ -1,7 +1,7 @@
 """Host side of the registration path: thin Python over the C ABI (include/deepi2p_b200.h).
 
 torch is used only for device memory, streams and pinned host buffers; every computation is a
-hand-written sm_100a kernel reached through ctypes.  No CPU fallback exists: without a CUDA
+hand-written sm_90a kernel reached through ctypes.  No CPU fallback exists: without a CUDA
 device or without the compiled library every entry point raises.
 
 Mirrors, in order of the reference's call stack (SURVEY.md 3.1):
@@ -27,7 +27,7 @@ TERMINATION = ("gradient_tolerance", "parameter_tolerance", "function_tolerance"
 
 def _require_cuda():
     if not torch.cuda.is_available():
-        raise _native.NativeError("deepi2p_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise _native.NativeError("deepi2p_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
 
 
 def _stream_ptr(stream=None):

@@ -1,4 +1,4 @@
-/* deepi2p_b200 -- C ABI of the B200-native inverse-camera-projection registration path.
+/* deepi2p_b200 -- C ABI of the H100-native inverse-camera-projection registration path.
  *
  * Plain C, no torch / pybind types: every pointer marked [dev] is a CUDA device pointer owned
  * by the caller, every launch goes to the cudaStream_t the caller passes (0 = legacy default
@@ -34,7 +34,7 @@ extern "C" {
 #define DIB_EINVAL (-22)   /* bad argument (shape, alignment, NULL)            */
 #define DIB_ENOMEM (-12)   /* workspace too small                              */
 #define DIB_ECUDA (-5)     /* a CUDA runtime call failed; see dib_last_error() */
-#define DIB_ENODEV (-19)   /* no sm_100 device                                 */
+#define DIB_ENODEV (-19)   /* no sm_90 device                                  */
 
 typedef void* dib_stream_t; /* cudaStream_t */
 

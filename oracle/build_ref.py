@@ -37,7 +37,7 @@ def built(name):
 def build(verbose=False):
     if not available():
         return None
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "4")
     from torch.utils import cpp_extension
     os.makedirs(OUT, exist_ok=True)

@@ -18,7 +18,6 @@
 //     steps, default tolerances) from its documentation / memory of
 //     trust_region_minimizer.cc, levenberg_marquardt_strategy.cc, dense_qr_solver.cc,
 //     corrector.cc, loss_function.cc, line_search.cc, polynomial.cc, parameter_block.h.
-// Checked on the GPU box as well (profiles/r02_probe_ceres_gpu_box.txt): no Ceres, no Eigen there either.
 // Known deliberate deviation: roots of the degree-4 derivative polynomial in the 3-sample
 // line-search interpolation are found by (total-step) Durand-Kerner iteration instead of companion
 // matrix eigenvalues (same roots, different rounding).

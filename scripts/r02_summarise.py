@@ -74,7 +74,7 @@ if os.path.exists(rep):
     tmp = "/tmp/%s_cubin" % tag
     os.makedirs(tmp, exist_ok=True)
     run("cuobjdump", "-xelf", "all", os.path.join(ROOT, "deepi2p_b200", "lib", "libdeepi2p_b200.so"), cwd=tmp)
-    dis = run("nvdisasm", "-c", os.path.join(tmp, "frustum_solver.sm_100a.cubin")).stdout
+    dis = run("nvdisasm", "-c", os.path.join(tmp, "frustum_solver.sm_90a.cubin")).stdout
     open("/tmp/%s.disasm" % tag, "w").write(dis)
     evals = "1547000"
     try:

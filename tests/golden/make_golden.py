@@ -4,8 +4,8 @@ oracle/build_ref.py.  Run in the build container only (the GPU box has no /root/
 
     python oracle/build_ref.py && python tests/golden/make_golden.py
 
-ball_query has no CPU implementation in the reference, and the solver needs Ceres, so neither has
-a fixture; see tests/test_ops_gpu.py::test_against_reference_kernels for the on-box check.
+ball_query has no CPU implementation in the reference: its fixture comes from the reference's CUDA
+kernel (tests/golden/make_ref_kernels_golden.py).  The solver needs Ceres and has no reference fixture.
 """
 import os
 import sys

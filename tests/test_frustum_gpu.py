@@ -80,9 +80,9 @@ def test_solve_matches_oracle(cuda, is_2d):
     ~3-4 % of full-size solves by > 1e-7 (tests/tools/parity_sensitivity_cpu.py).  The gate is therefore
     statistical: at least 97 % of the (sample, init) solves within 1e-4 rad / 1e-3 m of the oracle, 93 % with
     identical iteration / evaluation / termination records, a tiny median difference, and per registration either the
-    same best-of-I pose or a GPU best cost that is not worse than the oracle's.  (profiles/r02_trace_divergence.md
-    traces every out-of-gate solve of a 1440-solve full-size run to its first divergent evaluation and shows that
-    the same solves leave the gate when EITHER implementation's own input is moved by one ulp.)"""
+    same best-of-I pose or a GPU best cost that is not worse than the oracle's.  (tests/tools/trace_divergence.py
+    traces an out-of-gate solve to its first divergent evaluation; DESIGN.md 3.1 explains why such solves leave the
+    gate when either implementation's own input is moved by one ulp.)"""
     S, I, n = 10, 12, 4096
     xs, ls, inits, Ks = [], [], [], []
     smps = []

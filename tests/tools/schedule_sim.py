@@ -1,9 +1,10 @@
 """List-scheduling model of the solver's persistent grid: W workers (resident warps), problems taken in queue order
 (chunks of samples, rank-major inside a chunk), each problem busy for `evals` passes.  Compares scheduling orders by
 the modelled makespan and the modelled tail (queue empty -> last finish), in passes.  CPU tool over the .npz written by
-tests/tools/dump_solve_lengths.py."""
+tests/tools/dump_solve_lengths.py, or over a directory written by bench.py --dump-outputs (init.npy, stats.npy)."""
 import argparse
 import heapq
+import os
 
 import numpy as np
 
@@ -39,11 +40,11 @@ def simulate(evals, order, W):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("npz")
-    ap.add_argument("--workers", type=int, default=2960)
-    ap.add_argument("--chunk", type=int, default=256)
+    ap.add_argument("npz", help="dump_solve_lengths.py .npz or bench.py --dump-outputs directory")
+    ap.add_argument("--workers", type=int, default=2640)       # H100: 132 SMs x 2 CTAs x 10 warps
+    ap.add_argument("--chunk", type=int, default=86)          # the solver's chunk for 512 x 60 on an H100
     a = ap.parse_args()
-    d = np.load(a.npz)
+    d = {k: np.load(os.path.join(a.npz, k + ".npy")) for k in ("init", "stats")} if os.path.isdir(a.npz) else np.load(a.npz)
     init, stats = d["init"], d["stats"]
     evals = stats[..., 1].astype(np.float64)
     S, I = evals.shape
@@ -54,10 +55,10 @@ def main():
         "true length (bound)": evals,
         "random": np.random.default_rng(0).random((S, I)),
         "queue = init index": -np.arange(I)[None, :].repeat(S, 0).astype(np.float64),
-        "cost at init": d["cost0"],
-        "gradient max-norm at init": d["gnorm0"],
         "translation offset norm": np.linalg.norm(dt, axis=2),
     }
+    if "cost0" in d:                                                  # dump_solve_lengths.py only
+        keys.update({"cost at init": d["cost0"], "gradient max-norm at init": d["gnorm0"]})
     ideal = evals.sum() / a.workers
     print("S %d I %d  passes mean %.1f max %d  ideal makespan %.1f passes" % (S, I, evals.mean(), evals.max(), ideal))
     from scipy.stats import spearmanr
