@@ -20,6 +20,7 @@ EXPORTS = (
     "frustum_inside_mask_f32", "pose_error_batch",
     "index_max_forward", "ball_query_forward", "ball_query_xyz_workspace_bytes", "ball_query_xyz_forward",
     "cluster_assign_workspace_bytes", "cluster_assign_forward",
+    "pnp_ransac_workspace_bytes", "pnp_ransac_batch_f32", "epnp_batch_f64",
 )
 
 
@@ -120,6 +121,13 @@ def load():
     lib.cluster_assign_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]
     lib.ball_query_forward.restype = i32
     lib.ball_query_forward.argtypes = [vp, _c.c_float, vp, i32, i32, i32, i32, vp]
+    lib.pnp_ransac_workspace_bytes.restype = sz
+    lib.pnp_ransac_workspace_bytes.argtypes = [i32, i32, i32]
+    lib.pnp_ransac_batch_f32.restype = i32
+    lib.pnp_ransac_batch_f32.argtypes = [vp, vp, vp, vp, i32, i32, vp, f64, f64, f64, i32, f64, f64, _c.c_uint64,
+                                         vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.epnp_batch_f64.restype = i32
+    lib.epnp_batch_f64.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp]
     _lib = lib
     return lib
 

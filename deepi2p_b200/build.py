@@ -13,7 +13,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdeepi2p_b200.so")
-SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "ball_query_xyz.cu", "cluster_assign.cu"]
+SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "ball_query_xyz.cu", "cluster_assign.cu",
+           "pnp_ransac.cu"]
+# Compiled on their own without FMA contraction: oracle_pnp/pnp_oracle.cpp restates their arithmetic bit for bit.
+NOFMA_SOURCES = ["pnp_ransac.cu"]
 HEADERS = ["common.cuh", os.path.join("..", "..", "include", "deepi2p_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -42,6 +45,21 @@ def is_stale():
     return any(os.path.exists(d) and os.path.getmtime(d) > t for d in deps)
 
 
+def _nofma_objects(objdir, extra, verbose):
+    """Compile NOFMA_SOURCES to objects in objdir with --fmad=false; returns their paths."""
+    flags = [f for f in NVCC_FLAGS if f not in ("-shared", "--fmad=true")]
+    objs = []
+    for s in NOFMA_SOURCES:
+        obj = os.path.join(objdir, os.path.splitext(s)[0] + ".nofma.o")
+        cmd = [nvcc_path(), *flags, "--fmad=false", *extra, *os.environ.get("DIB_NVCC_EXTRA", "").split(), "-c",
+               "-o", obj, os.path.join(CSRC, s)]
+        if verbose:
+            print(" ".join(cmd), flush=True)
+        subprocess.check_call(cmd)
+        objs.append(obj)
+    return objs
+
+
 def build(force=False, verbose=False, extra=(), out=None):
     """Compile the library in-tree.  `out` names a variant file (lib/variants/<out>.so) instead of the default
     library; variants are a tuning aid (scripts/ab_prebuilt.sh) selected at run time with DIB_LIB_OVERRIDE."""
@@ -49,7 +67,7 @@ def build(force=False, verbose=False, extra=(), out=None):
         vdir = os.path.join(LIBDIR, "variants")
         os.makedirs(vdir, exist_ok=True)
         target = os.path.join(vdir, out + ".so")
-        srcs = [os.path.join(CSRC, s) for s in SOURCES]
+        srcs = [os.path.join(CSRC, s) for s in SOURCES if s not in NOFMA_SOURCES] + _nofma_objects(vdir, extra, verbose)
         cmd = [nvcc_path(), *NVCC_FLAGS, *extra, *os.environ.get("DIB_NVCC_EXTRA", "").split(), "-o", target, *srcs]
         if verbose:
             print(" ".join(cmd), flush=True)
@@ -58,7 +76,8 @@ def build(force=False, verbose=False, extra=(), out=None):
     if not force and not is_stale():
         return LIB
     os.makedirs(LIBDIR, exist_ok=True)
-    srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
+    srcs = [os.path.join(CSRC, s) for s in SOURCES if s not in NOFMA_SOURCES and os.path.exists(os.path.join(CSRC, s))]
+    srcs += _nofma_objects(LIBDIR, extra, verbose)
     env_extra = os.environ.get("DIB_NVCC_EXTRA", "").split()
     cmd = [nvcc_path(), *NVCC_FLAGS, *extra, *env_extra, "-o", LIB + ".tmp", *srcs]
     if verbose:

@@ -100,6 +100,67 @@ def load_batch(data_dir, names=None, which="coarse_prediction", enu2cam=False):
     return dict(names=list(names), xyz=xyz, label=label, n_pts=n_pts, K=K, P_gt=P)
 
 
+def load_batch_fine(data_dir, names=None, coarse="coarse_prediction", fine="fine_prediction", enu2cam=False):
+    """Legacy directory -> host arrays for the PnP path (registration_pnp.py:185-196 reads the same rows).
+
+    Returns dict(names, xyz f32 [S,3,Nmax], coarse int8 [S,Nmax] (1 = predicted inside, 0 otherwise and on padding),
+    fine int32 [S,Nmax] (grid cell), n_pts int32 [S], K f64 [S,9], P_gt f64 [S,4,4])."""
+    if names is None:
+        names = list_records(data_dir)
+    rec = load_batch(data_dir, names, coarse, enu2cam)
+    S, n_max = rec["label"].shape
+    fine_rows = np.zeros((S, n_max), dtype=np.int32)
+    for s, name in enumerate(names):
+        _, f, _, _ = load_record(data_dir, name, fine, enu2cam)
+        if f.size and (f.min() < -2 ** 31 or f.max() >= 2 ** 31):
+            raise ValueError("%s: fine cell indices do not fit int32" % name)
+        fine_rows[s, :f.shape[0]] = f
+    coarse_rows = (rec["label"] == 1).astype(np.int8)
+    return dict(names=rec["names"], xyz=rec["xyz"], coarse=coarse_rows, fine=fine_rows, n_pts=rec["n_pts"],
+                K=rec["K"], P_gt=rec["P_gt"])
+
+
+def register_directory_pnp(data_dir, H, W, fine_scale=1 / 32.0, iterations=500, reproj_err=0.6, confidence=0.99,
+                           seed=0, enu2cam=False, batch=512, names=None, device="cuda", out_dir=None):
+    """The __main__ of evaluation/registration_pnp.py:151-259 as one function: every frame of a legacy directory
+    through pnp.pnp_ransac_batch (the GPU path), errors by frustum.pose_error_batch, and the P_pred_all_np /
+    P_gt_all_np / cost_all_np files (cost = outlier ratio) the analysis script expects (:257-259)."""
+    import torch
+    from . import frustum, pnp
+
+    if names is None:
+        names = list_records(data_dir)
+    P_pred = np.zeros((len(names), 4, 4))
+    P_gt = np.zeros((len(names), 4, 4))
+    cost = np.zeros((len(names),))
+    for a in range(0, len(names), batch):
+        rec = load_batch_fine(data_dir, names[a:a + batch], enu2cam=enu2cam)
+        S, n_in = rec["coarse"].shape
+        ns = frustum.round_up(max(n_in, 1), 16)
+        dev = torch.device(device)
+        xyz = torch.zeros((S, 3, ns), dtype=torch.float32, device=dev)
+        c8 = torch.zeros((S, ns), dtype=torch.int8, device=dev)
+        f32 = torch.zeros((S, ns), dtype=torch.int32, device=dev)
+        xyz[:, :, :n_in] = torch.from_numpy(rec["xyz"]).to(dev)
+        c8[:, :n_in] = torch.from_numpy(rec["coarse"]).to(dev)
+        f32[:, :n_in] = torch.from_numpy(rec["fine"]).to(dev)
+        n_pts = torch.from_numpy(rec["n_pts"]).to(dev)
+        out = pnp.pnp_ransac_batch(xyz, c8, f32, n_pts, rec["K"], H, W, scale=fine_scale, iterations=iterations,
+                                   reproj_err=reproj_err, confidence=confidence, seed=seed + a)
+        P_pred[a:a + batch] = out["P"].cpu().numpy()
+        cost[a:a + batch] = out["outlier_ratio"].cpu().numpy()
+        P_gt[a:a + batch] = rec["P_gt"]
+    err = frustum.pose_error_batch(P_pred, P_gt)
+    t_err, r_err, ok = err["t_err"].cpu().numpy(), err["r_err"].cpu().numpy(), err["success"].cpu().numpy()
+    if out_dir is not None:
+        os.makedirs(out_dir, exist_ok=True)
+        np.save(os.path.join(out_dir, "P_pred_all_np.npy"), P_pred)
+        np.save(os.path.join(out_dir, "P_gt_all_np.npy"), P_gt)
+        np.save(os.path.join(out_dir, "cost_all_np.npy"), cost)
+    return dict(names=names, P_pred=P_pred, P_gt=P_gt, cost=cost, t_err=t_err, r_err=r_err, success=ok,
+                summary=summarize(t_err, r_err, cost, ok))
+
+
 def summarize(t_err, r_err, cost, ok):
     """registration_result_analysis.py:19-47 on the per-frame errors: frames with cost <= 1e-6 are dropped,
     RTE/RRE mean and sigma, success rate over the kept frames."""

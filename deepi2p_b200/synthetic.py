@@ -52,6 +52,25 @@ def make_sample(seed, n_points=20480, shape="kitti", flip=0.05):
                 ry_gt=ry, t_gt=t)
 
 
+def make_fine_labels(sample, scale=1 / 32.0, noise=0.3, seed=0):
+    """Fine predictions of a make_sample() frame: the fine-label rule of visualize_and_save_data.py:137-139 (cell
+    floor(u * scale) + floor(v * scale) * round(W * scale) of the GT projection), with a seeded fraction `noise` of the
+    points moved to a uniformly random cell.  Points behind the camera get cell 0.  Returns int32 [N]."""
+    P, K = sample["P_gt"], sample["K"]
+    q = P[:3, :3] @ sample["points"].astype(np.float64) + P[:3, 3:4]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        u = K[0, 0] * q[0] / q[2] + K[0, 2]
+        v = K[1, 1] * q[1] / q[2] + K[1, 2]
+    Wf, Hf = int(round(sample["W"] * scale)), int(round(sample["H"] * scale))
+    ok = (q[2] > 0.1) & np.isfinite(u) & np.isfinite(v)
+    cell = np.zeros(u.shape, dtype=np.int64)
+    cell[ok] = np.floor(u[ok] * scale).astype(np.int64) + np.floor(v[ok] * scale).astype(np.int64) * Wf
+    rng = np.random.default_rng(seed + 0xF1E)
+    moved = rng.uniform(size=cell.shape) < noise
+    cell = np.where(moved, rng.integers(0, Wf * Hf, cell.shape), cell)
+    return np.clip(cell, -2**31, 2**31 - 1).astype(np.int32)
+
+
 def make_inits(seed, init_y_angle, n_inits=60, ry_sigma=10.0 * math.pi / 180.0, t_amp=10.0):
     """The multi-start inits of registration_lsq.py:163-164, materialised:
     ry_i = init_y_angle + N(0, sigma), t_i = (0, 0, U(-amp, amp)).  Returns (ry[I], t[I,3])."""

@@ -240,6 +240,36 @@ int cluster_assign_forward(const float* pc, const float* node, int B, int N, int
                            int32_t* min_idx, int32_t* count, float* cluster_mean, float* pc_centers,
                            float* pc_decentered, void* workspace, size_t workspace_bytes, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * PnP-RANSAC registration from grid classifications (evaluation/registration_pnp.py:95-148: cv2.solvePnPRansac with
+ * SOLVEPNP_EPNP, iterationsCount, reprojectionError), batched over S frames.  DESIGN.md "PnP-RANSAC" states the
+ * contract.  Per frame: points with coarse_pred == 1 are kept (n_sel of them, input order); fine cell f -> pixel
+ * CORNER py = floor(f / Wf), px = f - py * Wf, Wf = W * scale, float64; K_f = scale * K (K[0][1] ignored);
+ * hypothesis h samples 5 distinct indices with Philox4x32-10, counter (h, s, draw, 0), key = seed, solves EPnP and
+ * counts inliers ((u-px)^2 + (v-py)^2 <= reproj_err^2); sequential adaptive stop (niters = min(niters,
+ * ceil(log(1-confidence) / log(1-w^5))) on each strictly better hypothesis with >= 5 inliers); EPnP refit on the
+ * winner's inliers.  P = I and outlier_ratio = 1 when n_sel < 4, no hypothesis wins, EPnP fails or |t| >= 14.14;
+ * else outlier_ratio = 1 - inliers / n_sel.  4 <= n_sel <= 5: EPnP on all points, inliers counted under that pose.
+ *   xyz [S][3][n_stride] f32, coarse_pred [S][n_stride] int8, fine_pred [S][n_stride] int32, n_pts [S] (NULL =
+ *   n_stride), K9 [S][9] f64 unscaled row-major -- all [dev].  0 <= S <= 65535 (larger batches: split them).
+ *   Outputs [dev]: P16_out [S][16], outlier_ratio_out [S], inliers_out [S] (the winner's count); may be NULL:
+ *   n_sel_out [S], hyp_used_out [S] (hypotheses the sequential rule evaluated), inlier_mask_out [S][n_stride] (1 =
+ *   selected point that is an inlier of the winner), hyp_pose_out [S][iterations][12] (R row-major | t; zeros for an
+ *   invalid hypothesis) and hyp_inliers_out [S][iterations] (0 for invalid); entries at h >= hyp_used are unspecified.
+ * workspace: [dev] 256-byte aligned, >= pnp_ransac_workspace_bytes(S, n_stride, iterations).
+ * epnp_batch_f64 (test hook): EPnP on B point sets, set b = rows offsets[b] .. offsets[b+1]-1 of xyz [N][3] f64 and
+ * uv [N][2] f64 pixels, intrinsics K9 [B][9] used as given; pose12_out [B][12], ok_out [B] int32 (0 = degenerate).
+ * ------------------------------------------------------------------------------------------ */
+size_t pnp_ransac_workspace_bytes(int S, int n_stride, int iterations);
+int pnp_ransac_batch_f32(const float* xyz, const int8_t* coarse_pred, const int32_t* fine_pred, const int32_t* n_pts,
+                         int n_stride, int S, const double* K9, double H, double W, double scale, int iterations,
+                         double reproj_err, double confidence, uint64_t seed, double* P16_out,
+                         double* outlier_ratio_out, int32_t* inliers_out, int32_t* n_sel_out, int32_t* hyp_used_out,
+                         uint8_t* inlier_mask_out, double* hyp_pose_out, int32_t* hyp_inliers_out, void* workspace,
+                         size_t workspace_bytes, dib_stream_t stream);
+int epnp_batch_f64(const double* xyz, const double* uv, const int32_t* offsets, int B, const double* K9,
+                   double* pose12_out, int32_t* ok_out, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

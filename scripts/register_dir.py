@@ -3,9 +3,11 @@
 
 Replaces `python evaluation/registration_lsq.py` + `registration_result_analysis.py` of the reference
 (registration_lsq.py:250-398, registration_result_analysis.py:13-47) for directories written by
-visualize_and_save_data.py:174-186.  Example:
+visualize_and_save_data.py:174-186, and, with --method pnp, `python evaluation/registration_pnp.py`
+(registration_pnp.py:151-259: grid classification + PnP-RANSAC, cost = outlier ratio).  Examples:
 
     python scripts/register_dir.py /data/kitti/save/run/data --H 160 --W 512 --out /data/kitti/save/run
+    python scripts/register_dir.py /data/kitti/save/run/data --H 160 --W 512 --method pnp --fine-scale 0.03125
 """
 import argparse
 import json
@@ -22,7 +24,14 @@ def main():
     ap.add_argument("data_dir")
     ap.add_argument("--H", type=float, required=True, help="image height (kitti 160, oxford 384, nuscenes 160)")
     ap.add_argument("--W", type=float, required=True, help="image width (kitti 512, oxford 640, nuscenes 320)")
-    ap.add_argument("--labels", default="coarse_prediction", choices=sorted(handoff.LABEL_ROWS))
+    ap.add_argument("--method", default="lsq", choices=("lsq", "pnp"),
+                    help="lsq: frustum classification + inverse camera projection (registration_lsq.py); "
+                         "pnp: grid classification + PnP-RANSAC (registration_pnp.py)")
+    ap.add_argument("--labels", default="coarse_prediction", choices=sorted(handoff.LABEL_ROWS),
+                    help="lsq only: the in/out-of-frustum row the solver reads")
+    ap.add_argument("--fine-scale", type=float, default=1 / 32.0,
+                    help="pnp only: fine grid resolution relative to the image (registration_pnp.py:163)")
+    ap.add_argument("--iterations", type=int, default=500, help="pnp only: RANSAC iterations (iterationsCount)")
     ap.add_argument("--enu2cam", action="store_true", help="nuScenes axis convention (registration_lsq.py:236-247)")
     ap.add_argument("--inits", type=int, default=60)
     ap.add_argument("--seed", type=int, default=0)
@@ -32,12 +41,20 @@ def main():
     ap.add_argument("--out", default=None, help="where to write P_pred_all_np.npy / P_gt_all_np.npy / cost_all_np.npy")
     args = ap.parse_args()
 
+    if args.method == "lsq" and args.labels.startswith("fine_"):
+        ap.error("--labels %s holds grid cell indices, not in/out-of-frustum labels; use --method pnp" % args.labels)
     names = handoff.list_records(args.data_dir)[::args.every]
-    res = handoff.register_directory(args.data_dir, args.H, args.W, which=args.labels, enu2cam=args.enu2cam,
-                                     n_inits=args.inits, seed=args.seed, is_2d=not args.is_3d, batch=args.batch,
-                                     names=names, out_dir=args.out)
+    if args.method == "pnp":
+        res = handoff.register_directory_pnp(args.data_dir, args.H, args.W, fine_scale=args.fine_scale,
+                                             iterations=args.iterations, seed=args.seed, enu2cam=args.enu2cam,
+                                             batch=args.batch, names=names, out_dir=args.out)
+    else:
+        res = handoff.register_directory(args.data_dir, args.H, args.W, which=args.labels, enu2cam=args.enu2cam,
+                                         n_inits=args.inits, seed=args.seed, is_2d=not args.is_3d, batch=args.batch,
+                                         names=names, out_dir=args.out)
     for i, n in enumerate(res["names"]):
-        print("%s - cost: %.1f, T: %.1f, R:%.1f" % (n, res["cost"][i], res["t_err"][i], res["r_err"][i]))
+        print(("%s - cost: %.2f, T: %.1f, R:%.1f" if args.method == "pnp" else "%s - cost: %.1f, T: %.1f, R:%.1f")
+              % (n, res["cost"][i], res["t_err"][i], res["r_err"][i]))
     s = res["summary"]
     print("RTE %.2f +- %.2f, RRE %.2f +- %.2f, success rate %.2f" % (s["rte_mean"], s["rte_sigma"], s["rre_mean"],
                                                                      s["rre_sigma"], s["success_rate"] * 100))

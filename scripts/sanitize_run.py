@@ -47,5 +47,16 @@ if which in ("all", "ops"):
     print("ball_query_xyz", point_ops.ball_query_xyz_forward(torch.from_numpy(pts).cuda(), torch.from_numpy(nodes).cuda(), 1.5, 12).sum().item())
     ca = point_ops.cluster_assign_forward(torch.from_numpy(pts).cuda(), torch.from_numpy(nodes).cuda(), 3)
     print("cluster_assign", ca["count"].sum().item(), ca["pc_decentered"].abs().sum().item())
+if which in ("all", "pnp"):
+    from deepi2p_b200 import pnp
+    fines = [syn.make_fine_labels(s, seed=i) for i, s in enumerate(smps)]
+    pts = [s["points"] for s in smps] + [smps[0]["points"][:, :40]]          # a ragged third frame
+    pred = [s["pred"] for s in smps] + [np.ones(40, np.int32)]
+    args = pnp.pack_frames(pts, pred, fines + [fines[0][:40]])
+    o = pnp.pnp_ransac_batch(*args, smps[0]["K"], smps[0]["H"], smps[0]["W"], iterations=150, return_all=True)
+    print("pnp_ransac", o["inliers"].cpu().tolist(), o["hyp_used"].cpu().tolist())
+    rng = np.random.default_rng(1)
+    print("epnp", pnp.epnp_batch([(rng.uniform(1, 9, (n_, 3)), rng.uniform(0, 16, (n_, 2))) for n_ in (5, 40)],
+                                 np.eye(3))[1].tolist())
 torch.cuda.synchronize()
 print("done")
