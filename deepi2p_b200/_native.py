@@ -21,6 +21,7 @@ EXPORTS = (
     "index_max_forward", "ball_query_forward", "ball_query_xyz_workspace_bytes", "ball_query_xyz_forward",
     "cluster_assign_workspace_bytes", "cluster_assign_forward",
     "pnp_ransac_workspace_bytes", "pnp_ransac_batch_f32", "epnp_batch_f64",
+    "icp_workspace_bytes", "icp_register_batch_f32", "icp_register_batch_counted_f32", "icp_build_index_f32",
 )
 
 
@@ -128,6 +129,16 @@ def load():
                                          vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
     lib.epnp_batch_f64.restype = i32
     lib.epnp_batch_f64.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp]
+    lib.icp_workspace_bytes.restype = sz
+    lib.icp_workspace_bytes.argtypes = [i32, i32, i32, i32]
+    lib.icp_register_batch_f32.restype = i32
+    lib.icp_register_batch_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, i32, f64, i32, f64, f64, i32,
+                                           vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.icp_register_batch_counted_f32.restype = i32
+    lib.icp_register_batch_counted_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, i32, f64, i32, f64, f64, i32,
+                                                   vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.icp_build_index_f32.restype = i32
+    lib.icp_build_index_f32.argtypes = [vp, vp, i32, i32, vp, sz, vp]
     _lib = lib
     return lib
 

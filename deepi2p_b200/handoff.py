@@ -161,6 +161,67 @@ def register_directory_pnp(data_dir, H, W, fine_scale=1 / 32.0, iterations=500, 
                 summary=summarize(t_err, r_err, cost, ok))
 
 
+def get_p_diff(P_pred, P_gt):
+    """get_P_diff of evaluation/icp/registration_icp.py:57-65 with the fold of :224-225, on the host: P_diff =
+    np.linalg.inv(P_pred) P_gt, t = |P_diff[:3,3]|, r = sum |euler 'xzy'| in degrees (scipy), r > 180 -> 360 - r.
+    The ICP poses carry the 2-D forcing, which is not a rigid transform, so the rigid inverse of pose_error_batch
+    does not apply.  Returns (t_err [S], r_err [S])."""
+    from scipy.spatial.transform import Rotation
+    P_pred = np.asarray(P_pred, dtype=np.float64).reshape(-1, 4, 4)
+    P_gt = np.asarray(P_gt, dtype=np.float64).reshape(-1, 4, 4)
+    t_err = np.zeros(len(P_pred))
+    r_err = np.zeros(len(P_pred))
+    for s in range(len(P_pred)):
+        D = np.dot(np.linalg.inv(P_pred[s]), P_gt[s])
+        t_err[s] = np.linalg.norm(D[0:3, 3])
+        r = np.sum(np.abs(Rotation.from_matrix(D[0:3, 0:3]).as_euler("xzy", degrees=True)))
+        r_err[s] = 360 - r if r > 180 else r
+    return t_err, r_err
+
+
+def register_directory_icp(data_dir, monodepth_dir, H, W, n_inits=60, seed=0, max_corr_dist=1.0, max_iteration=30,
+                           enu2cam=False, batch=64, names=None, device="cuda", out_dir=None, t_thresh=2.0,
+                           r_thresh=5.0):
+    """The __main__ of evaluation/icp/registration_icp.py:165-245 as one function: every frame of a legacy directory
+    and its <monodepth_dir>/<id>_pc.npy depth cloud, scale-calibrated with the ground truth (icp.calibrate_scale),
+    through icp.icp_register_batch (the GPU path, random_inits(S, n_inits, seed + first frame of the batch)), errors
+    by get_p_diff, and the P_pred_all_np / P_gt_all_np / cost_all_np files (cost = fitness, :241-243)."""
+    import torch
+    from . import icp
+
+    if names is None:
+        names = list_records(data_dir)
+    P_pred = np.zeros((len(names), 4, 4))
+    P_gt = np.zeros((len(names), 4, 4))
+    cost = np.zeros((len(names),))
+    for a in range(0, len(names), batch):
+        srcs, tgts = [], []
+        for s, name in enumerate(names[a:a + batch]):
+            pc, _, K, P = load_record(data_dir, name, enu2cam=enu2cam)
+            depth = np.load(os.path.join(monodepth_dir, name + "_pc.npy")).astype(np.float64)
+            if depth.ndim != 2 or depth.shape[0] != 3:
+                raise ValueError("%s_pc.npy: expected [3, N], got %s" % (name, depth.shape))
+            depth = depth * icp.calibrate_scale(pc, P, K, H, W, depth)
+            srcs.append(pc)
+            tgts.append(depth)
+            P_gt[a + s] = P
+        src, n = icp.pack_clouds(srcs, device)
+        tgt, m = icp.pack_clouds(tgts, device)
+        init = torch.from_numpy(icp.random_inits(len(srcs), n_inits, seed + a)).to(src.device)
+        out = icp.icp_register_batch(src, n, tgt, m, init, max_corr_dist=max_corr_dist, max_iteration=max_iteration)
+        P_pred[a:a + batch] = out["P"].cpu().numpy()
+        cost[a:a + batch] = out["fitness"].cpu().numpy()
+    t_err, r_err = get_p_diff(P_pred, P_gt)
+    ok = ((t_err < t_thresh) & (r_err < r_thresh)).astype(np.int32)
+    if out_dir is not None:
+        os.makedirs(out_dir, exist_ok=True)
+        np.save(os.path.join(out_dir, "P_pred_all_np.npy"), P_pred)
+        np.save(os.path.join(out_dir, "P_gt_all_np.npy"), P_gt)
+        np.save(os.path.join(out_dir, "cost_all_np.npy"), cost)
+    return dict(names=names, P_pred=P_pred, P_gt=P_gt, cost=cost, t_err=t_err, r_err=r_err, success=ok,
+                summary=summarize(t_err, r_err, cost, ok))
+
+
 def summarize(t_err, r_err, cost, ok):
     """registration_result_analysis.py:19-47 on the per-frame errors: frames with cost <= 1e-6 are dropped,
     RTE/RRE mean and sigma, success rate over the kept frames."""

@@ -81,6 +81,106 @@ def make_inits(seed, init_y_angle, n_inits=60, ry_sigma=10.0 * math.pi / 180.0, 
     return ry, t
 
 
+def _ray_boxes(o, d, lo, hi):
+    """Nearest positive hit distance of rays o + t d (d [R,3]) with axis-aligned boxes (lo, hi [B,3]); inf = none."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        inv = 1.0 / d
+        best = np.full(d.shape[0], np.inf)
+        for b in range(lo.shape[0]):
+            t1 = (lo[b] - o) * inv
+            t2 = (hi[b] - o) * inv
+            tmin = np.nanmax(np.minimum(t1, t2), axis=1)
+            tmax = np.nanmin(np.maximum(t1, t2), axis=1)
+            hit = (tmax >= np.maximum(tmin, 0.0)) & (tmin > 0.0)
+            best = np.where(hit & (tmin < best), tmin, best)
+    return best
+
+
+def make_icp_frame(seed, shape="oxford", n_rings=32, n_azimuth=640, ground=1.7, max_depth=80.0):
+    """One seeded monodepth + ICP frame (the inputs of evaluation/icp/registration_icp.py:196-218), ray-cast from a
+    scene of a ground plane (y = `ground`, y points down as in make_sample), a closed ring of 24 buildings 27-37 m from
+    the LiDAR and 20 small boxes inside it:
+
+      src  [3, n_rings * n_azimuth] float32  a 360 deg LiDAR pattern (elevations 15 deg up to 10 deg down)
+      tgt  [3, H * W] float64  the depth map of the ground-truth camera with an unknown global scale and smooth
+           multiplicative noise, back-projected through K^-1 in save_depth_map.py:84-102's order (index y * W + x)
+
+    Returns dict(src, tgt, depth [H,W], K, H, W, P_gt (LiDAR -> camera, Ry and (tx, 0, tz) like make_sample), scale
+    (the factor the depth map was multiplied by))."""
+    cfg = KITTI if shape == "kitti" else OXFORD
+    H, W, K = cfg["H"], cfg["W"], cfg["K"].copy()
+    rng = np.random.default_rng(seed + 0x1C9)
+    ry = rng.uniform(-math.pi, math.pi)
+    t = np.array([rng.uniform(-3, 3), 0.0, rng.uniform(-6, 6)])
+    P = np.eye(4)
+    P[:3, :3] = ry_matrix(ry)
+    P[:3, 3] = t
+    cam = -P[:3, :3].T @ t                      # camera centre in the LiDAR frame
+    lo, hi = [], []
+    for k in range(24):                         # buildings: 10 m squares on a 32 m circle overlap, so the ring is closed
+        a = 2 * math.pi * k / 24 + rng.uniform(-0.05, 0.05)
+        r = 32.0 + rng.uniform(-2, 2)
+        h = rng.uniform(8.0, 15.0)
+        c = np.array([r * math.sin(a), 0.0, r * math.cos(a)])
+        lo.append([c[0] - 5, ground - h, c[2] - 5])
+        hi.append([c[0] + 5, ground + 1.0, c[2] + 5])
+    while len(lo) < 44:                         # cars / kiosks, kept clear of the LiDAR and the camera
+        half = rng.uniform(0.75, 2.25, 2)
+        h = rng.uniform(1.0, 2.5)
+        a, r = rng.uniform(-math.pi, math.pi), rng.uniform(5.0, 22.0)
+        c = np.array([r * math.sin(a), 0.0, r * math.cos(a)])
+        clear = 3.0 + float(np.hypot(*half))
+        if np.hypot(c[0], c[2]) < clear or np.hypot(c[0] - cam[0], c[2] - cam[2]) < clear:
+            continue
+        lo.append([c[0] - half[0], ground - h, c[2] - half[1]])
+        hi.append([c[0] + half[0], ground + 1.0, c[2] + half[1]])
+    lo, hi = np.array(lo), np.array(hi)
+
+    def cast(o, d):
+        tb = _ray_boxes(o, d, lo, hi)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            tg = np.where(d[:, 1] > 1e-9, (ground - o[1]) / d[:, 1], np.inf)
+        return np.minimum(tb, np.where(tg > 0, tg, np.inf))
+
+    el = np.deg2rad(np.linspace(-15.0, 10.0, n_rings))
+    az = np.linspace(-math.pi, math.pi, n_azimuth, endpoint=False)
+    e, a = np.meshgrid(el, az, indexing="ij")
+    d = np.stack([np.cos(e) * np.sin(a), np.sin(e), np.cos(e) * np.cos(a)], -1).reshape(-1, 3)
+    rl = cast(np.zeros(3), d)
+    rl = np.where(np.isfinite(rl), rl, max_depth)
+    src = (d * rl[:, None]).T.astype(np.float32)
+
+    xv, yv = np.meshgrid(np.arange(W, dtype=np.float64), np.arange(H, dtype=np.float64))
+    pix = np.stack([xv, yv, np.ones_like(xv)], -1).reshape(-1, 3)
+    dcam = pix @ np.linalg.inv(K).T                            # z = 1: the hit distance is the depth
+    depth = cast(cam, dcam @ P[:3, :3])                        # rows of dcam @ R = R^T dcam
+    depth = np.minimum(np.where(np.isfinite(depth), depth, max_depth), max_depth).reshape(H, W)
+    scale = rng.uniform(0.5, 2.0)
+    ph = rng.uniform(0, 2 * math.pi, 4)
+    noise = 1.0 + 0.02 * (np.sin(xv / W * 2 * math.pi + ph[0]) * np.cos(yv / H * math.pi + ph[1])
+                          + 0.5 * np.sin(xv / W * 5 * math.pi + ph[2] + yv / H * 3 * math.pi) * math.cos(ph[3]))
+    depth = depth * noise * scale
+    tgt = np.linalg.inv(K) @ (pix * depth.reshape(-1, 1)).T
+    return dict(src=src, tgt=tgt, depth=depth, K=K, H=H, W=W, P_gt=P, scale=scale)
+
+
+def write_icp_handoff(data_dir, monodepth_dir, seeds, shape="oxford"):
+    """make_icp_frame frames as a hand-off directory (<id>_pc_label.npy / _K.npy / _P.npy, labels = the GT inside
+    mask) plus the <monodepth_dir>/<id>_pc.npy depth clouds registration_icp.py:204 reads.  Returns the frames by id."""
+    import os
+    from . import handoff
+    os.makedirs(monodepth_dir, exist_ok=True)
+    frames = {}
+    for i, s in enumerate(seeds):
+        f = make_icp_frame(s, shape)
+        name = "%06d_%02d" % (i, 0)
+        lab = inside_mask(f["src"], f["P_gt"], f["K"], f["H"], f["W"]).astype(np.int32)
+        handoff.save_record(data_dir, name, f["src"], lab, lab, lab, lab, f["K"], f["P_gt"][:3])
+        np.save(os.path.join(monodepth_dir, name + "_pc.npy"), f["tgt"])
+        frames[name] = f
+    return frames
+
+
 def make_index_max_inputs(seed, B=64, C=64, N=16384, K=64):
     rng = np.random.default_rng(seed)
     data = rng.standard_normal((B, C, N), dtype=np.float32)

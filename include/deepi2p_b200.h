@@ -270,6 +270,48 @@ int pnp_ransac_batch_f32(const float* xyz, const int8_t* coarse_pred, const int3
 int epnp_batch_f64(const double* xyz, const double* uv, const int32_t* offsets, int B, const double* K9,
                    double* pose12_out, int32_t* ok_out, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Multi-start point-to-point ICP of a LiDAR cloud against a monocular-depth cloud (evaluation/icp/registration_icp.py:
+ * 115-162: Open3D registration_icp with TransformationEstimationPointToPoint, default convergence criteria, the best
+ * of I random inits), batched over S frames.  DESIGN.md "ICP" states the contract.  One problem = (frame s, init i):
+ *   pass(T): q = T p for every source point (fp64, no FMA); its exact nearest target point (d2 = (dx*dx + dy*dy) +
+ *   dz*dz, ties -> lowest target index) is a correspondence iff d2 < max_corr_dist^2; fitness = n_corr / n_pts,
+ *   rmse = sqrt(sum d2 / n_corr) (0 without correspondences).  result = pass(init); then up to max_iteration times:
+ *   T = umeyama(correspondences) * T (rigid, no scaling; identity without correspondences), result = pass(T), stop
+ *   when |d fitness| < relative_fitness and |d rmse| < relative_rmse.
+ * Per frame: the first init whose fitness is strictly above the best so far (starting at 0.001) wins; none -> P = I,
+ * fitness 0.001, best -1.  force_2d != 0 sets P[0][1] = P[1][0] = P[1][2] = P[2][1] = 0, P[1][1] = 1 on the winner
+ * (registration_icp.py:127-133; not re-scored, the 3x3 block is then not orthonormal).
+ *   src [S][3][n_stride] f32, n_pts [S] i32 (NULL = n_stride), tgt [S][3][m_stride] f32, m_pts [S] (NULL = m_stride),
+ *   init16 [S][I][16] f64 row-major 4x4 -- all [dev].  Strides are multiples of 16; 0 <= S <= 65535,
+ *   1 <= I <= 4096, S * m_stride < 2^31; max_corr_dist > 0; max_iteration >= 0.
+ *   Outputs [dev]: P16_out [S][16], fitness_out [S]; may be NULL: best_out [S] (-1 = none), T_all [S][I][16],
+ *   fitness_all [S][I], rmse_all [S][I], stats_all [S][I][2] = (update steps, n_corr of the last pass).
+ * workspace: [dev] 256-byte aligned, >= icp_workspace_bytes(S, I, n_stride, m_stride) (the per-frame nearest-neighbour
+ *   index over the target, about 60 B per target point, and the per-problem results).
+ *   The target index holds up to 2^27 leaves of 16 points; every m_stride the S * m_stride < 2^31 rule admits fits.
+ * icp_register_batch_counted_f32 (measurement): the same call, which also adds (nearest-neighbour queries, point
+ *   distance evaluations) of its problems to counters [dev] (two unsigned 64-bit words, not cleared by the call).
+ * icp_build_index_f32 (measurement): only the per-frame index build of a call (target layout as above), into a
+ *   workspace of >= icp_workspace_bytes(S, 1, 16, m_stride) bytes; it computes nothing a caller can read.
+ * ------------------------------------------------------------------------------------------ */
+size_t icp_workspace_bytes(int S, int I, int n_stride, int m_stride);
+int icp_register_batch_f32(const float* src, const int32_t* n_pts, int n_stride, const float* tgt,
+                           const int32_t* m_pts, int m_stride, int S, const double* init16, int I,
+                           double max_corr_dist, int max_iteration, double relative_fitness, double relative_rmse,
+                           int force_2d, double* P16_out, double* fitness_out, int32_t* best_out, double* T_all,
+                           double* fitness_all, double* rmse_all, int32_t* stats_all, void* workspace,
+                           size_t workspace_bytes, dib_stream_t stream);
+int icp_register_batch_counted_f32(const float* src, const int32_t* n_pts, int n_stride, const float* tgt,
+                                   const int32_t* m_pts, int m_stride, int S, const double* init16, int I,
+                                   double max_corr_dist, int max_iteration, double relative_fitness,
+                                   double relative_rmse, int force_2d, double* P16_out, double* fitness_out,
+                                   int32_t* best_out, double* T_all, double* fitness_all, double* rmse_all,
+                                   int32_t* stats_all, unsigned long long* counters, void* workspace,
+                                   size_t workspace_bytes, dib_stream_t stream);
+int icp_build_index_f32(const float* tgt, const int32_t* m_pts, int m_stride, int S, void* workspace,
+                        size_t workspace_bytes, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -58,5 +58,16 @@ if which in ("all", "pnp"):
     rng = np.random.default_rng(1)
     print("epnp", pnp.epnp_batch([(rng.uniform(1, 9, (n_, 3)), rng.uniform(0, 16, (n_, 2))) for n_ in (5, 40)],
                                  np.eye(3))[1].tolist())
+if which in ("all", "icp"):
+    from deepi2p_b200 import icp
+    fr = syn.make_icp_frame(3, "kitti")
+    srcs = [fr["src"][:, ::16], fr["src"][:, ::16][:, :300], fr["src"][:, :0]]      # ragged, the last one empty
+    tgts = [(fr["tgt"][:, ::20] / fr["scale"]).astype(np.float32), (fr["tgt"][:, ::37] / fr["scale"]).astype(np.float32),
+            (fr["tgt"][:, :50] / fr["scale"]).astype(np.float32)]
+    src, n_src = icp.pack_clouds(srcs)
+    tgt, m_tgt = icp.pack_clouds(tgts)
+    init = torch.from_numpy(np.stack([np.concatenate([fr["P_gt"][None], icp.random_inits(1, 2, s)[0]]) for s in range(3)])).cuda()
+    o = icp.icp_register_batch(src, n_src, tgt, m_tgt, init, max_iteration=8, return_all=True)
+    print("icp", o["best"].cpu().tolist(), o["stats"][..., 0].cpu().tolist())
 torch.cuda.synchronize()
 print("done")
