@@ -22,6 +22,8 @@ EXPORTS = (
     "cluster_assign_workspace_bytes", "cluster_assign_forward",
     "pnp_ransac_workspace_bytes", "pnp_ransac_batch_f32", "epnp_batch_f64",
     "icp_workspace_bytes", "icp_register_batch_f32", "icp_register_batch_counted_f32", "icp_build_index_f32",
+    "voxel_downsample_workspace_bytes", "voxel_downsample_batch_f32", "estimate_normals_workspace_bytes",
+    "estimate_normals_batch_f32", "nearest_batch_f32",
 )
 
 
@@ -139,6 +141,16 @@ def load():
                                                    vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
     lib.icp_build_index_f32.restype = i32
     lib.icp_build_index_f32.argtypes = [vp, vp, i32, i32, vp, sz, vp]
+    lib.voxel_downsample_workspace_bytes.restype = sz
+    lib.voxel_downsample_workspace_bytes.argtypes = [i32, i32, i32]
+    lib.voxel_downsample_batch_f32.restype = i32
+    lib.voxel_downsample_batch_f32.argtypes = [vp, vp, i32, i32, vp, i32, f64, vp, vp, vp, vp, sz, vp]
+    lib.estimate_normals_workspace_bytes.restype = sz
+    lib.estimate_normals_workspace_bytes.argtypes = [i32, i32]
+    lib.estimate_normals_batch_f32.restype = i32
+    lib.estimate_normals_batch_f32.argtypes = [vp, vp, i32, i32, f64, i32, vp, vp, vp, vp, sz, vp]
+    lib.nearest_batch_f32.restype = i32
+    lib.nearest_batch_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp, sz, vp]
     _lib = lib
     return lib
 

@@ -26,52 +26,21 @@
 
 #include <cub/device/device_radix_sort.cuh>
 
-#include "common.cuh"
+#include "morton_index.cuh"
 
 namespace dib {
 namespace icp {
 
 constexpr int kThreads = 256;         // threads of one ICP problem (8 warps)
 constexpr int kWarps = kThreads / 32;
-constexpr int kLeaf = 16;             // sorted points per leaf box
-constexpr int kLeafShift = 4;
-constexpr int kMaxLevels = 28;
-constexpr int kStack = 32;
 constexpr int kSweeps = 8;            // one-sided Jacobi sweeps of the 3x3 SVD
 constexpr int kMoments = 16;          // sum d2, sum dq[3], sum dt[3], sum dt dq^T [9]
-// A descent pushes at most two children per popped node and pops one, so the stack never holds more than one entry
-// per level plus the root's.
-static_assert(kStack > kMaxLevels + 1, "the descent stack must hold one entry per level");
-static_assert(kMaxLevels <= 32, "a stack entry keeps the level in 5 bits");
 
-struct Levels {
-  int n;                    // levels of a full frame (m = m_stride)
-  int off[kMaxLevels];      // first node of level l within a frame's node array
-  int per_frame;            // nodes per frame
-};
-
-struct Work {
-  float* bbox;              // [S][6]
-  unsigned long long *key0, *key1;
-  int32_t *val0, *val1;
-  float4* pts;              // [S][m_stride]
-  float4 *lo, *hi;          // [S][per_frame]
+struct Work : Index {       // the target index and the per-problem results
   double* T;                // [S][I][16]
   double* fit;              // [S][I]
   double* rmse;             // [S][I]
-  void* sort_tmp;
-  size_t sort_tmp_bytes;
 };
-
-__host__ __device__ inline int level_count(int m, int l) {
-  return (int)(((long long)m + ((long long)kLeaf << l) - 1) >> (kLeafShift + l));
-}
-
-__device__ __forceinline__ int clamp_n(const int32_t* n, int s, int stride) {
-  if (!n) return stride;
-  const int v = n[s];
-  return v < 0 ? 0 : (v > stride ? stride : v);
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Index build.
@@ -182,63 +151,6 @@ __global__ void level_kernel(const int32_t* __restrict__ m_pts, int m_stride, in
   }
   lo[base + L.off[l] + k] = a;
   hi[base + L.off[l] + k] = b;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Exact nearest neighbour.  A box's lower bound is formed from its float corners with the same operations as d2, so
-// it never exceeds the d2 of a point inside it (rounding is monotone); a box is skipped only when its bound is
-// strictly above the best d2, so an equally distant point of lower index is still found.
-
-__device__ __forceinline__ double box_lb(const float4& lo, const float4& hi, double qx, double qy, double qz) {
-  const double dx = fmax(fmax((double)lo.x - qx, qx - (double)hi.x), 0.0);
-  const double dy = fmax(fmax((double)lo.y - qy, qy - (double)hi.y), 0.0);
-  const double dz = fmax(fmax((double)lo.z - qz, qz - (double)hi.z), 0.0);
-  return (dx * dx + dy * dy) + dz * dz;
-}
-
-struct Hit {
-  double d2;
-  int j;
-  float x, y, z;
-};
-
-__device__ __forceinline__ void nearest(const float4* __restrict__ pts, const float4* __restrict__ lo,
-                                        const float4* __restrict__ hi, const Levels& L, int m, int root, double qx,
-                                        double qy, double qz, Hit& h, unsigned long long& evals) {
-  h.j = INT_MAX;            // h.d2 holds the caller's bound (r^2): nothing at or beyond it can be a correspondence
-  if (m <= 0) return;
-  unsigned st_node[kStack];   // (node << 5) | level: node < 2^27 and level < 32 for every admitted m_stride
-  double st_lb[kStack];
-  int sp = 0;
-  st_node[sp] = (unsigned)root;
-  st_lb[sp++] = box_lb(lo[L.off[root]], hi[L.off[root]], qx, qy, qz);
-  while (sp > 0) {
-    --sp;
-    if (st_lb[sp] > h.d2) continue;
-    const int l = (int)(st_node[sp] & 31u), k = (int)(st_node[sp] >> 5);
-    if (l == 0) {
-      const int e = k * kLeaf + min(kLeaf, m - k * kLeaf);
-      for (int i = k * kLeaf; i < e; ++i) {
-        const float4 p = pts[i];
-        const double dx = qx - (double)p.x, dy = qy - (double)p.y, dz = qz - (double)p.z;
-        const double d2 = (dx * dx + dy * dy) + dz * dz;
-        const int j = __float_as_int(p.w);
-        ++evals;
-        if (d2 < h.d2 || (d2 == h.d2 && j < h.j)) {
-          h.d2 = d2; h.j = j; h.x = p.x; h.y = p.y; h.z = p.z;
-        }
-      }
-      continue;
-    }
-    const int c0 = 2 * k, nc = level_count(m, l - 1), o = L.off[l - 1];
-    const double lb0 = box_lb(lo[o + c0], hi[o + c0], qx, qy, qz);
-    const double lb1 = c0 + 1 < nc ? box_lb(lo[o + c0 + 1], hi[o + c0 + 1], qx, qy, qz) : DBL_MAX;
-    const bool first1 = lb1 < lb0;           // nearer child on top of the stack
-    const int cn = first1 ? c0 + 1 : c0, cf = first1 ? c0 : c0 + 1;
-    const double ln = first1 ? lb1 : lb0, lf = first1 ? lb0 : lb1;
-    if (lf <= h.d2) { st_node[sp] = ((unsigned)cf << 5) | (unsigned)(l - 1); st_lb[sp++] = lf; }
-    if (ln <= h.d2) { st_node[sp] = ((unsigned)cn << 5) | (unsigned)(l - 1); st_lb[sp++] = ln; }
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -493,23 +405,30 @@ Levels make_levels(int m_stride) {
 // hundred bytes per 3840-item tile; 8 B per item plus 4 MiB is far above it at every batch size.
 inline size_t sort_reserve(size_t N) { return 8 * N + ((size_t)4 << 20); }
 
-// Workspace carve-up; returns the bytes needed (base may be NULL).
-size_t carve(char* base, int S, int I, int m_stride, Work* wk) {
+size_t carve_index(char* base, size_t off, int S, int m_stride, Index* ix) {
   const size_t N = (size_t)S * m_stride;
   const Levels L = make_levels(m_stride);
-  size_t off = 0;
   auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += align256(bytes); return p; };
-  Work w;
+  Index w;
   w.bbox = (float*)take((size_t)S * 6 * 4);
   w.key0 = (unsigned long long*)take(N * 8); w.key1 = (unsigned long long*)take(N * 8);
   w.val0 = (int32_t*)take(N * 4); w.val1 = (int32_t*)take(N * 4);
   w.pts = (float4*)take(N * 16);
   w.lo = (float4*)take((size_t)S * L.per_frame * 16); w.hi = (float4*)take((size_t)S * L.per_frame * 16);
+  w.sort_tmp_bytes = sort_reserve(N);
+  w.sort_tmp = take(w.sort_tmp_bytes);
+  if (ix) *ix = w;
+  return off;
+}
+
+// Workspace carve-up; returns the bytes needed (base may be NULL).
+size_t carve(char* base, int S, int I, int m_stride, Work* wk) {
+  Work w;
+  size_t off = carve_index(base, 0, S, m_stride, &w);
+  auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += align256(bytes); return p; };
   w.T = (double*)take((size_t)S * I * 16 * 8);
   w.fit = (double*)take((size_t)S * I * 8);
   w.rmse = (double*)take((size_t)S * I * 8);
-  w.sort_tmp_bytes = sort_reserve(N);
-  w.sort_tmp = take(w.sort_tmp_bytes);
   if (wk) *wk = w;
   return off;
 }
@@ -531,8 +450,11 @@ int check_index_args(const float* tgt, int m_stride, int S, int I, void* workspa
   return DIB_OK;
 }
 
-// The per-frame index: bbox, Morton keys, radix sort, gather, one launch per tree level.
-int build_index(const float* tgt, const int32_t* m_pts, int m_stride, int S, const Levels& L, Work& wk,
+void cloud_bbox(const float* X, const int32_t* n_pts, int stride, int S, float* bbox, cudaStream_t st) {
+  bbox_kernel<<<S, 256, 0, st>>>(X, n_pts, stride, bbox);
+}
+
+int build_index(const float* tgt, const int32_t* m_pts, int m_stride, int S, const Levels& L, Index& wk,
                 cudaStream_t st) {
   const long long N = (long long)S * m_stride;
   const int nb = (int)((N + 255) / 256);
@@ -546,7 +468,7 @@ int build_index(const float* tgt, const int32_t* m_pts, int m_stride, int S, con
   size_t tmp = 0;
   DIB_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, vals, (int)N, 0, 48 + fb, st));
   if (tmp > wk.sort_tmp_bytes) {
-    set_error("icp: the radix sort needs %zu bytes of scratch, %zu reserved", tmp, wk.sort_tmp_bytes);
+    set_error("index: the radix sort needs %zu bytes of scratch, %zu reserved", tmp, wk.sort_tmp_bytes);
     return DIB_ENOMEM;
   }
   DIB_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(wk.sort_tmp, tmp, keys, vals, (int)N, 0, 48 + fb, st));

@@ -164,6 +164,42 @@ def make_icp_frame(seed, shape="oxford", n_rings=32, n_azimuth=640, ground=1.7, 
     return dict(src=src, tgt=tgt, depth=depth, K=K, H=H, W=W, P_gt=P, scale=scale)
 
 
+def make_lidar_scan(seed, n_rings=64, n_azimuth=2048, noise=0.01, ground=-1.73, max_range=80.0):
+    """One seeded HDL-64-shaped scan in Velodyne axes (x forward, y left, z up): n_rings elevations from +2 to -24.8
+    deg times n_azimuth azimuths, ray-cast against a ground plane z = `ground` and 30 boxes (buildings, cars) 4-40 m
+    away; rays that hit nothing return at max_range.  Ranges get N(0, noise) errors (noise = 0: ground points lie
+    exactly on the plane).  Returns dict(xyz [3, n_rings * n_azimuth] float32, intensity [n] float32 in [0, 1),
+    ground [n] bool)."""
+    rng = np.random.default_rng(seed + 0x5CA)
+    lo, hi = [], []
+    for _ in range(30):
+        a, r = rng.uniform(-math.pi, math.pi), rng.uniform(4.0, 40.0)
+        half = rng.uniform(0.8, 6.0, 2)
+        h = rng.uniform(1.2, 12.0)
+        c = np.array([r * math.cos(a), r * math.sin(a)])
+        if np.hypot(*c) < 2.0 + float(np.hypot(*half)):
+            continue
+        lo.append([c[0] - half[0], c[1] - half[1], ground - 1.0])
+        hi.append([c[0] + half[0], c[1] + half[1], ground + h])
+    lo, hi = np.array(lo), np.array(hi)
+    el = np.deg2rad(np.linspace(2.0, -24.8, n_rings))
+    az = np.linspace(-math.pi, math.pi, n_azimuth, endpoint=False)
+    e, a = np.meshgrid(el, az, indexing="ij")
+    d = np.stack([np.cos(e) * np.cos(a), np.cos(e) * np.sin(a), np.sin(e)], -1).reshape(-1, 3)
+    tb = _ray_boxes(np.zeros(3), d, lo, hi)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        tg = np.where(d[:, 2] < -1e-9, ground / d[:, 2], np.inf)
+    on_ground = tg < tb
+    t = np.minimum(np.minimum(tb, tg), max_range)
+    on_ground &= t < max_range
+    t = t + (rng.normal(0.0, noise, t.shape) if noise > 0 else 0.0)
+    xyz = d * t[:, None]
+    if noise == 0:
+        xyz[on_ground, 2] = ground
+    inten = rng.random(t.shape[0], dtype=np.float32)
+    return dict(xyz=xyz.T.astype(np.float32), intensity=inten, ground=on_ground)
+
+
 def write_icp_handoff(data_dir, monodepth_dir, seeds, shape="oxford"):
     """make_icp_frame frames as a hand-off directory (<id>_pc_label.npy / _K.npy / _P.npy, labels = the GT inside
     mask) plus the <monodepth_dir>/<id>_pc.npy depth clouds registration_icp.py:204 reads.  Returns the frames by id."""

@@ -312,6 +312,44 @@ int icp_register_batch_counted_f32(const float* src, const int32_t* n_pts, int n
 int icp_build_index_f32(const float* tgt, const int32_t* m_pts, int m_stride, int S, void* workspace,
                         size_t workspace_bytes, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * LiDAR scan preparation (data/kitti/kitti_pc_bin_to_npy_with_downsample_sn.py:48-74 and the loaders'
+ * downsample_with_intensity_sn / downsample_with_reflectance: Open3D voxel_down_sample, estimate_normals with
+ * KDTreeSearchParamHybrid, orient_normals_to_align_with_direction, and the 1-NN intensity transfer), batched over S
+ * clouds.  DESIGN.md "Scan preparation" states the contract.  All arithmetic is fp64 without FMA.
+ * Common rules: [dev] pointers, strides are multiples of 16, 0 <= S <= 65535, S * stride < 2^31, coordinates finite;
+ * count arrays (n_pts, m_pts, q_pts) may be NULL (= the stride); entries past a cloud's count are not written.
+ *
+ * voxel_downsample_batch_f32: xyz [S][3][n_stride] f32, optional attr [S][C][n_stride] f64 (0 <= C <= 64; NULL when
+ *   C = 0).  Per cloud: min_bound = min(p) - 0.5 v, voxel = floor((p - min_bound) / v); per occupied voxel, in ascending
+ *   (ix, iy, iz) order, the mean of its points and attributes (sums in ascending point index, then / count) into
+ *   xyz_out [S][3][n_stride] f64, attr_out [S][C][n_stride] f64, and the voxel count into m_pts_out [S] i32.
+ *   Returns DIB_EINVAL when a cloud spans 2^21 or more voxels along an axis.  The call reads the clouds' boxes back
+ *   to the host, so it waits for the work queued on the stream before it.
+ *   workspace >= voxel_downsample_workspace_bytes(S, n_stride, C), 256-byte aligned (about 44 B per point).
+ * estimate_normals_batch_f32: xyz [S][3][m_stride] f32.  Per point i: the min(max_nn, c) nearest points of the cloud
+ *   with d2 < radius^2 (itself included, ties -> lower index; 1 <= max_nn <= 64); fewer than 3 -> (0, 0, 1); else the
+ *   unit eigenvector of the smallest eigenvalue of the covariance about p_i (zero covariance -> 0); then a zero normal
+ *   becomes orient3 [host, 3 f64] and n . orient3 < 0 flips n.  normals_out [S][3][m_stride] f64; count_out
+ *   [S][m_stride] i32 (may be NULL) = neighbours used.
+ *   workspace >= estimate_normals_workspace_bytes(S, m_stride), 256-byte aligned (the Morton index of icp.cu).
+ * nearest_batch_f32: for each query q [S][3][q_stride] f64 (q_pts [S]), the index of the nearest point of xyz
+ *   [S][3][m_stride] f32 (d2 as above, ties -> lowest index; -1 for an empty cloud or d2 >= DBL_MAX / 2) into idx_out
+ *   [S][q_stride] i32.
+ *   workspace >= estimate_normals_workspace_bytes(S, m_stride).
+ * ------------------------------------------------------------------------------------------ */
+size_t voxel_downsample_workspace_bytes(int S, int n_stride, int C);
+int voxel_downsample_batch_f32(const float* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
+                               double voxel_size, double* xyz_out, double* attr_out, int32_t* m_pts_out,
+                               void* workspace, size_t workspace_bytes, dib_stream_t stream);
+size_t estimate_normals_workspace_bytes(int S, int m_stride);
+int estimate_normals_batch_f32(const float* xyz, const int32_t* m_pts, int m_stride, int S, double radius, int max_nn,
+                               const double* orient3, double* normals_out, int32_t* count_out, void* workspace,
+                               size_t workspace_bytes, dib_stream_t stream);
+int nearest_batch_f32(const double* q, const int32_t* q_pts, int q_stride, const float* xyz, const int32_t* m_pts,
+                      int m_stride, int S, int32_t* idx_out, void* workspace, size_t workspace_bytes,
+                      dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
