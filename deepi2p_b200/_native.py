@@ -24,6 +24,9 @@ EXPORTS = (
     "icp_workspace_bytes", "icp_register_batch_f32", "icp_register_batch_counted_f32", "icp_build_index_f32",
     "voxel_downsample_workspace_bytes", "voxel_downsample_batch_f32", "estimate_normals_workspace_bytes",
     "estimate_normals_batch_f32", "nearest_batch_f32",
+    "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32", "assemble_resample_workspace_bytes",
+    "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
+    "fps_batch_f64",
 )
 
 
@@ -151,6 +154,23 @@ def load():
     lib.estimate_normals_batch_f32.argtypes = [vp, vp, i32, i32, f64, i32, vp, vp, vp, vp, sz, vp]
     lib.nearest_batch_f32.restype = i32
     lib.nearest_batch_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp, sz, vp]
+    lib.assemble_accumulate_workspace_bytes.restype = sz
+    lib.assemble_accumulate_workspace_bytes.argtypes = [i32, i32, i32]
+    lib.assemble_accumulate_f32.restype = i32
+    lib.assemble_accumulate_f32.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp, vp, i32, vp, vp, sz,
+                                            vp]
+    lib.assemble_resample_workspace_bytes.restype = sz
+    lib.assemble_resample_workspace_bytes.argtypes = [i32, i32]
+    lib.assemble_resample_f32.restype = i32
+    lib.assemble_resample_f32.argtypes = [vp, vp, vp, vp, i32, i32, i32, _c.c_uint64, vp, f64, f64, i32, vp, vp, vp,
+                                          vp, vp, sz, vp]
+    lib.assemble_candidates_workspace_bytes.restype = sz
+    lib.assemble_candidates_workspace_bytes.argtypes = [i32, i32]
+    lib.assemble_candidates_f32.restype = i32
+    lib.assemble_candidates_f32.argtypes = [vp, i32, i32, _c.c_uint64, i32, i32, vp, vp, vp, sz, vp]
+    for name in ("fps_batch_f32", "fps_batch_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp]
     _lib = lib
     return lib
 

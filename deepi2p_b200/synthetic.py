@@ -200,6 +200,47 @@ def make_lidar_scan(seed, n_rings=64, n_azimuth=2048, noise=0.01, ground=-1.73, 
     return dict(xyz=xyz.T.astype(np.float32), intensity=inten, ground=on_ground)
 
 
+def _rigid(rng, rot_amp, t_amp):
+    a = rng.uniform(-rot_amp, rot_amp, 3)
+    c, s = np.cos(a), np.sin(a)
+    Rx = np.array([[1, 0, 0], [0, c[0], -s[0]], [0, s[0], c[0]]])
+    Ry = np.array([[c[1], 0, s[1]], [0, 1, 0], [-s[1], 0, c[1]]])
+    Rz = np.array([[c[2], -s[2], 0], [s[2], c[2], 0], [0, 0, 1]])
+    P = np.eye(4)
+    P[:3, :3] = Rz @ Ry @ Rx
+    P[:3, 3] = rng.uniform(-t_amp, t_amp, 3)
+    return P
+
+
+def make_loader_sample(seed, shape="kitti", n_rings=64, n_azimuth=512):
+    """One seeded loader sample for deepi2p_b200.assemble.  kitti: 7 make_lidar_scan frames (the anchor first, then
+    3 before and 3 after it, each moved by a small rigid frame_T as search_for_accumulation composes Pc^-1 P_ij Pc),
+    unit normals, Pc (camera <- velodyne) and Pji; oxford: one frame in camera axes (x right, y down, z forward), no
+    normals, and P_cam_pc.  Returns dict(frames [(xyz [3,n] f32, intensity [n] f32, sn [3,n] f32 or None)], frame_T
+    [T,4,4], K [3,3], and Pc / Pji (kitti) or P_cam_pc (oxford))."""
+    rng = np.random.default_rng(seed + 0x10AD)
+    K = np.array([[358.0, 0.0, 256.0], [0.0, 358.0, 80.0], [0.0, 0.0, 1.0]])
+    if shape == "kitti":
+        frames, Ts = [], []
+        for t in range(7):
+            sc = make_lidar_scan(seed * 16 + t, n_rings=n_rings, n_azimuth=n_azimuth)
+            nrm = rng.normal(0.0, 0.2, sc["xyz"].shape) + np.array([[0.0], [0.0], [1.0]])
+            nrm = (nrm / np.linalg.norm(nrm, axis=0)).astype(np.float32)
+            frames.append((sc["xyz"], sc["intensity"], nrm))
+            Ts.append(np.eye(4) if t == 0 else _rigid(rng, 0.02, 6.0))
+        Pc = np.eye(4)
+        Pc[:3, :3] = np.array([[0.0, -1.0, 0.0], [0.0, 0.0, -1.0], [1.0, 0.0, 0.0]]) @ _rigid(rng, 0.01, 0.0)[:3, :3]
+        Pc[:3, 3] = [0.06, -0.08, -0.27]
+        return dict(frames=frames, frame_T=np.stack(Ts), K=K, Pc=Pc, Pji=_rigid(rng, 0.05, 3.0))
+    if shape == "oxford":
+        sc = make_lidar_scan(seed * 16, n_rings=n_rings, n_azimuth=n_azimuth)
+        x, y, z = sc["xyz"]
+        cam = np.stack([-y, -z, x]).astype(np.float32)
+        return dict(frames=[(cam, sc["intensity"], None)], frame_T=np.eye(4)[None], K=K,
+                    P_cam_pc=_rigid(rng, 0.1, 5.0))
+    raise ValueError(f"shape must be 'kitti' or 'oxford' (got {shape!r})")
+
+
 def write_icp_handoff(data_dir, monodepth_dir, seeds, shape="oxford"):
     """make_icp_frame frames as a hand-off directory (<id>_pc_label.npy / _K.npy / _P.npy, labels = the GT inside
     mask) plus the <monodepth_dir>/<id>_pc.npy depth clouds registration_icp.py:204 reads.  Returns the frames by id."""

@@ -350,6 +350,53 @@ int nearest_batch_f32(const double* q, const int32_t* q_pts, int q_stride, const
                       int m_stride, int S, int32_t* idx_out, void* workspace, size_t workspace_bytes,
                       dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Batch assembly of the classifier's point inputs (the loaders' __getitem__ after the scan records are read:
+ * data/kitti_pc_img_pose_loader.py:199-446, data/oxford_pc_img_pose_loader.py:262-352).  DESIGN.md "Batch assembly"
+ * states the contract.  [dev] pointers; 0 <= S <= 65535; fp64 arithmetic without FMA, rounded once to float32.
+ * Random draws are Philox4x32-10 with key = seed and counter (position, sample, stream id, 0); stream ids: 1 resample
+ * key, 2 pc jitter, 3 sn jitter, 4 node_a candidates, 5 node_b candidates, 6 intensity jitter.
+ *
+ * assemble_accumulate_f32: T frames xyz [T][3][n_stride] f32, intensity [T][n_stride] f32, sn [T][3][n_stride] f32
+ *   (may be NULL), n_pts [T] i32 (NULL = n_stride); frame_sample [T] i32 non-decreasing in [0, S); frame_T16 [T][16]
+ *   f64 row-major.  p' = ((T00 x + T01 y) + T02 z) + T03 per row, normals get the rotation only; range_max > 0 keeps
+ *   points with x'^2 + z'^2 < range_max^2 in float32.  Each sample's kept points are written in (frame, index) order to
+ *   xyz_out [S][3][out_stride], intensity_out [S][out_stride], sn_out [S][3][out_stride] (with sn); count_out [S] i32.
+ *   workspace >= assemble_accumulate_workspace_bytes(T, n_stride, S), 256-byte aligned.
+ * assemble_resample_f32: S clouds as above (stride n_stride, counts n_pts [S]) to input_pt_num = N points each
+ *   (data/kitti_pc_img_pose_loader.py:158-171): with n >= N points, the N smallest (key, index); otherwise index o < r n
+ *   takes o mod n (r >= 1 the smallest with (r + 1) n >= N) and the rest the N - r n smallest keys, in ascending key
+ *   order.  jitter mask 1 = pc, 2 = sn, 4 = intensity: + (float)clip(sigma z, -clip, clip), z from Box-Muller; then
+ *   M16 [S][16] f64 (pc affine, sn rotation only).  xyz_out [S][3][N], intensity_out [S][N], sn_out [S][3][N] (may be
+ *   NULL; zeros without sn), src_out [S][N] i32 (index into the input cloud; -1 for an empty cloud).
+ *   workspace >= assemble_resample_workspace_bytes(S, n_stride), 256-byte aligned.
+ * assemble_candidates_f32: per sample of pc [S][3][N] f32, the m smallest-key points (node_set 0 = node_a, 1 = node_b),
+ *   in ascending key order: idx_out [S][m] i32, xyz_out [S][3][m] f32.  1 <= m <= N.
+ *   workspace >= assemble_candidates_workspace_bytes(S, N), 256-byte aligned.
+ * fps_batch_f32 / fps_batch_f64: farthest-point sampling (data/kitti_helper.py:224-243) of k points from each of S sets
+ *   xyz [S][3][n_stride] (n_pts [S] i32, NULL = n_stride), starting at start [S] i32 (NULL, or outside [0, n): 0).
+ *   d2 = (dx dx + dy dy) + dz dz in fp64; each round takes the point of largest running minimum, lowest index on ties.
+ *   1 <= k <= n_stride <= 65536; idx_out [S][k] i32, nodes_out [S][3][k] (-1 and zeros for an empty set).  No
+ *   workspace.  Sets above 8192 points run on a thread-block cluster.
+ * ------------------------------------------------------------------------------------------ */
+size_t assemble_accumulate_workspace_bytes(int T, int n_stride, int S);
+int assemble_accumulate_f32(const float* xyz, const float* intensity, const float* sn, const int32_t* n_pts,
+                            int n_stride, int T, const int32_t* frame_sample, const double* frame_T16, int S,
+                            double range_max, float* xyz_out, float* intensity_out, float* sn_out, int out_stride,
+                            int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+size_t assemble_resample_workspace_bytes(int S, int n_stride);
+int assemble_resample_f32(const float* xyz, const float* intensity, const float* sn, const int32_t* n_pts,
+                          int n_stride, int S, int input_pt_num, uint64_t seed, const double* M16, double sigma,
+                          double clip, int jitter, float* xyz_out, float* intensity_out, float* sn_out,
+                          int32_t* src_out, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+size_t assemble_candidates_workspace_bytes(int S, int N);
+int assemble_candidates_f32(const float* pc, int N, int S, uint64_t seed, int node_set, int m, int32_t* idx_out,
+                            float* xyz_out, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+int fps_batch_f32(const float* xyz, const int32_t* n_pts, int n_stride, int S, int k, const int32_t* start,
+                  int32_t* idx_out, float* nodes_out, dib_stream_t stream);
+int fps_batch_f64(const double* xyz, const int32_t* n_pts, int n_stride, int S, int k, const int32_t* start,
+                  int32_t* idx_out, double* nodes_out, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
