@@ -26,7 +26,8 @@ EXPORTS = (
     "estimate_normals_batch_f32", "nearest_batch_f32",
     "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32", "assemble_resample_workspace_bytes",
     "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
-    "fps_batch_f64",
+    "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
+    "interp_backward_f32",
 )
 
 
@@ -171,6 +172,14 @@ def load():
     for name in ("fps_batch_f32", "fps_batch_f64"):
         getattr(lib, name).restype = i32
         getattr(lib, name).argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp]
+    lib.interp_weights_f32.restype = i32
+    lib.interp_weights_f32.argtypes = [vp, i32, vp, vp, i32, i32, i32, i32, vp, vp, vp]
+    lib.interp_forward_f32.restype = i32
+    lib.interp_forward_f32.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp]
+    lib.interp_backward_workspace_bytes.restype = sz
+    lib.interp_backward_workspace_bytes.argtypes = [i32, i32, i32, i32]
+    lib.interp_backward_f32.restype = i32
+    lib.interp_backward_f32.argtypes = [vp, _c.c_int64, vp, vp, i32, i32, i32, i32, i32, vp, vp, sz, vp]
     _lib = lib
     return lib
 

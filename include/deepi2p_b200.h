@@ -397,6 +397,32 @@ int fps_batch_f32(const float* xyz, const int32_t* n_pts, int n_stride, int S, i
 int fps_batch_f64(const double* xyz, const int32_t* n_pts, int n_stride, int S, int k, const int32_t* start,
                   int32_t* idx_out, double* nodes_out, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Inverse-distance feature interpolation of the classifier's decoder (models/networks_united.py:76-103,
+ * KeypointDetector.upsample_by_interpolation; SURVEY.md 8f N9).  DESIGN.md 4.12 states the contract.  [dev] pointers;
+ * 0 <= B <= 65535, 1 <= M <= 2048, 1 <= k <= 8; float32 arithmetic without FMA, IEEE sqrt and division.
+ *
+ * interp_weights_f32: topk_idx [B][Nq][k] int32 (idx_bytes 4) or int64 (idx_bytes 8), query [B][3][Nq] f32, node
+ *   [B][3][M] f32.  Per query point d_j = sqrt((dx*dx + dy*dy) + dz*dz), dx = query - node[idx_j]; S = ((d_0 + d_1) +
+ *   ...) + d_{k-1}; w_j = 1 - d_j / S into w_out [B][Nq][k] f32, the index into idx_out [B][Nq][k] int32.  A point with
+ *   any index outside [0, M) reads no node and gets w = NaN, idx = -1 in all k slots.
+ * interp_forward_f32: out [B][C][Nq] = ((w_0 F[c][i_0] + w_1 F[c][i_1]) + ...) from features [B][C][M] f32 and the
+ *   weights call's w / idx; a point with idx = -1 gets NaN in all C channels.
+ * interp_backward_f32: grad_features [B][C][M] f32 = sum over (n, j) with idx[b][n][j] = m of w[b][n][j] *
+ *   grad_out[b][c][n], for grad_out with element (b, c, n) at b * grad_batch_stride + c * Nq + n (grad_batch_stride >=
+ *   0; a channel slice of a larger [B][C'][Nq] tensor passes C' * Nq).  The fp32 products are added exactly in fp64, in ascending (n, j) within fixed slices of n and the slices
+ *   in order, then rounded once: deterministic for a given shape, no atomics.  Points with idx = -1 contribute nothing.
+ *   workspace: [dev] 8-byte aligned, >= interp_backward_workspace_bytes(B, C, Nq, M) (fp64 slice partials).
+ * ------------------------------------------------------------------------------------------ */
+int interp_weights_f32(const void* topk_idx, int idx_bytes, const float* query, const float* node, int B, int Nq,
+                       int M, int k, float* w_out, int32_t* idx_out, dib_stream_t stream);
+int interp_forward_f32(const float* features, const float* w, const int32_t* idx, int B, int C, int Nq, int M, int k,
+                       float* out, dib_stream_t stream);
+size_t interp_backward_workspace_bytes(int B, int C, int Nq, int M);
+int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* w, const int32_t* idx, int B,
+                        int C, int Nq, int M, int k, float* grad_features, void* workspace, size_t workspace_bytes,
+                        dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -47,6 +47,15 @@ if which in ("all", "ops"):
     print("ball_query_xyz", point_ops.ball_query_xyz_forward(torch.from_numpy(pts).cuda(), torch.from_numpy(nodes).cuda(), 1.5, 12).sum().item())
     ca = point_ops.cluster_assign_forward(torch.from_numpy(pts).cuda(), torch.from_numpy(nodes).cuda(), 3)
     print("cluster_assign", ca["count"].sum().item(), ca["pc_decentered"].abs().sum().item())
+    # interp_weights / interp_forward / interp_backward (+ interp_reduce): M past one backward node range, a ragged
+    # channel chunk, one out-of-range index
+    nodes2 = torch.from_numpy(rng.uniform(0, 10, (2, 3, 150)).astype(np.float32)).cuda()
+    idx = point_ops.cluster_assign_forward(torch.from_numpy(pts).cuda(), nodes2, 3, want_centers=False)["min_k_idx"]
+    idx[1, 5, 2] = 150
+    feat = torch.randn(2, 70, 150, device="cuda", requires_grad=True)
+    up = point_ops.upsample_by_interpolation(idx, torch.from_numpy(pts).cuda(), nodes2, feat)
+    up.backward(torch.ones_like(up))
+    print("interp", torch.nan_to_num(up.detach()).abs().sum().item(), feat.grad.abs().sum().item())
 if which in ("all", "pnp"):
     from deepi2p_b200 import pnp
     fines = [syn.make_fine_labels(s, seed=i) for i, s in enumerate(smps)]
