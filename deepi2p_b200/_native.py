@@ -27,7 +27,7 @@ EXPORTS = (
     "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32", "assemble_resample_workspace_bytes",
     "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
     "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
-    "interp_backward_f32",
+    "interp_backward_f32", "image_assemble_workspace_bytes", "image_assemble_f32", "image_assemble_u8",
 )
 
 
@@ -180,6 +180,11 @@ def load():
     lib.interp_backward_workspace_bytes.argtypes = [i32, i32, i32, i32]
     lib.interp_backward_f32.restype = i32
     lib.interp_backward_f32.argtypes = [vp, _c.c_int64, vp, vp, i32, i32, i32, i32, i32, vp, vp, sz, vp]
+    lib.image_assemble_workspace_bytes.restype = sz
+    lib.image_assemble_workspace_bytes.argtypes = [i32, i32, i32]
+    for name in ("image_assemble_f32", "image_assemble_u8"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, sz, vp, vp, vp, i32, i32, i32, vp, vp, sz, vp]
     _lib = lib
     return lib
 

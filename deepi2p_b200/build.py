@@ -14,10 +14,10 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdeepi2p_b200.so")
 SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "ball_query_xyz.cu", "cluster_assign.cu",
-           "pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu"]
+           "pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu"]
 # Compiled on their own without FMA contraction: oracle_pnp/pnp_oracle.cpp, oracle_icp/icp_oracle.cpp and
-# oracle_prep/prep_oracle.cpp, oracle_assemble/ and oracle_interp/ restate their arithmetic bit for bit.
-NOFMA_SOURCES = ["pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu"]
+# oracle_prep/prep_oracle.cpp, oracle_assemble/, oracle_interp/ and oracle_image/ restate their arithmetic bit for bit.
+NOFMA_SOURCES = ["pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu"]
 HEADERS = ["common.cuh", "morton_index.cuh", "sym3_eig.cuh", os.path.join("..", "..", "include", "deepi2p_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -423,6 +423,43 @@ int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const 
                         int C, int Nq, int M, int k, float* grad_features, void* workspace, size_t workspace_bytes,
                         dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * The image side of classifier batches (data/kitti_pc_img_pose_loader.py:326-349,360-362,439-440,
+ * data/oxford_pc_img_pose_loader.py:238-259,300-301,368; SURVEY.md 8f N10).  DESIGN.md 4.13 states the contract.
+ * For each of S samples: rows [row0, row0 + rows) of an h x w x 3 uint8 frame (HWC, packed at src + offsets[s]),
+ * cv2.resize(INTER_LINEAR) to dh x dw (1 <= dh <= rows, 1 <= dw <= w; OpenCV's fixed-point arithmetic), the
+ * img_H x img_W window at (dy, dx) of the resized image, with jitter torchvision's ColorJitter steps on a PIL image in
+ * the given order (0 brightness, 1 contrast, 2 saturation, 3 hue; Pillow's arithmetic), with flip a column flip, and
+ * the CHW write into img_out [S][3][img_H][img_W] (float32 holding the integer values, or uint8).
+ *
+ * src: [dev] packed frames of src_bytes bytes.  offsets [host] int64 [S]; params [host] int32 [S][DIB_IMAGE_PARAMS]
+ * indexed by the DIB_IMG_* constants (flip, jitter 0 or 1; shift is the hue step's uint8 shift,
+ * (uint8)(int32)(hue * 255)); factors [host] float32 [S][3] = (brightness, contrast, saturation).  Every field is
+ * checked on the host (DIB_EINVAL).  workspace: [dev] 256-byte aligned, >= image_assemble_workspace_bytes(S, img_H,
+ * img_W) (DIB_ENOMEM); the parameters are uploaded into it on `stream`.  Deterministic: the contrast mean is an exact
+ * integer sum.
+ * ------------------------------------------------------------------------------------------ */
+#define DIB_IMAGE_PARAMS 16
+#define DIB_IMG_H 0
+#define DIB_IMG_W 1
+#define DIB_IMG_ROW0 2
+#define DIB_IMG_ROWS 3
+#define DIB_IMG_DH 4
+#define DIB_IMG_DW 5
+#define DIB_IMG_DY 6
+#define DIB_IMG_DX 7
+#define DIB_IMG_FLIP 8
+#define DIB_IMG_JITTER 9
+#define DIB_IMG_ORDER 10 /* 4 entries */
+#define DIB_IMG_SHIFT 14
+size_t image_assemble_workspace_bytes(int S, int img_H, int img_W);
+int image_assemble_f32(const uint8_t* src, size_t src_bytes, const int64_t* offsets, const int32_t* params,
+                       const float* factors, int S, int img_H, int img_W, float* img_out, void* workspace,
+                       size_t workspace_bytes, dib_stream_t stream);
+int image_assemble_u8(const uint8_t* src, size_t src_bytes, const int64_t* offsets, const int32_t* params,
+                      const float* factors, int S, int img_H, int img_W, uint8_t* img_out, void* workspace,
+                      size_t workspace_bytes, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
