@@ -2133,9 +2133,10 @@ template <typename CT>
 static int residuals_single(const CT* xyz, const int8_t* label, int n, int n_stride, const double* K9,
                             const double* x, double H, double W, int is_2d, const int32_t* row_offset,
                             double* residuals, dib_stream_t stream) {
-  DIB_REQUIRE(xyz && label && K9 && x && row_offset && residuals, "NULL argument");
+  DIB_REQUIRE(xyz && label && K9 && x && residuals, "NULL argument");
   DIB_REQUIRE(n >= 0 && n <= n_stride, "bad n");
-  if (n == 0) return DIB_OK;
+  if (n == 0) return DIB_OK;                            // no rows: the (empty) row offsets may be NULL
+  DIB_REQUIRE(row_offset, "NULL argument");
   cudaStream_t st = (cudaStream_t)stream;
   const int blocks = (n + 255) / 256;
   if (is_2d)

@@ -454,7 +454,12 @@ def inside_mask_batch(xyz, n_pts, P, K, H, W, stream=None):
 def pose_error_batch(P_pred, P_gt, t_thresh=2.0, r_thresh=5.0, stream=None):
     """Batched get_P_diff (registration_lsq.py:87-95) + the authors' success criterion
     (registration_result_analysis.py:37-38).  Returns dict(t_err [S] m, r_err [S] deg, success [S] int32,
-    success_rate float tensor)."""
+    success_rate float tensor).
+
+    P_pred is inverted as a general 4x4 matrix (as np.linalg.inv does), and r_err follows scipy's
+    Rotation.from_matrix(...).as_euler('xzy') step for step, including its orthogonalisation of a non-rigid block and
+    its gimbal-lock rule (DESIGN.md 4.14); oracle.pose_diff_restated reproduces the results bit for bit.  A rotation
+    block with det <= 0 (where scipy raises) or a NaN gives r_err = NaN and success 0."""
     _require_cuda()
     lib = _native.load()
     Pp = torch.as_tensor(P_pred, dtype=torch.float64)

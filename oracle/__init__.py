@@ -227,6 +227,156 @@ def pose_diff(P_pred, P_gt):
     return t_diff, angles
 
 
+# ---- pose_error_batch restated (csrc/metrics.cu): the kernel's fp64 operations in the kernel's order --------------
+# Every step is +, -, *, /, sqrt or a comparison, each correctly rounded in numpy and in the kernel (compiled without
+# FMA contraction), so the kernel reproduces these arrays bit for bit.  DESIGN.md 4.14 describes it.
+_PI = math.pi
+_ATAN_C = [(-1.0) ** k / (2 * k + 1) for k in range(12)]      # atan(z) = z * sum_k (-1)^k z^(2k) / (2k+1)
+
+
+def _atan2_restated(y, x):
+    """atan2 from two argument halvings and a 12-term series on |t| <= tan(pi/16) (a few ulp)."""
+    ax, ay = np.abs(x), np.abs(y)
+    swap = ay > ax
+    num, den = np.where(swap, ax, ay), np.where(swap, ay, ax)
+    t = np.where(den == 0, 0.0, num / np.where(den == 0, 1.0, den))
+    t = t / (1.0 + np.sqrt(1.0 + t * t))
+    t = t / (1.0 + np.sqrt(1.0 + t * t))
+    z = t * t
+    p = np.full_like(z, _ATAN_C[11])
+    for k in range(10, -1, -1):
+        p = p * z + _ATAN_C[k]
+    r = 4.0 * (t * p)
+    r = np.where(swap, _PI / 2 - r, r)
+    r = np.where(np.signbit(x), _PI - r, r)
+    return np.where(np.signbit(y), -r, r)
+
+
+def _wrap_pi(a):
+    """(a + pi) % (2 pi) - pi with numpy's floor remainder."""
+    m = np.fmod(a + _PI, 2 * _PI)
+    m = np.where(m == 0, 0.0, np.where(m < 0, m + 2 * _PI, m))
+    return m - _PI
+
+
+def _inv4_rows3(A):
+    """Rows 0..2 of the cofactor inverse of 4x4 matrices A [S,4,4] (fp64, one division per entry)."""
+    a = [[A[:, r, c] for c in range(4)] for r in range(4)]
+    s0 = a[0][0] * a[1][1] - a[1][0] * a[0][1]
+    s1 = a[0][0] * a[1][2] - a[1][0] * a[0][2]
+    s2 = a[0][0] * a[1][3] - a[1][0] * a[0][3]
+    s3 = a[0][1] * a[1][2] - a[1][1] * a[0][2]
+    s4 = a[0][1] * a[1][3] - a[1][1] * a[0][3]
+    s5 = a[0][2] * a[1][3] - a[1][2] * a[0][3]
+    c5 = a[2][2] * a[3][3] - a[3][2] * a[2][3]
+    c4 = a[2][1] * a[3][3] - a[3][1] * a[2][3]
+    c3 = a[2][1] * a[3][2] - a[3][1] * a[2][2]
+    c2 = a[2][0] * a[3][3] - a[3][0] * a[2][3]
+    c1 = a[2][0] * a[3][2] - a[3][0] * a[2][2]
+    c0 = a[2][0] * a[3][1] - a[3][0] * a[2][1]
+    det = s0 * c5 - s1 * c4 + s2 * c3 + s3 * c2 - s4 * c1 + s5 * c0
+    return [[(a[1][1] * c5 - a[1][2] * c4 + a[1][3] * c3) / det,
+             (-a[0][1] * c5 + a[0][2] * c4 - a[0][3] * c3) / det,
+             (a[3][1] * s5 - a[3][2] * s4 + a[3][3] * s3) / det,
+             (-a[2][1] * s5 + a[2][2] * s4 - a[2][3] * s3) / det],
+            [(-a[1][0] * c5 + a[1][2] * c2 - a[1][3] * c1) / det,
+             (a[0][0] * c5 - a[0][2] * c2 + a[0][3] * c1) / det,
+             (-a[3][0] * s5 + a[3][2] * s2 - a[3][3] * s1) / det,
+             (a[2][0] * s5 - a[2][2] * s2 + a[2][3] * s1) / det],
+            [(a[1][0] * c4 - a[1][1] * c2 + a[1][3] * c0) / det,
+             (-a[0][0] * c4 + a[0][1] * c2 - a[0][3] * c0) / det,
+             (a[3][0] * s4 - a[3][1] * s2 + a[3][3] * s0) / det,
+             (-a[2][0] * s4 + a[2][1] * s2 - a[2][3] * s0) / det]]
+
+
+def _cof3(m):
+    """Cofactor matrix and determinant of 3x3 matrices given as nested lists of [S] arrays."""
+    C = [[m[1][1] * m[2][2] - m[1][2] * m[2][1], m[1][2] * m[2][0] - m[1][0] * m[2][2],
+          m[1][0] * m[2][1] - m[1][1] * m[2][0]],
+         [m[0][2] * m[2][1] - m[0][1] * m[2][2], m[0][0] * m[2][2] - m[0][2] * m[2][0],
+          m[0][1] * m[2][0] - m[0][0] * m[2][1]],
+         [m[0][1] * m[1][2] - m[0][2] * m[1][1], m[0][2] * m[1][0] - m[0][0] * m[1][2],
+          m[0][0] * m[1][1] - m[0][1] * m[1][0]]]
+    det = m[0][0] * C[0][0] + m[0][1] * C[0][1] + m[0][2] * C[0][2]
+    return C, det
+
+
+POLAR_MAX_ITER = 64
+
+
+def pose_diff_restated(P_pred, P_gt, t_thresh=2.0, r_thresh=5.0):
+    """The arithmetic of pose_error_batch (csrc/metrics.cu) for P_pred, P_gt [S,4,4]: (t_err [S], r_err [S] degrees,
+    success [S] int32).  Follows get_P_diff (np.linalg.inv, scipy from_matrix + as_euler('xzy')) step for step:
+    general inverse; orthogonality test |M M^T - I| <= 1e-12 + 1e-5 I else the polar factor (scipy's U V^T); the
+    largest-of-(diag, trace) quaternion; the quaternion Euler extraction with its gimbal-lock rule.  A rotation block
+    with det <= 0 (scipy raises) or NaN gives r_err = NaN, success = 0."""
+    A = np.asarray(P_pred, dtype=np.float64).reshape(-1, 4, 4)
+    B = np.asarray(P_gt, dtype=np.float64).reshape(-1, 4, 4)
+    with np.errstate(all="ignore"):
+        inv = _inv4_rows3(A)
+        D = [[((inv[i][0] * B[:, 0, j] + inv[i][1] * B[:, 1, j]) + inv[i][2] * B[:, 2, j]) + inv[i][3] * B[:, 3, j]
+              for j in range(4)] for i in range(3)]
+        t = [D[i][3] for i in range(3)]
+        te = np.sqrt((t[0] * t[0] + t[1] * t[1]) + t[2] * t[2])
+        M = [[D[i][j] for j in range(3)] for i in range(3)]
+        _, det = _cof3(M)
+        valid = det > 0
+        ortho = np.ones_like(det, dtype=bool)
+        for i in range(3):
+            for j in range(3):
+                g = (M[i][0] * M[j][0] + M[i][1] * M[j][1]) + M[i][2] * M[j][2]
+                ortho &= np.abs(g - 1.0) <= 1e-12 + 1e-5 if i == j else np.abs(g) <= 1e-12
+        # polar factor by Newton's iteration X <- (X + X^-T) / 2 for the samples that fail the test
+        active = ~ortho & valid
+        for _ in range(POLAR_MAX_ITER):
+            if not active.any():
+                break
+            C, dX = _cof3(M)
+            X = [[0.5 * (M[i][j] + C[i][j] / dX) for j in range(3)] for i in range(3)]
+            done = np.ones_like(active)
+            for i in range(3):
+                for j in range(3):
+                    done &= np.abs(X[i][j] - M[i][j]) < 1e-10      # quadratic convergence: X is now exact
+                    M[i][j] = np.where(active, X[i][j], M[i][j])
+            active &= ~done
+        # quaternion (x, y, z, w) from the largest of m00, m11, m22, trace (first one on ties)
+        tr = (M[0][0] + M[1][1]) + M[2][2]
+        choice = np.zeros(det.shape, dtype=np.int64)
+        best = M[0][0]
+        for c, v in ((1, M[1][1]), (2, M[2][2]), (3, tr)):
+            choice = np.where(v > best, c, choice)
+            best = np.where(v > best, v, best)
+        q = [None] * 4
+        cand = []
+        for i in range(3):
+            j, k = (i + 1) % 3, (i + 2) % 3
+            qi = [None] * 4
+            qi[i] = (1.0 - tr) + 2.0 * M[i][i]
+            qi[j] = M[j][i] + M[i][j]
+            qi[k] = M[k][i] + M[i][k]
+            qi[3] = M[k][j] - M[j][k]
+            cand.append(qi)
+        cand.append([M[2][1] - M[1][2], M[0][2] - M[2][0], M[1][0] - M[0][1], 1.0 + tr])
+        for e in range(4):
+            q[e] = np.select([choice == c for c in range(4)], [cand[c][e] for c in range(4)])
+        qn = np.sqrt(((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3])
+        qx, qy, qz, qw = (v / qn for v in q)
+        # extrinsic 'xzy': axes (i, j, k) = (0, 2, 1), sign = -1, lambda = pi / 2
+        a, b, c, d = qw - qz, qx - qy, qz + qw, -qy - qx
+        half_sum = _atan2_restated(b, a)
+        half_diff = _atan2_restated(d, c)
+        mid = 2.0 * _atan2_restated(np.sqrt(c * c + d * d), np.sqrt(a * a + b * b))
+        lock0 = np.abs(mid) <= 1e-7                 # middle angle -pi/2: third angle 0, first 2 half_sum
+        lock1 = ~lock0 & (np.abs(mid - _PI) <= 1e-7)  # middle angle +pi/2: third angle 0, first -2 half_diff
+        first = np.where(lock0, 2.0 * half_sum, np.where(lock1, -2.0 * half_diff, half_sum - half_diff))
+        third = np.where(lock0 | lock1, 0.0, -(half_sum + half_diff))
+        deg = 180.0 / _PI
+        re = (np.abs(_wrap_pi(first) * deg) + np.abs(_wrap_pi(mid - _PI / 2) * deg)) + np.abs(_wrap_pi(third) * deg)
+        re = np.where(valid, re, np.nan)
+        ok = ((te < t_thresh) & (re < r_thresh)).astype(np.int32)
+    return te, re, ok
+
+
 def index_max(data, index, K):
     """Oracle for index_max.forward_* (index_max.cpp:73-112)."""
     lib = _lib("libops_oracle.so")
