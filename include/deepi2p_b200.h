@@ -244,12 +244,14 @@ int ball_query_xyz_forward(const float* points, const float* nodes, float radius
  * intermediates of models/networks_pc.py:60-85) -------------------------------------------------
  * pc [B][3][N] f32, node [B][3][M] f32 [dev].  Outputs [dev]:
  *   min_k_idx [B][N][k] i32  k nearest nodes of each point, nearest first (torch.topk(diff, k, largest=False), :63-64);
- *                            key ((dx*dx + dy*dy) + dz*dz) in float32 without fma, ties -> lower node index
+ *                            key ((dx*dx + dy*dy) + dz*dz) in float32 without fma, ties -> lower node index,
+ *                            +inf after every finite key and NaN after +inf (k distinct nodes always)
  *   min_idx   [B][N]    i32  = min_k_idx[..][0], the `index` argument of index_max (:65,:88-90)
  *   count     [B][M]    i32  points per node (mask_row_sum, :69-72; mask_row_max = count > 0)
- *   cluster_mean [B][3][M] f32 = float(sum_fixed * 2^-24) / (float(count) + 1e-5f), sum_fixed = exact int64 sum
- *                            of rint(x * 2^24) -- order independent (:74-76); points with a non-finite coordinate are
- *                            left out of count and sums (they still get min_idx 0)
+ *   cluster_mean [B][3][M] f32 = round_f32(sum_fixed * 2^-24) / (float(count) + 1e-5f), sum_fixed = the exact
+ *                            (two-word) sum of rint(x * 2^24) -- order independent (:74-76), at most 2^-25 per point
+ *                            from the exact sum; points with a coordinate of magnitude >= 2^39 or a non-finite one
+ *                            are left out of count and sums (they keep their min_k_idx / min_idx)
  *   pc_centers, pc_decentered [B][3][N] f32 (each may be NULL): cluster_mean gathered by min_idx, pc - centers (:78-82)
  * 1 <= k <= min(8, M), M <= 2048.  workspace: [dev], 8-byte aligned, >= cluster_assign_workspace_bytes(B, M). */
 size_t cluster_assign_workspace_bytes(int B, int M);

@@ -453,29 +453,48 @@ def ball_query_xyz(points, nodes, radius, K):
     return out
 
 
+def int_to_f32(v):
+    """The integer v rounded once to float32 (nearest, ties to even): cut to 53 bits with a sticky bit for the rest,
+    which float64 holds exactly, then one rounding to float32."""
+    s = max(abs(v).bit_length() - 53, 0)
+    m = abs(v) >> s
+    if s and abs(v) & ((1 << s) - 1):
+        m |= 1
+    return np.float32(math.copysign(float(m), v)) * np.float32(2.0 ** s)
+
+
 def cluster_assign(pc, node, k):
     """Oracle for cluster_assign_forward: the clustering front-end of models/networks_pc.py:60-85.
 
     pc [B,3,N], node [B,3,M].  Ordering key = float32 ((dx*dx + dy*dy) + dz*dz) (numpy float32 arithmetic has no
-    fma), stable sort => ties go to the lower node index (torch.topk leaves them unspecified; sqrt is monotone).
-    Sums are exact fixed point (rint(x * 2^24) in int64), mean = float32(sum * 2^-24) / (float32(count) + 1e-5f)."""
+    fma), stable sort => ties go to the lower node index (torch.topk leaves them unspecified; sqrt is monotone), +inf
+    after finite keys, NaN last.  Sums: each coordinate rounded to the 2^-24 grid (rint(x * 2^24), an int64), the
+    integers added exactly; mean = round_f32(sum * 2^-24) / (float32(count) + 1e-5f).  Points with a coordinate of
+    magnitude >= 2^39 (no int64 image) or a non-finite one join no count or sum."""
     p = np.asarray(pc, dtype=np.float32)
     q = np.asarray(node, dtype=np.float32)
     B, _, N = p.shape
     M = q.shape[2]
-    d = p[:, :, :, None] - q[:, :, None, :]                      # [B,3,N,M], point - node
-    d2 = (d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]
+    with np.errstate(over="ignore", invalid="ignore"):
+        d = p[:, :, :, None] - q[:, :, None, :]                  # [B,3,N,M], point - node
+        d2 = (d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]
     order = np.argsort(d2, axis=2, kind="stable")[:, :, :k].astype(np.int32)
     min_idx = order[:, :, 0]
     count = np.zeros((B, M), dtype=np.int32)
-    sums = np.zeros((B, 3, M), dtype=np.int64)
-    finite = np.isfinite(p).all(axis=1)                           # non-finite points join no count / sum
-    fixed = np.rint(np.where(finite[:, None, :], p, 0).astype(np.float64) * 16777216.0).astype(np.int64)
+    with np.errstate(invalid="ignore"):
+        summed = (np.abs(p) < np.float32(2.0 ** 39)).all(axis=1)  # False for inf / NaN too
+    fixed = np.rint(np.where(summed[:, None, :], p, 0).astype(np.float64) * 16777216.0).astype(np.int64)
+    # exact sums of any number of points below 2^31: the low 32 bits and the rest are added apart, then joined
+    lo, hi = fixed & 0xffffffff, fixed >> 32
+    s_lo = np.zeros((B, 3, M), dtype=np.int64)
+    s_hi = np.zeros((B, 3, M), dtype=np.int64)
     for b in range(B):
-        np.add.at(count[b], min_idx[b][finite[b]], 1)
+        np.add.at(count[b], min_idx[b][summed[b]], 1)
         for a in range(3):
-            np.add.at(sums[b, a], min_idx[b][finite[b]], fixed[b, a][finite[b]])
-    num = (sums.astype(np.float64) * (1.0 / 16777216.0)).astype(np.float32)
+            np.add.at(s_lo[b, a], min_idx[b][summed[b]], lo[b, a][summed[b]])
+            np.add.at(s_hi[b, a], min_idx[b][summed[b]], hi[b, a][summed[b]])
+    num = np.array([int_to_f32((int(h) << 32) + int(l)) for h, l in zip(s_hi.ravel(), s_lo.ravel())],
+                   dtype=np.float32).reshape(B, 3, M) * np.float32(2.0 ** -24)
     mean = num / (count.astype(np.float32)[:, None, :] + np.float32(1e-5))
     centers = np.take_along_axis(mean, np.broadcast_to(min_idx[:, None, :].astype(np.int64), (B, 3, N)), axis=2)
     return dict(min_k_idx=order, min_idx=min_idx.copy(), count=count, cluster_mean=mean.astype(np.float32),

@@ -56,6 +56,30 @@ if which in ("all", "ops"):
     up = point_ops.upsample_by_interpolation(idx, torch.from_numpy(pts).cuda(), nodes2, feat)
     up.backward(torch.ones_like(up))
     print("interp", torch.nan_to_num(up.detach()).abs().sum().item(), feat.grad.abs().sum().item())
+    # interp rows with repeated indices (all equal, one pair equal, S = 0) beside distinct ones, M = 129 with every
+    # index in the last node range
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+    from test_point_ops_edges_cpu import fps_cloud, interp_case
+    for case in ((2, 200, 10, 40, 3, 0, 10), (1, 300, 129, 48, 3, 128, 129)):
+        i_, q_, n_, f_ = (torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in interp_case(0, *case))
+        f_.requires_grad_(True)
+        up = point_ops.upsample_by_interpolation(i_, q_, n_, f_)
+        up.backward(torch.ones_like(up))
+        print("interp repeated", case, torch.nan_to_num(f_.grad).abs().sum().item())
+    # farthest-point sampling on the cluster path: 8 CTAs with empty slices and k above two of the counts, f32 / f64
+    from deepi2p_b200 import _native
+    fp = np.stack([fps_cloud("lattice", 65536, s) for s in range(3)])
+    for dt in (torch.float32, torch.float64):
+        x = torch.from_numpy(np.ascontiguousarray(fp)).to(dt).cuda()
+        cnt = torch.tensor([1, 100, 8193], dtype=torch.int32, device="cuda")
+        st = torch.tensor([0, 99, 8192], dtype=torch.int32, device="cuda")
+        fi = torch.empty((3, 150), dtype=torch.int32, device="cuda")
+        fn_ = torch.empty((3, 3, 150), dtype=dt, device="cuda")
+        lib = _native.load()
+        f = lib.fps_batch_f32 if dt == torch.float32 else lib.fps_batch_f64
+        _native.check(f(x.data_ptr(), cnt.data_ptr(), 65536, 3, 150, st.data_ptr(), fi.data_ptr(), fn_.data_ptr(),
+                        torch.cuda.current_stream().cuda_stream), "fps_batch")
+        print("fps cluster, empty slices", dt, fi[:, :4].tolist())
 if which in ("all", "pnp"):
     from deepi2p_b200 import pnp
     fines = [syn.make_fine_labels(s, seed=i) for i, s in enumerate(smps)]
