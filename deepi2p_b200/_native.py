@@ -29,6 +29,7 @@ EXPORTS = (
     "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
     "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
     "interp_backward_f32", "image_assemble_workspace_bytes", "image_assemble_f32", "image_assemble_u8",
+    "classifier_loss_workspace_bytes", "classifier_loss_forward_f32", "classifier_loss_backward_f32",
 )
 
 
@@ -192,6 +193,15 @@ def load():
     for name in ("image_assemble_f32", "image_assemble_u8"):
         getattr(lib, name).restype = i32
         getattr(lib, name).argtypes = [vp, sz, vp, vp, vp, i32, i32, i32, vp, vp, sz, vp]
+    lib.classifier_loss_workspace_bytes.restype = sz
+    lib.classifier_loss_workspace_bytes.argtypes = [i32, i32]
+    lib.classifier_loss_forward_f32.restype = i32
+    lib.classifier_loss_forward_f32.argtypes = [vp, _c.c_int64, vp, _c.c_int64, i32, vp, vp, vp, i32, i32, f64, f64,
+                                                f64, i32, i32, f64, f64, i32, f64, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                                vp, vp, vp, vp, vp, sz, vp]
+    lib.classifier_loss_backward_f32.restype = i32
+    lib.classifier_loss_backward_f32.argtypes = [vp, _c.c_int64, vp, _c.c_int64, i32, i32, i32, vp, vp, vp, vp, vp, vp,
+                                                 vp, f64, f64, i32, f64, vp, vp, vp]
     _lib = lib
     return lib
 

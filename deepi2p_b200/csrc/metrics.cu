@@ -11,6 +11,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "project.cuh"
 
 namespace dib {
 
@@ -26,17 +27,8 @@ __global__ void inside_mask_kernel(const float* __restrict__ xyz, const int32_t*
     const double* P = P16 + (size_t)s * 16;
     const double* K = K9 + (size_t)s * 9;
     const float* b = xyz + (size_t)s * 3 * n_stride;
-    const double x = b[i], y = b[n_stride + i], z = b[2 * (size_t)n_stride + i];
-    // P_points = (P [x y z 1]^T)[0:3]
-    const double X = P[0] * x + P[1] * y + P[2] * z + P[3];
-    const double Y = P[4] * x + P[5] * y + P[6] * z + P[7];
-    const double Z = P[8] * x + P[9] * y + P[10] * z + P[11];
-    // K_pc = K P_points ; pxpy = K_pc[0:2] / K_pc[2]
-    const double kx = K[0] * X + K[1] * Y + K[2] * Z;
-    const double ky = K[3] * X + K[4] * Y + K[5] * Z;
-    const double kz = K[6] * X + K[7] * Y + K[8] * Z;
-    const double u = kx / kz, v = ky / kz;
-    out = (u >= 0.0 && u <= W - 1.0 && v >= 0.0 && v <= H - 1.0 && Z > 0.1) ? 1 : 0;
+    double u, v;
+    out = project_inside(P, K, b[i], b[n_stride + i], b[2 * (size_t)n_stride + i], H, W, &u, &v) ? 1 : 0;
   }
   mask[(size_t)s * n_stride + i] = out;
 }

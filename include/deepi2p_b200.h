@@ -479,6 +479,41 @@ int image_assemble_u8(const uint8_t* src, size_t src_bytes, const int64_t* offse
                       const float* factors, int S, int img_H, int img_W, uint8_t* img_out, void* workspace,
                       size_t workspace_bytes, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training targets, losses, accuracies and predictions of the classifier (models/multimodal_classifier.py:135-191,
+ * coarse-only :482-508; SURVEY.md 8f N11).  DESIGN.md 4.15 states the contract.  [dev] pointers; 1 <= B <= 65535,
+ * N >= 1, B * N < 2^31, focal_gamma >= 0.  Scores: element (b, c, n) at b * batch_stride + c * N + n.  fine = NULL is
+ * the coarse-only classifier (the fine outputs are then not written and may be NULL).  No synchronous call.
+ *
+ * classifier_loss_forward_f32: pc [B][3][N] f32, P12 [B][12] f64 (rows 0..2 of P), K9 [B][9] f64.  Coarse label:
+ *   the rule of frustum_inside_mask_f32, bit for bit; fine label floor(u / s) + floor(v / s) * W_f for inside points,
+ *   -1 otherwise (L == H_f * W_f, floor((W-1)/s) < W_f and floor((H-1)/s) < H_f are checked on the host).  Writes
+ *   coarse_labels / coarse_pred int8 [B][N], fine_labels / fine_pred int32 [B][N], lse f32 [2][B][N] (each fine
+ *   row's max m and log sum exp(z - m), read by the backward), the f32 scalars loss = coarse_loss + fine_loss, coarse_loss (kornia focal
+ *   mean times coarse_loss_alpha) and fine_loss (cross-entropy mean over inside points, 0 if there is none), accuracy
+ *   [2] f32 (coarse over all points, fine over inside points; NaN when there is none), and int32 n_inside [B],
+ *   coarse_correct [B], fine_correct [B], n_inside_total [1].  Sums are fp64 in an order fixed by the shape.
+ *   workspace: [dev] 8-byte aligned, >= classifier_loss_workspace_bytes(B, N) (per-CTA partials).
+ * classifier_loss_backward_f32: grad_coarse [B][2][N] and grad_fine [B][L][N] f32 (either may be NULL), contiguous,
+ *   for the upstream gradients grad_loss, grad_coarse_loss, grad_fine_loss (each a [dev] f32 scalar) of the
+ *   forward's three losses, from its labels, lse and n_inside_total.
+ * ------------------------------------------------------------------------------------------ */
+size_t classifier_loss_workspace_bytes(int B, int N);
+int classifier_loss_forward_f32(const float* coarse, int64_t coarse_batch_stride, const float* fine,
+                                int64_t fine_batch_stride, int L, const float* pc, const double* P12, const double* K9,
+                                int B, int N, double H, double W, double fine_scale, int H_f, int W_f,
+                                double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
+                                int8_t* coarse_labels, int32_t* fine_labels, int8_t* coarse_pred, int32_t* fine_pred,
+                                float* lse, float* loss, float* coarse_loss, float* fine_loss, float* accuracy,
+                                int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
+                                int32_t* n_inside_total, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+int classifier_loss_backward_f32(const float* coarse, int64_t coarse_batch_stride, const float* fine,
+                                 int64_t fine_batch_stride, int L, int B, int N, const int8_t* coarse_labels,
+                                 const int32_t* fine_labels, const float* lse, const int32_t* n_inside_total,
+                                 const float* grad_loss, const float* grad_coarse_loss, const float* grad_fine_loss,
+                                 double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
+                                 float* grad_coarse, float* grad_fine, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
