@@ -30,6 +30,8 @@ EXPORTS = (
     "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
     "interp_backward_f32", "image_assemble_workspace_bytes", "image_assemble_f32", "image_assemble_u8",
     "classifier_loss_workspace_bytes", "classifier_loss_forward_f32", "classifier_loss_backward_f32",
+    "cluster_pool_forward_f32", "cluster_pool_backward_workspace_bytes", "cluster_pool_backward_f32",
+    "knn_group_forward_f32", "knn_group_backward_workspace_bytes", "knn_group_backward_f32",
 )
 
 
@@ -202,6 +204,18 @@ def load():
     lib.classifier_loss_backward_f32.restype = i32
     lib.classifier_loss_backward_f32.argtypes = [vp, _c.c_int64, vp, _c.c_int64, i32, i32, i32, vp, vp, vp, vp, vp, vp,
                                                  vp, f64, f64, i32, f64, vp, vp, vp]
+    lib.cluster_pool_forward_f32.restype = i32
+    lib.cluster_pool_forward_f32.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp]
+    lib.cluster_pool_backward_workspace_bytes.restype = sz
+    lib.cluster_pool_backward_workspace_bytes.argtypes = [i32, i32, i32, i32]
+    lib.cluster_pool_backward_f32.restype = i32
+    lib.cluster_pool_backward_f32.argtypes = [vp, vp, _c.c_int64, vp, vp, vp, i32, i32, i32, i32, vp, vp, sz, vp]
+    lib.knn_group_forward_f32.restype = i32
+    lib.knn_group_forward_f32.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
+    lib.knn_group_backward_workspace_bytes.restype = sz
+    lib.knn_group_backward_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
+    lib.knn_group_backward_f32.restype = i32
+    lib.knn_group_backward_f32.argtypes = [vp, _c.c_int64, vp, i32, i32, i32, i32, i32, vp, vp, sz, vp]
     _lib = lib
     return lib
 

@@ -26,9 +26,9 @@
 //     non-finite one is left out of its node's count and sums.  mean = round_f32(sum * 2^-24) /
 //     (float(count) + 1e-5f), the first rounding done once from the two-word sum.
 #include <cfloat>
-#include <type_traits>
 
 #include "common.cuh"
+#include "nearest_k.cuh"
 
 namespace dib {
 
@@ -38,7 +38,6 @@ constexpr int kCaMaxK = 8;
 constexpr int kCaMaxNodes = 2048;
 constexpr double kCaFixedScale = 16777216.0;        // 2^24
 constexpr float kCaFixedLimit = 549755813888.0f;    // 2^39: |x| * 2^24 < 2^63
-constexpr unsigned kCaNanKey = 0x7f800001u;         // every NaN d2 maps here: after +inf (0x7f800000)
 
 // hi:lo += v (two's complement): the returned old low word tells whether this addition carried, so the high word
 // receives exactly the carries and sign extensions, whatever order the additions land in.
@@ -47,39 +46,6 @@ __device__ __forceinline__ void add_wide_shared(unsigned long long* lo, int* hi,
   const unsigned long long old = atomicAdd(lo, u);
   const int h = (int)(old + u < old) - (int)(v < 0);
   if (h) atomicAdd(hi, h);
-}
-
-// The K nearest nodes of (x, y, z) by (key, node index), nearest first.  kAll = false keys on the float d2 and keeps
-// finite ones only: one compare per node, and enough unless fewer than K distances are finite, which the return value
-// reports.  kAll = true keys on the bits of d2 (never negative, so the bit order is the value order) with every NaN
-// clamped to kCaNanKey, just above +inf; the empty slots' key is above every node's, so every node has a place.
-template <int K, bool kAll>
-__device__ __forceinline__ bool nearest_k(float x, float y, float z, const float* s_node, int M, int (&bi)[K]) {
-  using Key = typename std::conditional<kAll, unsigned, float>::type;
-  Key bd[K];
-#pragma unroll
-  for (int j = 0; j < K; ++j) {
-    if constexpr (kAll) bd[j] = 0xffffffffu; else bd[j] = __int_as_float(0x7f800000);
-    bi[j] = j;
-  }
-#pragma unroll 4
-  for (int m = 0; m < M; ++m) {
-    const float dx = __fsub_rn(x, s_node[m]), dy = __fsub_rn(y, s_node[M + m]), dz = __fsub_rn(z, s_node[2 * M + m]);
-    const float f = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-    Key d2;
-    if constexpr (kAll) d2 = min(__float_as_uint(f), kCaNanKey); else d2 = f;
-    if (!(d2 < bd[K - 1])) continue;                  // strict: on a tie the earlier (lower) node stays
-    // sorted insert from the back; all indices are compile-time, so bd / bi stay in registers
-#pragma unroll
-    for (int j = K - 1; j >= 1; --j) {
-      const bool shift = d2 < bd[j - 1];
-      const bool here = !shift && d2 < bd[j];
-      bd[j] = shift ? bd[j - 1] : (here ? d2 : bd[j]);
-      bi[j] = shift ? bi[j - 1] : (here ? m : bi[j]);
-    }
-    if (d2 < bd[0]) { bd[0] = d2; bi[0] = m; }
-  }
-  if constexpr (kAll) return true; else return bd[K - 1] < __int_as_float(0x7f800000);
 }
 
 template <int K>

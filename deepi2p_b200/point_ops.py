@@ -134,7 +134,18 @@ def cluster_assign_forward(pc, node, k=1, want_centers=True):
 
 INTERP_MAX_K = 8
 INTERP_MAX_NODES = 2048
-_interp_ws = {}
+_backward_ws = {}
+
+
+def _backward_workspace(dev, stream, need):
+    """The fp64 slice partials of the interpolation's and the encoder ops' backwards: one scratch per stream (launches
+    on one stream run in order, so they can share it; launches on different streams may overlap)."""
+    key = (dev.index, stream)
+    ws = _backward_ws.get(key)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(max(need, 1 << 16), dtype=torch.uint8, device=dev)
+        _backward_ws[key] = ws
+    return ws
 
 
 def _check_interp_args(topk_idx, query, node, features):
@@ -209,12 +220,7 @@ class _Interpolation(torch.autograd.Function):
             gF = torch.empty((B, C, M), dtype=torch.float32, device=dev)
             if gF.numel():
                 stream = torch.cuda.current_stream().cuda_stream
-                need = lib.interp_backward_workspace_bytes(B, C, Nq, M)
-                key = (dev.index, stream)
-                ws = _interp_ws.get(key)
-                if ws is None or ws.numel() < need:
-                    ws = torch.empty(max(need, 1 << 16), dtype=torch.uint8, device=dev)
-                    _interp_ws[key] = ws
+                ws = _backward_workspace(dev, stream, lib.interp_backward_workspace_bytes(B, C, Nq, M))
                 bstride = grad_out.stride(0) if B > 1 else 0
                 rc = lib.interp_backward_f32(grad_out.data_ptr(), bstride, w.data_ptr(), idx.data_ptr(), B, C, Nq, M,
                                              k, gF.data_ptr(), ws.data_ptr(), ws.numel(), stream)
@@ -235,3 +241,193 @@ def upsample_by_interpolation(topk_idx, query, node, features):
     grad."""
     _check_interp_args(topk_idx, query, node, features)
     return _Interpolation.apply(topk_idx, query, node, features)
+
+
+KNN_MAX_K = 32
+KNN_MAX_NODES = 2048
+
+
+def _check_device(tensors, device):
+    for t, name in tensors:
+        if not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor/variable")
+        if not t.is_contiguous():
+            raise RuntimeError(f"{name} must be contiguous")
+        if t.device != device:
+            raise RuntimeError(f"{name} must be on {device}")
+
+
+def _check_pool_args(features, min_idx, M):
+    """Shape, dtype and bound checks first (they need no device), then device and layout."""
+    for t, name in ((features, "features"), (min_idx, "min_idx")):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor")
+    if features.dtype != torch.float32:
+        raise RuntimeError(f"features must have dtype {torch.float32}")
+    if min_idx.dtype != torch.int32:
+        raise RuntimeError(f"min_idx must have dtype {torch.int32}")
+    if features.dim() != 3 or min_idx.dim() != 2 or min_idx.shape[0] != features.shape[0] \
+            or min_idx.shape[1] != features.shape[2]:
+        raise RuntimeError("features must be [B,C,N] and min_idx [B,N]")
+    if features.shape[2] < 1:
+        raise RuntimeError("features: need N >= 1")
+    if isinstance(M, bool) or int(M) != M or M < 1:
+        raise RuntimeError(f"M must be an integer >= 1, got {M}")
+    _check_device(((features, "features"), (min_idx, "min_idx")), features.device)
+
+
+class _ClusterMaxPool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, features, min_idx, M, broadcast):
+        lib = _native.load()
+        B, C, N = features.shape
+        dev = features.device
+        with torch.cuda.device(dev):
+            sel = torch.empty((B, C, M), dtype=torch.int32, device=dev)
+            mask = torch.empty((B, M), dtype=torch.float32, device=dev)
+            pooled = torch.empty((B, C, M), dtype=torch.float32, device=dev)
+            scattered = torch.empty((B, C, N), dtype=torch.float32, device=dev) if broadcast else None
+            if B:
+                rc = lib.cluster_pool_forward_f32(features.data_ptr(), min_idx.data_ptr(), B, C, N, M, sel.data_ptr(),
+                                                  mask.data_ptr(), pooled.data_ptr(),
+                                                  scattered.data_ptr() if broadcast and scattered.numel() else None,
+                                                  torch.cuda.current_stream().cuda_stream)
+                _native.check(rc, "cluster_pool_forward_f32")
+        ctx.set_materialize_grads(False)           # a missing pooled or scattered gradient stays None
+        ctx.save_for_backward(min_idx, sel, mask)
+        ctx.shape = (B, C, N, M)
+        return (pooled, scattered) if broadcast else pooled
+
+    @staticmethod
+    def backward(ctx, grad_pooled, grad_scattered=None):
+        if not ctx.needs_input_grad[0] or (grad_pooled is None and grad_scattered is None):
+            return None, None, None, None
+        min_idx, sel, mask = ctx.saved_tensors
+        B, C, N, M = ctx.shape
+        dev = sel.device
+        if grad_pooled is not None:
+            grad_pooled = grad_pooled.float().contiguous()
+        if grad_scattered is not None:
+            # any batch stride with (channel, point) strides (N, 1): a channel slice of a torch.cat gradient needs
+            # no copy
+            grad_scattered = grad_scattered.float()
+            if (C > 1 and grad_scattered.stride(1) != N) or (N > 1 and grad_scattered.stride(2) != 1):
+                grad_scattered = grad_scattered.contiguous()
+        lib = _native.load()
+        with torch.cuda.device(dev):
+            gF = torch.empty((B, C, N), dtype=torch.float32, device=dev)
+            if gF.numel():
+                stream = torch.cuda.current_stream().cuda_stream
+                ws, ws_bytes = None, 0
+                if grad_scattered is not None:
+                    ws = _backward_workspace(dev, stream, lib.cluster_pool_backward_workspace_bytes(B, C, N, M))
+                    ws_bytes = ws.numel()
+                gs_ptr = grad_scattered.data_ptr() if grad_scattered is not None else None
+                bstride = grad_scattered.stride(0) if grad_scattered is not None and B > 1 else 0
+                rc = lib.cluster_pool_backward_f32(grad_pooled.data_ptr() if grad_pooled is not None else None, gs_ptr,
+                                                   bstride, min_idx.data_ptr(), sel.data_ptr(), mask.data_ptr(), B, C,
+                                                   N, M, gF.data_ptr(), ws.data_ptr() if ws is not None else None,
+                                                   ws_bytes, stream)
+                _native.check(rc, "cluster_pool_backward_f32")
+        return gF, None, None, None
+
+
+def cluster_max_pool(features, min_idx, M, broadcast=False):
+    """SO-Net masked max-pool of PCEncoder.forward (models/networks_pc.py:88-104) in one op, with a deterministic
+    feature gradient (DESIGN.md 4.16).
+
+    features [B,C,N] float32 and min_idx [B,N] int32 (cluster_assign_forward's) CUDA, M >= 1 segments.  Returns pooled
+    [B,C,M] = features[b,c,sel] * mask[b,m], sel = index_max_forward(features, min_idx, M) and mask[b,m] = 1.0 where
+    some point has min_idx == m (else 0.0: an empty segment gives features[b,c,0] * 0.0, -0.0 or NaN included).  With
+    broadcast=True returns (pooled, scattered), scattered [B,C,N] = pooled[b,c,min_idx[b,n]].  A point whose min_idx
+    is outside [0, M) joins no segment, gets NaN in every channel of scattered and no share of the gradient.
+    Differentiable with respect to `features`: fp64 sums in an order fixed by the shape, no float atomics."""
+    _check_pool_args(features, min_idx, M)
+    return _ClusterMaxPool.apply(features, min_idx, int(M), bool(broadcast))
+
+
+def _check_knn_args(query, database, features, K):
+    """Shape, dtype, bound and autograd checks first (they need no device), then device and layout."""
+    for t, name in ((query, "query"), (database, "database"), (features, "features")):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor")
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name} must have dtype {torch.float32}")
+        if t.dim() != 3:
+            raise RuntimeError(f"{name} must have 3 dimensions")
+    B, N = database.shape[0], database.shape[2]
+    if query.shape[0] != B or query.shape[1] != 3 or database.shape[1] != 3 or features.shape[0] != B \
+            or features.shape[2] != N:
+        raise RuntimeError("query must be [B,3,M], database [B,3,N] and features [B,C,N]")
+    if isinstance(K, bool) or int(K) != K or not 1 <= K <= KNN_MAX_K:
+        raise RuntimeError(f"K: need 1 <= K <= {KNN_MAX_K}, got {K}")
+    if not 1 <= N <= KNN_MAX_NODES:
+        raise RuntimeError(f"database: need 1 <= N <= {KNN_MAX_NODES}, got {N}")
+    if K > N:
+        raise RuntimeError(f"K: need K <= N, got K = {K} and N = {N}")
+    if query.requires_grad or database.requires_grad:
+        raise RuntimeError("knn_group has no gradient with respect to query or database: detach them")
+    _check_device(((query, "query"), (database, "database"), (features, "features")), features.device)
+
+
+class _KnnGroup(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, query, database, features, K):
+        lib = _native.load()
+        B, C, N = features.shape
+        M = query.shape[2]
+        dev = features.device
+        with torch.cuda.device(dev):
+            idx = torch.empty((B, M, K), dtype=torch.int32, device=dev)
+            grouped = torch.empty((B, 3 + C, M, K), dtype=torch.float32, device=dev)
+            if idx.numel():
+                rc = lib.knn_group_forward_f32(query.data_ptr(), database.data_ptr(), features.data_ptr(), B, C, M, N,
+                                               K, idx.data_ptr(), grouped.data_ptr(),
+                                               torch.cuda.current_stream().cuda_stream)
+                _native.check(rc, "knn_group_forward_f32")
+        ctx.mark_non_differentiable(idx)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(idx)
+        ctx.shape = (B, C, M, N, K)
+        return idx, grouped
+
+    @staticmethod
+    def backward(ctx, grad_idx, grad_grouped):
+        if not ctx.needs_input_grad[2]:
+            return None, None, None, None
+        idx, = ctx.saved_tensors
+        B, C, M, N, K = ctx.shape
+        dev = idx.device
+        if grad_grouped is None:                   # grouped took no part in the loss: a zero gradient, not materialised
+            return None, None, None, None
+        # any batch stride with (row, query, neighbour) strides (M * K, K, 1).  There are always 3 + C >= 3 rows, so the
+        # row stride is checked whatever M and K are (at M = K = 1 a slice of a cat along dim 3 has row stride != 1)
+        grad_grouped = grad_grouped.float()
+        if grad_grouped.stride(1) != M * K or (M > 1 and grad_grouped.stride(2) != K) \
+                or (K > 1 and grad_grouped.stride(3) != 1):
+            grad_grouped = grad_grouped.contiguous()
+        lib = _native.load()
+        with torch.cuda.device(dev):
+            gF = torch.empty((B, C, N), dtype=torch.float32, device=dev)
+            if gF.numel():
+                stream = torch.cuda.current_stream().cuda_stream
+                ws = _backward_workspace(dev, stream, lib.knn_group_backward_workspace_bytes(B, C, M, N, K))
+                bstride = grad_grouped.stride(0) if B > 1 else 0
+                rc = lib.knn_group_backward_f32(grad_grouped.data_ptr() if M else None, bstride, idx.data_ptr(), B, C,
+                                                M, N, K, gF.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+                _native.check(rc, "knn_group_backward_f32")
+        return None, None, gF, None
+
+
+def knn_group(query, database, features, K):
+    """Node kNN grouping of GeneralKNNFusionModule.forward (models/layers_pc.py:793-807) in one op, with a
+    deterministic feature gradient (DESIGN.md 4.16).
+
+    query [B,3,M], database [B,3,N], features [B,C,N] float32 CUDA; 1 <= K <= 32, K <= N <= 2048.  Returns (knn_idx
+    [B,M,K] int32, grouped [B,3+C,M,K]): knn_idx holds the K nearest database nodes of each query, nearest first, by
+    cluster_assign's key (f32 ((dx*dx + dy*dy) + dz*dz) without fma, ties -> lower index, +inf after finite keys, NaN
+    after +inf); grouped rows 0-2 are database[idx] - query and rows 3 onward features[idx], the tensor
+    layers_pc.py:807 concatenates.  Differentiable with respect to `features` only (fp64 sums in an order fixed by the
+    shape, no float atomics); query and database must not require grad, as the reference detaches both."""
+    _check_knn_args(query, database, features, K)
+    return _KnnGroup.apply(query, database, features, int(K))

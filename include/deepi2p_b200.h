@@ -443,6 +443,44 @@ int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const 
                         dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * The point encoder's SO-Net cluster max-pool and node kNN grouping (models/networks_pc.py:88-111,
+ * models/layers_pc.py:793-807; SURVEY.md 8f N12).  DESIGN.md 4.16 states the contract.  [dev] pointers; 0 <= B <= 65535.
+ * Backwards: fp64 sums in an order fixed by the shape, rounded once to f32; no float atomics.
+ *
+ * cluster_pool_forward_f32: features [B][C][N] f32, min_idx [B][N] int32 (cluster_assign_forward's), N >= 1, M >= 1.
+ *   sel [B][C][M] int32 = index_max_forward(features, min_idx, M) (the same kernel); mask [B][M] f32 = 1.0f where some
+ *   point has min_idx == m, else 0.0f; pooled [B][C][M] = features[b][c][sel] * mask (one f32 multiply: an empty
+ *   segment gives features[b][c][0] * 0.0f); scattered [B][C][N] (NULL: not written) = pooled[b][c][min_idx[b][n]],
+ *   NaN for a point whose min_idx is outside [0, M) (it joins no segment).
+ * cluster_pool_backward_f32: grad_features [B][C][N] f32 = sum over m with sel[b][c][m] = n of mask[b][m] *
+ *   (grad_pooled[b][c][m] + sum over n' with min_idx[b][n'] = m of grad_scattered[b][c][n']), the inner sum in
+ *   ascending n' within fixed slices of n' and the slices in order, then the terms in ascending m.  grad_pooled
+ *   [B][C][M] contiguous and grad_scattered (element (b, c, n) at b * grad_scattered_batch_stride + c * N + n) may each
+ *   be NULL (a zero gradient).  sel and mask are the forward's.  workspace: [dev] 8-byte aligned, >=
+ *   cluster_pool_backward_workspace_bytes(B, C, N, M) when grad_scattered is given (fp64 slice partials), else unused.
+ * knn_group_forward_f32: query [B][3][M], database [B][3][N], features [B][C][N] f32; 1 <= N <= 2048, 1 <= K <= min(32,
+ *   N).  knn_idx [B][M][K] int32: the K nearest database nodes of each query, nearest first, by cluster_assign's key
+ *   (((dx*dx + dy*dy) + dz*dz) in f32 without fma, ties -> lower index, +inf after finite keys, NaN after +inf).
+ *   grouped [B][3 + C][M][K] f32: rows 0..2 database[idx] - query, rows 3.. features[idx].
+ * knn_group_backward_f32: grad_features [B][C][N] f32 = sum over (m, j) with knn_idx[b][m][j] = n of
+ *   grad_grouped[b][3 + c][m][j], in ascending (m, j) within fixed slices and the slices in order.  grad_grouped element
+ *   (b, r, m, j) at b * grad_batch_stride + (r * M + m) * K + j; rows 0..2 (the coordinates) are not read.  workspace:
+ *   [dev] 8-byte aligned, >= knn_group_backward_workspace_bytes(B, C, M, N, K) (fp64 slice partials).
+ * ------------------------------------------------------------------------------------------ */
+int cluster_pool_forward_f32(const float* features, const int32_t* min_idx, int B, int C, int N, int M, int32_t* sel,
+                             float* mask, float* pooled, float* scattered, dib_stream_t stream);
+size_t cluster_pool_backward_workspace_bytes(int B, int C, int N, int M);
+int cluster_pool_backward_f32(const float* grad_pooled, const float* grad_scattered, int64_t grad_scattered_batch_stride,
+                              const int32_t* min_idx, const int32_t* sel, const float* mask, int B, int C, int N, int M,
+                              float* grad_features, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+int knn_group_forward_f32(const float* query, const float* database, const float* features, int B, int C, int M,
+                          int N, int K, int32_t* knn_idx, float* grouped, dib_stream_t stream);
+size_t knn_group_backward_workspace_bytes(int B, int C, int M, int N, int K);
+int knn_group_backward_f32(const float* grad_grouped, int64_t grad_batch_stride, const int32_t* knn_idx, int B, int C,
+                           int M, int N, int K, float* grad_features, void* workspace, size_t workspace_bytes,
+                           dib_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * The image side of classifier batches (data/kitti_pc_img_pose_loader.py:326-349,360-362,439-440,
  * data/oxford_pc_img_pose_loader.py:238-259,300-301,368; SURVEY.md 8f N10).  DESIGN.md 4.13 states the contract.
  * For each of S samples: rows [row0, row0 + rows) of an h x w x 3 uint8 frame (HWC, packed at src + offsets[s]),
