@@ -32,6 +32,7 @@ EXPORTS = (
     "classifier_loss_workspace_bytes", "classifier_loss_forward_f32", "classifier_loss_backward_f32",
     "cluster_pool_forward_f32", "cluster_pool_backward_workspace_bytes", "cluster_pool_backward_f32",
     "knn_group_forward_f32", "knn_group_backward_workspace_bytes", "knn_group_backward_f32",
+    "attn_fusion_forward_f32", "attn_fusion_backward_f32",
 )
 
 
@@ -216,6 +217,10 @@ def load():
     lib.knn_group_backward_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
     lib.knn_group_backward_f32.restype = i32
     lib.knn_group_backward_f32.argtypes = [vp, _c.c_int64, vp, i32, i32, i32, i32, i32, vp, vp, sz, vp]
+    lib.attn_fusion_forward_f32.restype = i32
+    lib.attn_fusion_forward_f32.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp]
+    lib.attn_fusion_backward_f32.restype = i32
+    lib.attn_fusion_backward_f32.argtypes = [vp, _c.c_int64, vp, vp, i32, i32, i32, i32, vp, vp, vp]
     _lib = lib
     return lib
 

@@ -431,3 +431,84 @@ def knn_group(query, database, features, K):
     shape, no float atomics); query and database must not require grad, as the reference detaches both."""
     _check_knn_args(query, database, features, K)
     return _KnnGroup.apply(query, database, features, int(K))
+
+
+FUSION_MAX_BATCH = 65535
+FUSION_MAX_ROWS = 32 * 65535      # C and P: 65535 row tiles of 32 in the kernel's grid
+
+
+def _check_fusion_args(img_features, attention):
+    """Type, dimension, dtype, shape and bound checks first (they need no device), then device and layout."""
+    for t, name in ((img_features, "img_features"), (attention, "attention")):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor")
+        if t.dim() != 3:
+            raise RuntimeError(f"{name} must have 3 dimensions")
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name} must have dtype {torch.float32}")
+    B, C, P = img_features.shape
+    M = attention.shape[2]
+    if attention.shape[0] != B or attention.shape[1] != P:
+        raise RuntimeError("img_features must be [B,C,P] and attention [B,P,M]")
+    if not 1 <= B <= FUSION_MAX_BATCH:
+        raise RuntimeError(f"img_features: need 1 <= B <= {FUSION_MAX_BATCH}, got {B}")
+    if min(C, P, M) < 1:
+        raise RuntimeError(f"need C, P, M >= 1, got C = {C}, P = {P}, M = {M}")
+    if max(C, P) > FUSION_MAX_ROWS or M > 2 ** 31 - 1:
+        raise RuntimeError(f"need C, P <= {FUSION_MAX_ROWS} and M < 2^31, got C = {C}, P = {P}, M = {M}")
+    _check_device(((img_features, "img_features"), (attention, "attention")), img_features.device)
+
+
+class _AttentionFusion(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, img_features, attention):
+        lib = _native.load()
+        B, C, P = img_features.shape
+        M = attention.shape[2]
+        dev = img_features.device
+        with torch.cuda.device(dev):
+            out = torch.empty((B, C, M), dtype=torch.float32, device=dev)
+            rc = lib.attn_fusion_forward_f32(img_features.data_ptr(), attention.data_ptr(), B, C, P, M, out.data_ptr(),
+                                             torch.cuda.current_stream().cuda_stream)
+        _native.check(rc, "attn_fusion_forward_f32")
+        ctx.set_materialize_grads(False)           # a missing output gradient stays None
+        ctx.save_for_backward(img_features, attention)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        need_F, need_A = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if grad_out is None or not (need_F or need_A):
+            return None, None
+        F, A = ctx.saved_tensors
+        B, C, P = F.shape
+        M = A.shape[2]
+        dev = F.device
+        # any batch stride with (channel, node) strides (M, 1): a channel slice of a torch.cat gradient needs no copy
+        grad_out = grad_out.float()
+        if (C > 1 and grad_out.stride(1) != M) or (M > 1 and grad_out.stride(2) != 1):
+            grad_out = grad_out.contiguous()
+        lib = _native.load()
+        with torch.cuda.device(dev):
+            gF = torch.empty((B, C, P), dtype=torch.float32, device=dev) if need_F else None
+            gA = torch.empty((B, P, M), dtype=torch.float32, device=dev) if need_A else None
+            bstride = grad_out.stride(0) if B > 1 else 0
+            rc = lib.attn_fusion_backward_f32(grad_out.data_ptr(), bstride, F.data_ptr(), A.data_ptr(), B, C, P, M,
+                                              gF.data_ptr() if need_F else None, gA.data_ptr() if need_A else None,
+                                              torch.cuda.current_stream().cuda_stream)
+        _native.check(rc, "attn_fusion_backward_f32")
+        return gF, gA
+
+
+def attention_fusion(img_features, attention):
+    """Attention-weighted image features of KeypointDetector.forward (models/networks_united.py:149-150,172-174,
+    torch.mean(img_features.unsqueeze(3) * attention.unsqueeze(1), dim=2)) without its B x C x P x M product
+    (DESIGN.md 4.17).
+
+    img_features [B,C,P] (the feature map's .view(B, C, -1)) and attention [B,P,M] float32 CUDA, contiguous, on one
+    device.  Returns out [B,C,M], out[b,c,m] = float((sum over p ascending of F[b,c,p] * A[b,p,m]) / P), one fp64
+    accumulator per output over the exact products, so the result does not depend on tiling, batch composition or the
+    TF32 flags.  Differentiable with respect to both inputs with the same rule (sums over m for img_features, over c
+    for attention); an input that needs no gradient costs nothing in the backward."""
+    _check_fusion_args(img_features, attention)
+    return _AttentionFusion.apply(img_features, attention)

@@ -481,6 +481,27 @@ int knn_group_backward_f32(const float* grad_grouped, int64_t grad_batch_stride,
                            dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * The classifier's attention-weighted image-feature fusion (models/networks_united.py:149-150,172-174,
+ * torch.mean(F.unsqueeze(3) * A.unsqueeze(1), dim=2); SURVEY.md 8f N13).  DESIGN.md 4.17 states the contract.  [dev]
+ * pointers; 1 <= B <= 65535, C, P, M >= 1, C and P <= 2097120.  Every sum has one fp64 accumulator starting at +0.0
+ * and adds the exact products of f32 operands in ascending order; the sum divided by P in fp64 is rounded once to
+ * f32.  No atomics, no workspace: bit-identical across runs, streams and batch compositions.
+ *
+ * attn_fusion_forward_f32: img_features F [B][C][P] and attention A [B][P][M] f32, contiguous.  out [B][C][M] =
+ *   float((sum over p ascending of F[b][c][p] * A[b][p][m]) / P).
+ * attn_fusion_backward_f32: grad_out gO element (b, c, m) at b * grad_batch_stride + c * M + m (grad_batch_stride >= 0;
+ *   a channel slice of a larger [B][C'][M] tensor passes C' * M).  grad_img_features [B][C][P] = float((sum over m
+ *   ascending of gO[b][c][m] * A[b][p][m]) / P) and grad_attention [B][P][M] = float((sum over c ascending of
+ *   F[b][c][p] * gO[b][c][m]) / P); either may be NULL (not computed), and then the operand only it reads (attention
+ *   for grad_img_features, img_features for grad_attention) may be NULL too.
+ * ------------------------------------------------------------------------------------------ */
+int attn_fusion_forward_f32(const float* img_features, const float* attention, int B, int C, int P, int M, float* out,
+                            dib_stream_t stream);
+int attn_fusion_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* img_features,
+                             const float* attention, int B, int C, int P, int M, float* grad_img_features,
+                             float* grad_attention, dib_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * The image side of classifier batches (data/kitti_pc_img_pose_loader.py:326-349,360-362,439-440,
  * data/oxford_pc_img_pose_loader.py:238-259,300-301,368; SURVEY.md 8f N10).  DESIGN.md 4.13 states the contract.
  * For each of S samples: rows [row0, row0 + rows) of an h x w x 3 uint8 frame (HWC, packed at src + offsets[s]),

@@ -80,6 +80,15 @@ if which in ("all", "ops"):
         _native.check(f(x.data_ptr(), cnt.data_ptr(), 65536, 3, 150, st.data_ptr(), fi.data_ptr(), fn_.data_ptr(),
                         torch.cuda.current_stream().cuda_stream), "fps_batch")
         print("fps cluster, empty slices", dt, fi[:, :4].tolist())
+    # image-attention fusion: ragged 32 x 32 tiles (forward, both gradients) and ragged 64 x 64 tiles, with a gradient
+    # that is a channel slice of a torch.cat
+    for B_, C_, P_, M_ in ((2, 33, 50, 129), (6, 700, 333, 450)):
+        Ff = torch.randn(B_, C_, P_, device="cuda", requires_grad=True)
+        Af = torch.randn(B_, P_, M_, device="cuda", requires_grad=True)
+        of = point_ops.attention_fusion(Ff, Af)
+        torch.cat((of, torch.zeros_like(of)), dim=1).backward(torch.ones(B_, 2 * C_, M_, device="cuda"))
+        print("attention_fusion", (B_, C_, P_, M_), of.abs().sum().item(), Ff.grad.abs().sum().item(),
+              Af.grad.abs().sum().item())
 if which in ("all", "pnp"):
     from deepi2p_b200 import pnp
     fines = [syn.make_fine_labels(s, seed=i) for i, s in enumerate(smps)]
