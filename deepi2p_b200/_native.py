@@ -24,7 +24,7 @@ EXPORTS = (
     "pnp_ransac_workspace_bytes", "pnp_ransac_batch_f32", "epnp_batch_f64",
     "icp_workspace_bytes", "icp_register_batch_f32", "icp_register_batch_counted_f32", "icp_build_index_f32",
     "voxel_downsample_workspace_bytes", "voxel_downsample_batch_f32", "estimate_normals_workspace_bytes",
-    "estimate_normals_batch_f32", "nearest_batch_f32",
+    "estimate_normals_batch_f32", "nearest_batch_f32", "sym3_eig_batch_f64",
     "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32", "assemble_resample_workspace_bytes",
     "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
     "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
@@ -166,6 +166,8 @@ def load():
     lib.estimate_normals_batch_f32.argtypes = [vp, vp, i32, i32, f64, i32, vp, vp, vp, vp, sz, vp]
     lib.nearest_batch_f32.restype = i32
     lib.nearest_batch_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp, sz, vp]
+    lib.sym3_eig_batch_f64.restype = i32
+    lib.sym3_eig_batch_f64.argtypes = [vp, i32, vp, vp, vp]
     lib.assemble_accumulate_workspace_bytes.restype = sz
     lib.assemble_accumulate_workspace_bytes.argtypes = [i32, i32, i32]
     lib.assemble_accumulate_f32.restype = i32

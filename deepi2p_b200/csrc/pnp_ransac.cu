@@ -318,6 +318,16 @@ __device__ bool warp_epnp(const Pts<T>& P, const Cam& c, Scratch* w, double out[
   const double C[9] = {cov[0], cov[1], cov[2], cov[1], cov[3], cov[4], cov[2], cov[4], cov[5]};
   double lam[3], E[9], sc[3];
   sym3_eig_desc(C, lam, E);
+  // A coplanar or collinear set has lam[2] = 0, so the computed lam[2] is rounding noise and the fourth control point
+  // has an arbitrary depth: EPnP then returns wrong poses as valid.  Each entry of C is a sum of
+  // m + 5 additions (m = ceil(n / 32) terms per lane, then the 5-level butterfly) of terms dx dy carrying 3 roundings,
+  // so |dC_ij| <= gamma_{m+8} sum |dx_i dx_j| and ||dC||_2 <= 9 gamma_{m+8} lam[0]; the Jacobi eigenvalues of C add
+  // at most 52 u lam[0] (30 u ||C||_F, ||C||_F <= sqrt(3) lam[0]).  By Weyl's inequality a computed lam[2] at or
+  // below that sum cannot be told from 0, and the set is rejected (DESIGN.md 4.8).  u = 2^-53.  lam[0] >= 1e75 (a
+  // spread above about 1e37) is rejected too: the Jacobi sweeps on C and on kabsch()'s H^T H (of the order of C^2)
+  // sum the squares of their entries, which would overflow and end the sweeps before the first rotation.
+  const double tol = (9.0 * (double)((n + 31) / 32 + 8) + 52.0) * 0x1p-53;
+  if (!(lam[2] > tol * lam[0]) || !(lam[0] < 1e75)) return false;
   for (int k = 0; k < 3; ++k) {
     sc[k] = sqrt(lam[k] / n);
     if (!(sc[k] > 0.0) || !isfinite(sc[k])) return false;

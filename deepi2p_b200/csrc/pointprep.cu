@@ -412,6 +412,18 @@ int nearest_batch(const double* q, const int32_t* q_pts, int q_stride, const flo
   return DIB_OK;
 }
 
+// Test hook: sym3_eig_desc on n independent 3x3 matrices, one thread each, compiled as its callers are (--fmad=false).
+__global__ void __launch_bounds__(128) sym3_eig_kernel(const double* __restrict__ C, int n, double* __restrict__ lam,
+                                                       double* __restrict__ E) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  double c[9], l[3], e[9];
+  for (int q = 0; q < 9; ++q) c[q] = C[(size_t)t * 9 + q];
+  sym3_eig_desc(c, l, e);
+  for (int q = 0; q < 3; ++q) lam[(size_t)t * 3 + q] = l[q];
+  for (int q = 0; q < 9; ++q) E[(size_t)t * 9 + q] = e[q];
+}
+
 }  // namespace prep
 }  // namespace dib
 
@@ -447,6 +459,15 @@ int nearest_batch_f32(const double* q, const int32_t* q_pts, int q_stride, const
                       dib_stream_t stream) {
   return dib::prep::nearest_batch(q, q_pts, q_stride, xyz, m_pts, m_stride, S, idx_out, workspace, workspace_bytes,
                                   (cudaStream_t)stream);
+}
+
+int sym3_eig_batch_f64(const double* C, int n, double* lam, double* E, dib_stream_t stream) {
+  DIB_REQUIRE(C && lam && E, "NULL argument (C, lam, E)");
+  DIB_REQUIRE(n >= 0, "bad sizes (n=%d)", n);
+  if (n == 0) return DIB_OK;
+  dib::prep::sym3_eig_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(C, n, lam, E);
+  DIB_CHECK_CUDA(cudaGetLastError());
+  return DIB_OK;
 }
 
 }  // extern "C"

@@ -39,8 +39,9 @@ def pnp_ransac_batch(xyz, coarse_pred, fine_pred, n_pts, K, H, W, scale=1 / 32.0
     scale-W x scale-H grid), n_pts [S] int32 or None (= Ns), all on one CUDA device; K [3,3] or [S,3,3] (unscaled).
     Returns dict(P [S,4,4] f64, outlier_ratio [S] f64, inliers [S] i32, n_sel [S] i32, hyp_used [S] i32) and, with
     return_all, inlier_mask [S,Ns] u8, hyp_pose [S,iterations,12] f64 (R row-major | t), hyp_inliers [S,iterations]
-    i32 (entries at h >= hyp_used unspecified).  `out`: the dict of an earlier call with the same shapes; its tensors
-    are overwritten in place."""
+    i32 (entries at h >= hyp_used unspecified: zero or a scored hypothesis past the stop in a new dict, kept from the
+    earlier call with `out`).  `out`: the dict of an earlier call with the same shapes; its tensors are overwritten in
+    place."""
     _require_cuda()
     lib = _native.load()
     S, Ns = _check_frames(xyz, coarse_pred, fine_pred, n_pts)
@@ -61,6 +62,12 @@ def pnp_ransac_batch(xyz, coarse_pred, fine_pred, n_pts, K, H, W, scale=1 / 32.0
             res = out
         else:
             res = {k: torch.empty(shp, dtype=dt, device=dev) for k, (shp, dt) in shapes.items()}
+            if return_all:
+                # a frame that stops early never writes the tail of its hypothesis rows; zeroed, it does not carry
+                # whatever the allocator handed out, so two identical calls return identical arrays
+                with torch.cuda.stream(stream):
+                    res["hyp_pose"].zero_()
+                    res["hyp_inliers"].zero_()
         sp = _stream_ptr(stream)
         ws = _workspace(max(lib.pnp_ransac_workspace_bytes(S, Ns, max(iterations, 1)), 1), dev, sp)
         rc = lib.pnp_ransac_batch_f32(

@@ -139,6 +139,23 @@ def nearest(q, q_pts, xyz, m_pts, stream=None):
     return idx
 
 
+def sym3_eig_batch(C):
+    """Test hook: the 3x3 symmetric eigensolver of the normals and of EPnP (csrc/sym3_eig.cuh) on each matrix of C
+    [n,3,3] (numpy, read as given).  Returns (lam [n,3] descending, E [n,3,3] with column k the eigenvector of lam[k])
+    as numpy float64."""
+    _require_cuda()
+    lib = _native.load()
+    C = np.ascontiguousarray(np.asarray(C, dtype=np.float64).reshape(-1, 9))
+    n = C.shape[0]
+    dev = torch.device("cuda")
+    tC = torch.from_numpy(C).to(dev)
+    lam = torch.zeros((n, 3), dtype=torch.float64, device=dev)
+    E = torch.zeros((n, 9), dtype=torch.float64, device=dev)
+    rc = lib.sym3_eig_batch_f64(_ptr(tC), n, _ptr(lam), _ptr(E), _stream_ptr())
+    _native.check(rc, "sym3_eig_batch_f64")
+    return lam.cpu().numpy(), E.cpu().numpy().reshape(n, 3, 3)
+
+
 def prepare_scans(xyz, intensity, n_pts, voxel_size=VOXEL_SIZE, sn_radius=SN_RADIUS, sn_max_nn=SN_MAX_NN,
                   orient=(0.0, 0.0, 1.0), stream=None):
     """kitti_pc_bin_to_npy_with_downsample_sn.py:48-74 for S scans: voxel_down_sample(voxel_size), estimate_normals

@@ -356,6 +356,9 @@ int icp_build_index_f32(const float* tgt, const int32_t* m_pts, int m_stride, in
  *   [S][3][m_stride] f32 (d2 as above, ties -> lowest index; -1 for an empty cloud or d2 >= DBL_MAX / 2) into idx_out
  *   [S][q_stride] i32.
  *   workspace >= estimate_normals_workspace_bytes(S, m_stride).
+ * sym3_eig_batch_f64 (test hook): the 3x3 symmetric eigensolver that the normals and EPnP share, on n matrices C
+ *   [n][9] f64 row-major (read as given, not symmetrised) -> eigenvalues lam [n][3] in descending order and
+ *   eigenvectors E [n][9] (row-major, column k belongs to lam[k]), all [dev].
  * ------------------------------------------------------------------------------------------ */
 size_t voxel_downsample_workspace_bytes(int S, int n_stride, int C);
 int voxel_downsample_batch_f32(const float* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
@@ -368,6 +371,7 @@ int estimate_normals_batch_f32(const float* xyz, const int32_t* m_pts, int m_str
 int nearest_batch_f32(const double* q, const int32_t* q_pts, int q_stride, const float* xyz, const int32_t* m_pts,
                       int m_stride, int S, int32_t* idx_out, void* workspace, size_t workspace_bytes,
                       dib_stream_t stream);
+int sym3_eig_batch_f64(const double* C, int n, double* lam, double* E, dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Batch assembly of the classifier's point inputs (the loaders' __getitem__ after the scan records are read:

@@ -40,6 +40,8 @@ def _load():
         lib.pnp_oracle_sample.argtypes = [i32, i32, i32, ctypes.c_uint64, vp]
         lib.pnp_oracle_update_niters.restype = i32
         lib.pnp_oracle_update_niters.argtypes = [i32, i32, i32, f64]
+        lib.pnp_oracle_sym3_eig.restype = None
+        lib.pnp_oracle_sym3_eig.argtypes = [vp, i32, vp, vp]
         lib.pnp_oracle_epnp.restype = i32
         lib.pnp_oracle_epnp.argtypes = [vp, vp, i32, vp, vp]
         lib.pnp_oracle_frame.restype = i32
@@ -62,6 +64,16 @@ def sample(h, s, n, seed):
 
 def update_niters(niters, cnt, n, confidence=0.99):
     return int(_load().pnp_oracle_update_niters(niters, cnt, n, confidence))
+
+
+def sym3_eig(C):
+    """The 3x3 Jacobi eigensolver shared by EPnP and the normals on each matrix of C [n,3,3] (read as given).  Returns
+    (lam [n,3] descending, E [n,3,3], column k the eigenvector of lam[k])."""
+    C = np.ascontiguousarray(np.asarray(C, dtype=np.float64).reshape(-1, 9))
+    lam = np.zeros((C.shape[0], 3))
+    E = np.zeros((C.shape[0], 9))
+    _load().pnp_oracle_sym3_eig(_ptr(C), C.shape[0], _ptr(lam), _ptr(E))
+    return lam, E.reshape(-1, 3, 3)
 
 
 def epnp(xyz, uv, K):

@@ -273,6 +273,10 @@ bool epnp(const Frame& f, const int* idx, int n, const Cam& c, double out[12]) {
   }
   double lam[3], E[9];
   sym3_eig_desc(C, lam, E);
+  // Coplanar (and collinear) sets: lam[2] within the rounding bound of lam[0] -> degenerate; a spread whose squares
+  // would overflow the Jacobi sweeps -> rejected (DESIGN.md 4.8).
+  const double tol = (9.0 * (double)((n + 31) / 32 + 8) + 52.0) * 0x1p-53;
+  if (!(lam[2] > tol * lam[0]) || !(lam[0] < 1e75)) return false;
   double sc[3];
   for (int k = 0; k < 3; ++k) {
     sc[k] = std::sqrt(lam[k] / n);
@@ -504,6 +508,11 @@ int pnp_oracle_update_niters(int niters, int cnt, int n, double confidence) {
   if (!(den < 0.0)) return niters;                      // 1 - w^5 rounds to 1: no bound
   const double k = std::ceil(std::log(1.0 - confidence) / den);
   return k < (double)niters ? (int)k : niters;
+}
+
+// sym3_eig_desc on n matrices C [n][9] -> lam [n][3], E [n][9] (the kernels' sym3_eig_batch_f64).
+void pnp_oracle_sym3_eig(const double* C, int n, double* lam, double* E) {
+  for (int t = 0; t < n; ++t) sym3_eig_desc(C + 9 * (size_t)t, lam + 3 * (size_t)t, E + 9 * (size_t)t);
 }
 
 // EPnP on n packed correspondences (xyz [n][3], uv [n][2], K9 unscaled row-major). Returns 1 on success.
