@@ -258,6 +258,55 @@ def write_icp_handoff(data_dir, monodepth_dir, seeds, shape="oxford"):
     return frames
 
 
+def seeded_state_dict(model, seed):
+    """Seeded weights for a network's state_dict, the same on every machine (numpy draws in sorted key order):
+    convolution and linear weights N(0, 1 / fan_in), other weights (the norms') 1 + N(0, 0.1^2), biases and running
+    means N(0, 0.1^2), running variances U(0.5, 1.5); num_batches_tracked is kept.  Returns a dict of CPU tensors
+    with the dtypes of `model.state_dict()`."""
+    import torch
+    rng = np.random.default_rng(seed)
+    out = {}
+    ref = model.state_dict()
+    for k in sorted(ref):
+        v = ref[k]
+        if k.endswith("num_batches_tracked"):
+            out[k] = v.detach().cpu().clone()
+            continue
+        shape = tuple(v.shape)
+        if k.endswith("running_var"):
+            a = rng.uniform(0.5, 1.5, shape)
+        elif k.endswith(".weight") and len(shape) > 1:
+            a = rng.standard_normal(shape) / math.sqrt(int(np.prod(shape[1:])))
+        elif k.endswith(".weight"):
+            a = 1.0 + 0.1 * rng.standard_normal(shape)
+        else:
+            a = 0.1 * rng.standard_normal(shape)
+        out[k] = torch.from_numpy(np.asarray(a, dtype=np.float64)).to(v.dtype)
+    return out
+
+
+def make_network_inputs(seed, B=2, N=2048, Ma=128, Mb=128, H=64, W=128, L=8):
+    """Seeded classifier-network inputs (numpy float32): pc, node_a, node_b uniform in a 40 x 6 x 40 m box (drawn
+    independently, so no node coincides with a point), intensity U(0, 1), unit normals sn, img U(0, 1) [B,3,H,W], and
+    the weights of a linear test loss lw_coarse [B,2,N], lw_fine [B,L,N] ~ N(0, 1)."""
+    rng = np.random.default_rng(seed)
+
+    def cloud(n):
+        return np.stack([rng.uniform(-20, 20, (B, n)), rng.uniform(-3, 3, (B, n)),
+                         rng.uniform(-20, 20, (B, n))], 1).astype(np.float32)
+    sn = rng.standard_normal((B, 3, N))
+    sn = (sn / np.linalg.norm(sn, axis=1, keepdims=True)).astype(np.float32)
+    pc = cloud(N)
+    intensity = rng.uniform(0, 1, (B, 1, N)).astype(np.float32)
+    node_a, node_b = cloud(Ma), cloud(Mb)
+    img = rng.uniform(0, 1, (B, 3, H, W)).astype(np.float32)
+    rng = np.random.default_rng(seed + 1)
+    lw_coarse = rng.standard_normal((B, 2, N)).astype(np.float32)
+    lw_fine = rng.standard_normal((B, L, N)).astype(np.float32)
+    return dict(pc=pc, intensity=intensity, sn=sn, node_a=node_a, node_b=node_b, img=img, lw_coarse=lw_coarse,
+                lw_fine=lw_fine)
+
+
 def make_index_max_inputs(seed, B=64, C=64, N=16384, K=64):
     rng = np.random.default_rng(seed)
     data = rng.standard_normal((B, C, N), dtype=np.float32)
