@@ -32,7 +32,7 @@ EXPORTS = (
     "classifier_loss_workspace_bytes", "classifier_loss_forward_f32", "classifier_loss_backward_f32",
     "cluster_pool_forward_f32", "cluster_pool_backward_workspace_bytes", "cluster_pool_backward_f32",
     "knn_group_forward_f32", "knn_group_backward_workspace_bytes", "knn_group_backward_f32",
-    "attn_fusion_forward_f32", "attn_fusion_backward_f32",
+    "attn_fusion_forward_f32", "attn_fusion_backward_f32", "jpeg_decode_workspace_bytes", "jpeg_decode_batch_u8",
 )
 
 
@@ -223,6 +223,10 @@ def load():
     lib.attn_fusion_forward_f32.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp]
     lib.attn_fusion_backward_f32.restype = i32
     lib.attn_fusion_backward_f32.argtypes = [vp, _c.c_int64, vp, vp, i32, i32, i32, i32, vp, vp, vp]
+    lib.jpeg_decode_workspace_bytes.restype = sz
+    lib.jpeg_decode_workspace_bytes.argtypes = [vp, i32, sz, i32]
+    lib.jpeg_decode_batch_u8.restype = i32
+    lib.jpeg_decode_batch_u8.argtypes = [vp, sz, vp, vp, vp, i32, i32, vp, sz, vp, vp, sz, vp]
     _lib = lib
     return lib
 

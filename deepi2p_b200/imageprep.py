@@ -3,7 +3,9 @@ ColorJitter on a PIL image, column flip, CHW float conversion and the K updates 
 326-349,360-362,439-440, data/oxford_pc_img_pose_loader.py:238-259,300-301,368, and the same steps of the nuScenes
 loader), for S samples at once and bit for bit against cv2 and Pillow.
 
-pack_images packs ragged HWC uint8 frames into one device buffer; image_params draws the per-sample crop offsets and
+pack_images packs ragged HWC uint8 frames into one device buffer, and decode_jpeg_batch / read_jpeg_batch decode the
+loaders' JPEG frames (Image.open(path).convert("RGB"), bit for bit; csrc/jpeg.cu, DESIGN.md 4.19) into the same
+buffer on the device; image_params draws the per-sample crop offsets and
 jitter on the host; assemble_images runs csrc/imageprep.cu and composes K in fp64.  kitti_image_args /
 oxford_image_args are the two loaders' options; nuScenes is crop_top_rows=100, img_scale=0.2, 160 x 320,
 jitter_prob=0.5.  augment_img is a host drop-in for the loaders' augment_img that works on current torchvision.
@@ -13,6 +15,7 @@ import numpy as np
 import torch
 
 from . import _native
+from . import jpeg as _jpeg
 from .assemble import MODES
 from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace
 
@@ -64,6 +67,65 @@ def pack_images(images, device="cuda"):
     flat = np.concatenate([a.reshape(-1) for a in arrs]) if arrs else np.zeros(0, np.uint8)
     return dict(data=torch.from_numpy(flat).to(torch.device(device)), offsets=offsets,
                 shapes=np.array([a.shape[:2] for a in arrs], dtype=np.int64).reshape(-1, 2))
+
+
+JPEG_WINDOW_BITS = 8192          # bit length of the windows the Huffman decoder synchronises (csrc/jpeg.cu)
+
+
+def decode_jpeg_batch(blobs, device="cuda", stream=None, *, _window_bits=None):
+    """Decode S JPEG streams (bytes-like) on the GPU into pack_images' dict: data uint8 [sum 3 h w] on `device`
+    (HWC RGB, each image equal to np.asarray(PIL.Image.open(BytesIO(b)).convert("RGB")) on Pillow 12.2 /
+    libjpeg-turbo), offsets int64 [S], shapes int64 [S,2] (h, w), so assemble_images takes it as it is.
+
+    Supported: 8-bit baseline / extended sequential Huffman, one scan of 1 (grey, replicated to RGB) or 3 (YCbCr)
+    components, 4:4:4 / 4:2:2 / 4:2:0 / 4:4:0, any Huffman tables, restart intervals, any size.  Anything else --
+    progressive, arithmetic, lossless, 12-bit, multi-scan, CMYK / YCCK, RGB-coded, other sampling factors -- and a
+    truncated or corrupt entropy-coded segment raise ValueError("image i: <reason>"); the whole call raises, and no
+    output is returned for any image.  Corrupt data that still decodes validly is not detected.  The call waits for
+    the decode to finish (the per-image status is read back).  _window_bits is a test hook: the synchronisation
+    window length in bits."""
+    _require_cuda()
+    lib = _native.load()
+    dev = torch.device(device)
+    S = len(blobs)
+    pk = _jpeg.pack_batch(blobs)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):
+        out = torch.empty(pk["out_bytes"], dtype=torch.uint8, device=dev)
+        if S:
+            wb = int(_window_bits) if _window_bits is not None else JPEG_WINDOW_BITS
+            sp = _stream_ptr(stream)
+            data = torch.from_numpy(pk["data"]).to(dev) if pk["data"].size else torch.zeros(1, dtype=torch.uint8, device=dev)
+            huff = torch.from_numpy(pk["huff"]).to(dev, non_blocking=True)
+            quant = torch.from_numpy(pk["quant"]).to(dev, non_blocking=True)
+            status = torch.zeros((S, 2), dtype=torch.int32, device=dev)
+            desc = np.ascontiguousarray(pk["desc"])
+            nws = lib.jpeg_decode_workspace_bytes(desc.ctypes.data, S, pk["data"].size, wb)
+            if nws == 0:
+                raise _native.NativeError("jpeg_decode_workspace_bytes rejected the batch")
+            ws = _workspace(nws, dev, sp)
+            rc = lib.jpeg_decode_batch_u8(_ptr(data), pk["data"].size, desc.ctypes.data, _ptr(huff), _ptr(quant), S, wb,
+                                          _ptr(out), out.numel(), _ptr(status), _ptr(ws), ws.numel(), sp)
+            _native.check(rc, "jpeg_decode")
+            st = status.cpu().numpy()
+            bad = np.flatnonzero(st[:, 0])
+            if bad.size:
+                i = int(bad[0])
+                raise ValueError(f"image {i}: {_jpeg.STATUS.get(int(st[i, 0]), f'status {int(st[i, 0])}')}")
+            decode_jpeg_batch.last_rounds = st[:, 1].copy()
+    return dict(data=out, offsets=pk["offsets"], shapes=pk["shapes"])
+
+
+decode_jpeg_batch.last_rounds = np.zeros(0, np.int32)
+
+
+def read_jpeg_batch(paths, device="cuda", stream=None):
+    """The loaders' Image.open(path).convert("RGB") for S JPEG files: reads the files on the host and decodes them
+    with decode_jpeg_batch."""
+    blobs = []
+    for p in paths:
+        with open(p, "rb") as f:
+            blobs.append(f.read())
+    return decode_jpeg_batch(blobs, device=device, stream=stream)
 
 
 def image_params(shapes, mode, rng=None, img_H=160, img_W=512, img_scale=0.5, crop_top_rows=0, crop_bottom_rows=0,

@@ -577,6 +577,38 @@ int classifier_loss_backward_f32(const float* coarse, int64_t coarse_batch_strid
                                  double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
                                  float* grad_coarse, float* grad_fine, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Batched JPEG decoding (the Oxford and nuScenes loaders' Image.open(<frame>.jpg)).  DESIGN.md 4.19 states the
+ * contract: 8-bit sequential Huffman streams with one scan of 1 or 3 components, decoded bit for bit as libjpeg-turbo
+ * does with its defaults (ISLOW IDCT, fancy upsampling) into HWC uint8 RGB, grey replicated to three channels.
+ * deepi2p_b200/jpeg.py parses the headers and fills the inputs.
+ *
+ * data: [dev] data_bytes bytes holding each image's entropy-coded data (from the byte after its SOS segment to
+ *   the end of the file).  desc: [host] int64 [S][DIB_JPEG_DESC]: slots 0..39 as csrc/jpeg.cu lists them (offsets
+ *   into data and out, size, restart interval, MCU grid and per-component sampling, block grid, downsampled size
+ *   and first block; slot 45 the component of each MCU block, 4 bits each); the other slots are the library's and are
+ *   ignored.  huff: [dev] int32 [S][6][DIB_JPEG_HUFF_WORDS] (DC, AC table of each component; jpeg.py
+ *   device_huff_table); quant: [dev] int32 [S][3][64] quantisers in natural order, as int16 values.
+ *   window_bits: the bit length, in [32, 2^20], of the windows the Huffman decoder synchronises (8192 is the
+ *   default; smaller values force more synchronisation work and exist for tests).  out: [dev] out_bytes bytes, image s at desc offset.
+ *   status: [dev] int32 [S][2]: DIB_JPEG_* code of image s, then the synchronisation rounds its decode took.  An image
+ *   with a non-zero code has no pixels written.  workspace: [dev] 256-byte aligned, >=
+ *   jpeg_decode_workspace_bytes(desc, S, data_bytes, window_bits) (0 for invalid descriptors).  Deterministic: no
+ *   atomics touch the output.
+ * ------------------------------------------------------------------------------------------ */
+#define DIB_JPEG_DESC 48
+#define DIB_JPEG_HUFF_WORDS 356
+#define DIB_JPEG_OK 0
+#define DIB_JPEG_TRUNCATED 1 /* the entropy-coded data has no ending marker                   */
+#define DIB_JPEG_MARKER 2    /* the data ends in a marker other than EOI (e.g. a second scan)  */
+#define DIB_JPEG_RESTARTS 3  /* the restart-marker count does not match the DRI               */
+#define DIB_JPEG_HUFFMAN 4   /* an invalid Huffman code                                       */
+#define DIB_JPEG_MCUS 5      /* an interval's data does not hold exactly its MCUs (truncated) */
+size_t jpeg_decode_workspace_bytes(const int64_t* desc, int S, size_t data_bytes, int window_bits);
+int jpeg_decode_batch_u8(const uint8_t* data, size_t data_bytes, const int64_t* desc, const int32_t* huff,
+                         const int32_t* quant, int S, int window_bits, uint8_t* out, size_t out_bytes,
+                         int32_t* status, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
