@@ -23,9 +23,11 @@ EXPORTS = (
     "cluster_assign_workspace_bytes", "cluster_assign_forward",
     "pnp_ransac_workspace_bytes", "pnp_ransac_batch_f32", "epnp_batch_f64",
     "icp_workspace_bytes", "icp_register_batch_f32", "icp_register_batch_counted_f32", "icp_build_index_f32",
-    "voxel_downsample_workspace_bytes", "voxel_downsample_batch_f32", "estimate_normals_workspace_bytes",
+    "voxel_downsample_workspace_bytes", "voxel_downsample_batch_f32", "voxel_downsample_batch_f64",
+    "estimate_normals_workspace_bytes",
     "estimate_normals_batch_f32", "nearest_batch_f32", "sym3_eig_batch_f64",
-    "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32", "assemble_resample_workspace_bytes",
+    "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32",
+    "assemble_accumulate_f64_workspace_bytes", "assemble_accumulate_f64", "assemble_resample_workspace_bytes",
     "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
     "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
     "interp_backward_f32", "image_assemble_workspace_bytes", "image_assemble_f32", "image_assemble_u8",
@@ -158,8 +160,9 @@ def load():
     lib.icp_build_index_f32.argtypes = [vp, vp, i32, i32, vp, sz, vp]
     lib.voxel_downsample_workspace_bytes.restype = sz
     lib.voxel_downsample_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.voxel_downsample_batch_f32.restype = i32
-    lib.voxel_downsample_batch_f32.argtypes = [vp, vp, i32, i32, vp, i32, f64, vp, vp, vp, vp, sz, vp]
+    for name in ("voxel_downsample_batch_f32", "voxel_downsample_batch_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i32, i32, vp, i32, f64, vp, vp, vp, vp, sz, vp]
     lib.estimate_normals_workspace_bytes.restype = sz
     lib.estimate_normals_workspace_bytes.argtypes = [i32, i32]
     lib.estimate_normals_batch_f32.restype = i32
@@ -173,6 +176,10 @@ def load():
     lib.assemble_accumulate_f32.restype = i32
     lib.assemble_accumulate_f32.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp, vp, i32, vp, vp, sz,
                                             vp]
+    lib.assemble_accumulate_f64_workspace_bytes.restype = sz
+    lib.assemble_accumulate_f64_workspace_bytes.argtypes = [i32, i32, i32]
+    lib.assemble_accumulate_f64.restype = i32
+    lib.assemble_accumulate_f64.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp, vp, i32, vp, vp, sz, vp]
     lib.assemble_resample_workspace_bytes.restype = sz
     lib.assemble_resample_workspace_bytes.argtypes = [i32, i32]
     lib.assemble_resample_f32.restype = i32

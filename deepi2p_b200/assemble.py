@@ -1,6 +1,7 @@
 """Classifier input batches on the GPU: the loaders' point side after the scan records are read (frame accumulation,
 the voxel step, downsample_np, augmentation, the camera transform and the farthest-point node sets of
-data/kitti_pc_img_pose_loader.py:199-446 and data/oxford_pc_img_pose_loader.py:262-352).
+data/kitti_pc_img_pose_loader.py:199-446, data/oxford_pc_img_pose_loader.py:262-352 and
+data/nuscenes_pc_img_pose_loader.py:194-380).
 
 accumulate, resample, candidates and farthest_point_sample wrap the C-ABI calls of csrc/assemble.cu for S samples at
 once; assemble_batch chains them (with pointprep.voxel_downsample for the voxel step) into the loader's point side;
@@ -61,23 +62,34 @@ def angles2rotation_matrix(angles):
     return Rz @ (Ry @ Rx)
 
 
-def random_transforms(S, mode, amplitudes=(0.0, 0.0, 0.0, 0.0, 2.0 * math.pi, 0.0), rng=None, flip=True):
+def _amplitudes(a, name):
+    a = np.asarray(a, dtype=np.float64).reshape(-1)
+    if a.shape != (6,) or not np.isfinite(a).all():
+        raise ValueError(f"{name} must be six finite numbers (tx, ty, tz, rx, ry, rz)")
+    return a
+
+
+def random_transforms(S, mode, amplitudes=(0.0, 0.0, 0.0, 0.0, 2.0 * math.pi, 0.0), rng=None, flip=True,
+                      val_amplitudes=None):
     """The loaders' Pr for S samples: `train` draws t ~ U(-a, a) and angles ~ U(-a, a) for amplitudes (tx, ty, tz,
     rx, ry, rz) (generate_random_transform) and, with `flip`, Pr <- Pr diag(-1, 1, 1, 1) with probability 1/2;
-    `val_random_Ry` draws only ry ~ U(-2 pi, 2 pi); other modes give the identity.  rng: a numpy Generator or a seed.
+    `val_random_Ry` draws only ry ~ U(-2 pi, 2 pi), or, with val_amplitudes, t and angles as `train` does from those
+    amplitudes (never flipped); other modes give the identity.  rng: a numpy Generator or a seed.
     Returns (Pr [S,4,4] float64, flip [S] bool)."""
     if mode not in MODES:
         raise ValueError(f"mode must be one of {MODES} (got {mode!r})")
+    if val_amplitudes is not None:
+        val_amplitudes = _amplitudes(val_amplitudes, "val_amplitudes")
     rng = rng if isinstance(rng, np.random.Generator) else np.random.default_rng(rng)
     Pr = np.tile(np.eye(4), (S, 1, 1))
     flipped = np.zeros(S, dtype=bool)
-    if mode == "train":
-        a = np.asarray(amplitudes, dtype=np.float64).reshape(6)
+    if mode == "train" or (mode == "val_random_Ry" and val_amplitudes is not None):
+        a = np.asarray(amplitudes, dtype=np.float64).reshape(6) if mode == "train" else val_amplitudes
         t = rng.uniform(-a[:3], a[:3], (S, 3))
         ang = rng.uniform(-a[3:], a[3:], (S, 3))
         Pr[:, :3, :3] = angles2rotation_matrix(ang)
         Pr[:, :3, 3] = t
-        if flip:
+        if flip and mode == "train":
             flipped = rng.random(S) > 0.5
             Pr[flipped, :, 0] *= -1.0
     elif mode == "val_random_Ry":
@@ -104,6 +116,20 @@ def oxford_args(P_cam_pc, translation_max=10.0, pc_max_range=50.0):
                 amplitudes=(tm, 0.5 * tm, tm, 0.0, 2.0 * math.pi, 0.0), flip=False, jitter=("pc", "intensity"))
 
 
+EGO_BOX = (-0.8, 0.8, -2.7, 2.7)     # data/nuscenes_pc_img_pose_loader.py:200-206: (x_lo, x_hi, y_lo, y_hi), strict
+
+
+def nuscenes_args(P_cam_pc):
+    """assemble_batch arguments of the nuScenes loader: pre = I, P = P_cam_pc Pr^-1 with Pr a rotation about z in
+    `train` and `val_random_Ry` alike, the ego-vehicle box removed from every sweep in its own frame, sweeps
+    accumulated in fp64, voxel 0.2 on the fp64 cloud, no range mask, no flip, jitter on pc and intensity.  P_cam_pc
+    [4,4] or [S,4,4] (camera <- anchor lidar, nuscenes.pose_chain)."""
+    rz = (0.0, 0.0, 0.0, 0.0, 0.0, 2.0 * math.pi)
+    return dict(pre=np.eye(4), P_base=np.asarray(P_cam_pc, dtype=np.float64), voxel_size=0.2, range_max=None,
+                exclude_box=EGO_BOX, accumulate_f64=True, amplitudes=rz, val_amplitudes=rz, flip=False,
+                jitter=("pc", "intensity"))
+
+
 def _jitter_mask(jitter):
     m = 0
     for j in jitter:
@@ -117,12 +143,24 @@ def _f32(t, name, shape, dev):
     _check(t, name, torch.float32, shape, dev)
 
 
-def accumulate(xyz, intensity, sn, n_pts, frame_sample, frame_T, range_max=None, stream=None):
+def _exclude_box(box):
+    if box is None:
+        return None
+    b = np.asarray(box, dtype=np.float64).reshape(-1)
+    if b.shape != (4,) or not np.isfinite(b).all() or b[0] > b[1] or b[2] > b[3]:
+        raise ValueError(f"exclude_box must be four finite numbers (x_lo, x_hi, y_lo, y_hi), lo <= hi (got {box!r})")
+    return b.astype(np.float32)
+
+
+def accumulate(xyz, intensity, sn, n_pts, frame_sample, frame_T, range_max=None, stream=None, exclude_box=None,
+               f64=False):
     """Frame accumulation for S samples.  xyz [T,3,n] f32, intensity [T,n] f32, sn [T,3,n] f32 or None (CUDA); n_pts
     [T] host ints; frame_sample [T] host ints, non-decreasing from 0 (sample of each frame, anchor frame first);
     frame_T [T,4,4] float64 (host).  Returns (xyz [S,3,A], intensity [S,A], sn [S,3,A] or None, count [S] int32 CUDA,
     count host numpy) with each sample's frames moved by frame_T and concatenated; range_max keeps x^2 + z^2 <
-    range_max^2.  The counts are read back once."""
+    range_max^2.  exclude_box (x_lo, x_hi, y_lo, y_hi), rounded to float32, drops the points strictly inside it,
+    tested on each frame's own coordinates before frame_T; with f64 the coordinates stay fp64 (xyz float64, no sn).
+    The counts are read back once."""
     _require_cuda()
     lib = _native.load()
     if not (isinstance(xyz, torch.Tensor) and xyz.is_cuda and xyz.dim() == 3 and xyz.shape[1] == 3):
@@ -147,21 +185,34 @@ def accumulate(xyz, intensity, sn, n_pts, frame_sample, frame_T, range_max=None,
     if not bool(torch.isfinite(xyz).all()):
         raise ValueError("xyz has a non-finite coordinate")
     r = 0.0 if range_max is None else pointprep._positive(range_max, "range_max")
+    box = _exclude_box(exclude_box)
+    if f64 not in (True, False):
+        raise ValueError(f"f64 must be a bool (got {f64!r})")
+    if f64 and sn is not None:
+        raise ValueError("fp64 accumulation carries no sn")
+    if box is not None and not f64:
+        raise ValueError("exclude_box needs the fp64 accumulation")
     S = int(fs[-1]) + 1
     A = round_up(max(int(np.bincount(fs, weights=npts).max()), 1), 16)
     with torch.cuda.device(dev), torch.cuda.stream(stream):
         fs_d = torch.from_numpy(fs.astype(np.int32)).to(dev)
         n_d = torch.from_numpy(npts.astype(np.int32)).to(dev)
         FT_d = torch.from_numpy(FT).to(dev)
-        out_x = torch.zeros((S, 3, A), dtype=torch.float32, device=dev)
+        out_x = torch.zeros((S, 3, A), dtype=torch.float64 if f64 else torch.float32, device=dev)
         out_i = torch.zeros((S, A), dtype=torch.float32, device=dev)
         out_n = torch.zeros((S, 3, A), dtype=torch.float32, device=dev) if sn is not None else None
         cnt = torch.zeros((S,), dtype=torch.int32, device=dev)
         sp = _stream_ptr(stream)
-        ws = _workspace(lib.assemble_accumulate_workspace_bytes(T, n, S), dev, sp)
-        rc = lib.assemble_accumulate_f32(_ptr(xyz), _ptr(intensity), _ptr(sn), _ptr(n_d), n, T, _ptr(fs_d), _ptr(FT_d),
-                                         S, r, _ptr(out_x), _ptr(out_i), _ptr(out_n), A, _ptr(cnt), _ptr(ws),
-                                         ws.numel(), sp)
+        if f64:
+            ws = _workspace(lib.assemble_accumulate_f64_workspace_bytes(T, n, S), dev, sp)
+            rc = lib.assemble_accumulate_f64(_ptr(xyz), _ptr(intensity), _ptr(n_d), n, T, _ptr(fs_d), _ptr(FT_d), S, r,
+                                             None if box is None else box.ctypes.data_as(_native._c.c_void_p),
+                                             _ptr(out_x), _ptr(out_i), A, _ptr(cnt), _ptr(ws), ws.numel(), sp)
+        else:
+            ws = _workspace(lib.assemble_accumulate_workspace_bytes(T, n, S), dev, sp)
+            rc = lib.assemble_accumulate_f32(_ptr(xyz), _ptr(intensity), _ptr(sn), _ptr(n_d), n, T, _ptr(fs_d),
+                                             _ptr(FT_d), S, r, _ptr(out_x), _ptr(out_i), _ptr(out_n), A, _ptr(cnt),
+                                             _ptr(ws), ws.numel(), sp)
         _native.check(rc, "assemble_accumulate")
         cnt_h = cnt.cpu().numpy()
     return out_x, out_i, out_n, cnt, cnt_h
@@ -169,10 +220,13 @@ def accumulate(xyz, intensity, sn, n_pts, frame_sample, frame_T, range_max=None,
 
 def _voxel_step(xyz, inten, sn, cnt, cnt_h, N, voxel_size, stream):
     """The loaders' `if n > 2 N` branch: downsample_with_intensity_sn / downsample_with_reflectance on the samples that
-    take it, with the drop-ins' arithmetic (intensity / max in float32, means in float64, times max, then float32)."""
+    take it, with the drop-ins' arithmetic (intensity / max in float32, means in float64, times max, then float32).
+    xyz is float32 (updated in place) or float64 (voxelised in fp64; the other samples are rounded).  Returns the
+    float32 coordinates and the counts."""
+    xyz32 = xyz if xyz.dtype == torch.float32 else xyz.to(torch.float32)
     vox = np.nonzero(cnt_h > 2 * N)[0]
     if len(vox) == 0:
-        return cnt, cnt_h
+        return xyz32, cnt, cnt_h
     dev = xyz.device
     sel = torch.from_numpy(vox).to(dev)
     A = xyz.shape[2]
@@ -185,7 +239,7 @@ def _voxel_step(xyz, inten, sn, cnt, cnt_h, N, voxel_size, stream):
         rows += [sn[sel][:, a].double() for a in range(3)]
     attr = (torch.stack(rows, 1) * valid[:, None]).contiguous()
     out = pointprep.voxel_downsample(xyz[sel].contiguous(), ns, voxel_size, attr=attr, stream=stream)
-    xyz[sel] = out["xyz"].to(torch.float32)
+    xyz32[sel] = out["xyz"].to(torch.float32)
     inten[sel] = (out["attr"][:, 0] * imax.double()[:, None]).to(torch.float32)
     if sn is not None:
         sn[sel] = out["attr"][:, 1:4].to(torch.float32)
@@ -193,7 +247,7 @@ def _voxel_step(xyz, inten, sn, cnt, cnt_h, N, voxel_size, stream):
     cnt[sel] = out["m_pts"]
     cnt_h = cnt_h.copy()
     cnt_h[vox] = out["m_pts"].cpu().numpy()
-    return cnt, cnt_h
+    return xyz32, cnt, cnt_h
 
 
 def resample(xyz, intensity, sn, n_pts, N, seed, M=None, jitter=(), sigma=SIGMA, clip=CLIP, stream=None):
@@ -326,29 +380,39 @@ def pack_frames(samples, device="cuda"):
 def assemble_batch(frames, mode, seed, input_pt_num=INPUT_PT_NUM, node_a_num=NODE_NUM, node_b_num=NODE_NUM,
                    voxel_size=0.3, range_max=None, pre=np.eye(4), P_base=np.eye(4),
                    amplitudes=(0.0, 0.0, 0.0, 0.0, 2.0 * math.pi, 0.0), flip=True, jitter=("pc", "sn"),
-                   sigma=SIGMA, clip=CLIP, rng=None, stream=None):
+                   sigma=SIGMA, clip=CLIP, rng=None, stream=None, exclude_box=None, accumulate_f64=False,
+                   val_amplitudes=None):
     """The loaders' point side for S samples.  frames: dict(xyz [T,3,n] f32, intensity [T,n] f32, sn [T,3,n] f32 or
     None -- CUDA; n_pts [T], frame_sample [T] (non-decreasing from 0, anchor frame first) and frame_T [T,4,4] float64
-    on the host).  kitti_args / oxford_args give pre, P_base and the rest as the two loaders compose them.  Steps:
-    accumulate (range mask), the voxel step for clouds above 2 input_pt_num points, downsample_np, Pr from
-    random_transforms(mode, amplitudes, rng) with jitter in train mode, points -> (Pr pre) p, and farthest-point
-    node sets from 8 M candidates each.  Returns dict(pc [S,3,N], intensity [S,1,N], sn [S,3,N], node_a [S,3,Ma],
-    node_b [S,3,Mb] f32, node_a_idx, node_b_idx (into pc) int32, Pr [S,4,4] f64, P [S,3,4] f32, P44 [S,4,4] f64,
-    flip [S] bool, n_before_resample [S] int32)."""
+    on the host).  kitti_args / oxford_args / nuscenes_args give pre, P_base and the rest as the loaders compose them.
+    Steps: accumulate (exclusion box, range mask; fp64 with accumulate_f64), the voxel step for clouds above 2
+    input_pt_num points (on the fp64 cloud with accumulate_f64; every cloud is then rounded to float32), downsample_np,
+    Pr from random_transforms(mode, amplitudes, rng, flip, val_amplitudes) with jitter in train mode, points -> (Pr
+    pre) p, and farthest-point node sets from 8 M candidates each.  Returns dict(pc [S,3,N], intensity [S,1,N], sn
+    [S,3,N], node_a [S,3,Ma], node_b [S,3,Mb] f32, node_a_idx, node_b_idx (into pc) int32, Pr [S,4,4] f64, P [S,3,4]
+    f32, P44 [S,4,4] f64, flip [S] bool, n_before_resample [S] int32)."""
     N = int(input_pt_num)
     if N < 1:
         raise ValueError(f"input_pt_num must be at least 1 (got {input_pt_num})")
     for m in (node_a_num, node_b_num):
         if int(m) != m or m < 1 or 8 * m > N:
             raise ValueError(f"8 * node_num ({8 * m}) must be in [8, input_pt_num={N}]")
+    if val_amplitudes is not None:
+        _amplitudes(val_amplitudes, "val_amplitudes")
+    if accumulate_f64 not in (True, False):
+        raise ValueError(f"accumulate_f64 must be a bool (got {accumulate_f64!r})")
+    if _exclude_box(exclude_box) is not None and not accumulate_f64:
+        raise ValueError("exclude_box needs accumulate_f64=True")
     xyz, inten, sn, cnt, cnt_h = accumulate(frames["xyz"], frames["intensity"], frames.get("sn"), frames["n_pts"],
-                                            frames["frame_sample"], frames["frame_T"], range_max, stream)
+                                            frames["frame_sample"], frames["frame_T"], range_max, stream, exclude_box,
+                                            accumulate_f64)
     if cnt_h.min() < 1:
         raise ValueError(f"sample {int(np.argmin(cnt_h))} has no point left to assemble")
     S = cnt_h.shape[0]
     with torch.cuda.device(xyz.device), torch.cuda.stream(stream):
-        cnt, cnt_h = _voxel_step(xyz, inten, sn, cnt, cnt_h, N, pointprep._positive(voxel_size, "voxel_size"), stream)
-        Pr, flipped = random_transforms(S, mode, amplitudes, rng, flip)
+        xyz, cnt, cnt_h = _voxel_step(xyz, inten, sn, cnt, cnt_h, N, pointprep._positive(voxel_size, "voxel_size"),
+                                      stream)
+        Pr, flipped = random_transforms(S, mode, amplitudes, rng, flip, val_amplitudes)
         pre = np.broadcast_to(np.asarray(pre, dtype=np.float64), (S, 4, 4))
         P44 = compose(np.broadcast_to(np.asarray(P_base, dtype=np.float64), (S, 4, 4)), rigid_inverse(Pr))
         out = resample(xyz, inten, sn, cnt, N, seed, M=compose(Pr, pre), jitter=jitter if mode == "train" else (),

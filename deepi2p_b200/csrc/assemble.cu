@@ -2,9 +2,10 @@
 // scan records are read (data/kitti_pc_img_pose_loader.py:199-446, data/oxford_pc_img_pose_loader.py:262-352).
 // DESIGN.md "Batch assembly" states the contract; oracle_assemble/ is its numpy restatement.
 //
-// accumulate  one thread per (frame, point): p' = T p in fp64 with a fixed association, rounded once to float32;
-//             normals get the rotation only; an optional float32 range mask (x^2 + z^2 < r^2); a scan over the keep
-//             flags compacts every sample's frames into one cloud in (frame, index) order
+// accumulate  one thread per (frame, point): p' = T p in fp64 with a fixed association, rounded once to float32 (or
+//             kept in fp64: assemble_accumulate_f64); normals get the rotation only; an optional float32 x / y
+//             exclusion box on the source coordinates and an optional float32 range mask (x'^2 + z'^2 < r^2); a scan
+//             over the keep flags compacts every sample's frames into one cloud in (frame, index) order
 // resample    a 64-bit Philox key per point, a stable segmented radix sort by key (ties: ascending index); output o
 //             takes o mod n while o < r n (the fixed repeats of downsample_np) and the (o - r n)-th point in key order
 //             after that; float32 jitter from Box-Muller on Philox words; p' = M p in fp64, rounded to float32
@@ -116,15 +117,18 @@ struct AccArgs {
   const double* frame_T;     // [T][16]
   int S;
   float range2;              // <= 0: no mask
+  bool box;                  // drop source points with x_lo < x < x_hi and y_lo < y < y_hi (float32 compares)
+  float x_lo, x_hi, y_lo, y_hi;
   float *xyz_out, *intensity_out, *sn_out;
+  double* xyz64_out;         // the fp64 variant's coordinates (instead of xyz_out; no sn)
   int out_stride;
 };
 
-__device__ __forceinline__ void acc_point(const AccArgs& a, int t, int j, float p[3]) {
+__device__ __forceinline__ void acc_point(const AccArgs& a, int t, int j, double p[3]) {
   const double* M = a.frame_T + (size_t)t * 16;
   const float* X = a.xyz + (size_t)t * 3 * a.n_stride;
   const double x = X[j], y = X[(size_t)a.n_stride + j], z = X[(size_t)2 * a.n_stride + j];
-  for (int r = 0; r < 3; ++r) p[r] = (float)affine_row(M, r, x, y, z);
+  for (int r = 0; r < 3; ++r) p[r] = affine_row(M, r, x, y, z);
 }
 
 __global__ void acc_flag_kernel(AccArgs a, int32_t* __restrict__ flag) {
@@ -137,10 +141,16 @@ __global__ void acc_flag_kernel(AccArgs a, int32_t* __restrict__ flag) {
     const int s = a.frame_sample[t];
     if (j < clamp_count(a.n_pts, t, a.n_stride) && s >= 0 && s < a.S) {
       f = 1;
-      if (a.range2 > 0.0f) {
-        float p[3];
+      if (a.box) {
+        const float* X = a.xyz + (size_t)t * 3 * a.n_stride;
+        const float x = X[j], y = X[(size_t)a.n_stride + j];
+        f = !(x > a.x_lo && x < a.x_hi && y > a.y_lo && y < a.y_hi);
+      }
+      if (f && a.range2 > 0.0f) {
+        double p[3];
         acc_point(a, t, j, p);
-        f = p[0] * p[0] + p[2] * p[2] < a.range2;
+        const float px = (float)p[0], pz = (float)p[2];
+        f = px * px + pz * pz < a.range2;
       }
     }
   }
@@ -159,6 +169,7 @@ __global__ void acc_first_kernel(const int32_t* __restrict__ frame_sample, int T
   first[s] = s == S ? T : lo;
 }
 
+template <bool F64>
 __global__ void acc_scatter_kernel(AccArgs a, const int32_t* __restrict__ flag, const int32_t* __restrict__ pos,
                                    const int32_t* __restrict__ first, int32_t* __restrict__ count_out) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -171,9 +182,14 @@ __global__ void acc_scatter_kernel(AccArgs a, const int32_t* __restrict__ flag, 
   const int s = a.frame_sample[t];
   const int o = pos[g] - pos[(size_t)first[s] * a.n_stride];
   if (o < 0 || o >= a.out_stride) return;
-  float p[3];
+  double p[3];
   acc_point(a, t, j, p);
-  for (int r = 0; r < 3; ++r) a.xyz_out[((size_t)s * 3 + r) * a.out_stride + o] = p[r];
+  for (int r = 0; r < 3; ++r) {
+    if constexpr (F64)
+      a.xyz64_out[((size_t)s * 3 + r) * a.out_stride + o] = p[r];
+    else
+      a.xyz_out[((size_t)s * 3 + r) * a.out_stride + o] = (float)p[r];
+  }
   a.intensity_out[(size_t)s * a.out_stride + o] = a.intensity[(size_t)t * a.n_stride + j];
   if (a.sn) {
     const double* M = a.frame_T + (size_t)t * 16;
@@ -183,10 +199,15 @@ __global__ void acc_scatter_kernel(AccArgs a, const int32_t* __restrict__ flag, 
   }
 }
 
+template <bool F64>
 int accumulate(const AccArgs& a, int32_t* count_out, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  DIB_REQUIRE(a.xyz && a.intensity && a.frame_sample && a.frame_T && a.xyz_out && a.intensity_out && count_out,
+  DIB_REQUIRE(a.xyz && a.intensity && a.frame_sample && a.frame_T && (F64 ? (void*)a.xyz64_out : (void*)a.xyz_out) &&
+              a.intensity_out && count_out,
               "NULL argument (xyz, intensity, frame_sample, frame_T, xyz_out, intensity_out, count_out)");
   DIB_REQUIRE(!a.sn || a.sn_out, "NULL argument (sn_out with sn)");
+  DIB_REQUIRE(!a.box || (std::isfinite(a.x_lo) && std::isfinite(a.x_hi) && std::isfinite(a.y_lo) &&
+                         std::isfinite(a.y_hi) && a.x_lo <= a.x_hi && a.y_lo <= a.y_hi),
+              "exclude_box must be finite with x_lo <= x_hi and y_lo <= y_hi");
   DIB_REQUIRE(a.T >= 0 && a.S >= 0 && a.S <= kMaxS, "T=%d, S=%d: need T >= 0 and 0 <= S <= %d", a.T, a.S, kMaxS);
   DIB_REQUIRE(a.n_stride >= 1 && a.out_stride >= 1, "n_stride and out_stride must be positive");
   DIB_REQUIRE((long long)a.T * a.n_stride < (1LL << 31) - 1 && (long long)a.S * a.out_stride < (1LL << 31),
@@ -207,7 +228,7 @@ int accumulate(const AccArgs& a, int32_t* count_out, void* workspace, size_t wor
   DIB_REQUIRE(tmp <= kScratch, "accumulate: scan scratch %zu exceeds %zu", tmp, kScratch);
   DIB_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(wk.tmp, tmp, wk.flag, wk.pos, (int)N, st));
   const long long M = N - 1 > a.S ? N - 1 : a.S;
-  acc_scatter_kernel<<<(int)((M + 255) / 256), 256, 0, st>>>(a, wk.flag, wk.pos, wk.first, count_out);
+  acc_scatter_kernel<F64><<<(int)((M + 255) / 256), 256, 0, st>>>(a, wk.flag, wk.pos, wk.first, count_out);
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
 }
@@ -575,9 +596,26 @@ int assemble_accumulate_f32(const float* xyz, const float* intensity, const floa
                             int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream) {
   DIB_REQUIRE(std::isfinite(range_max), "range_max must be finite (<= 0: no range mask)");
   const float r2 = range_max > 0.0 ? (float)(range_max * range_max) : 0.0f;
-  const dib::asmb::AccArgs a{xyz, intensity, sn, n_pts, n_stride, T, frame_sample, frame_T16, S, r2,
-                             xyz_out, intensity_out, sn_out, out_stride};
-  return dib::asmb::accumulate(a, count_out, workspace, workspace_bytes, (cudaStream_t)stream);
+  const dib::asmb::AccArgs a{xyz, intensity, sn, n_pts, n_stride, T, frame_sample, frame_T16, S, r2, false,
+                             0.0f, 0.0f, 0.0f, 0.0f, xyz_out, intensity_out, sn_out, nullptr, out_stride};
+  return dib::asmb::accumulate<false>(a, count_out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t assemble_accumulate_f64_workspace_bytes(int T, int n_stride, int S) {
+  return assemble_accumulate_workspace_bytes(T, n_stride, S);
+}
+
+int assemble_accumulate_f64(const float* xyz, const float* intensity, const int32_t* n_pts, int n_stride, int T,
+                            const int32_t* frame_sample, const double* frame_T16, int S, double range_max,
+                            const float* exclude_box, double* xyz_out, float* intensity_out, int out_stride,
+                            int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream) {
+  DIB_REQUIRE(std::isfinite(range_max), "range_max must be finite (<= 0: no range mask)");
+  const float r2 = range_max > 0.0 ? (float)(range_max * range_max) : 0.0f;
+  const float* b = exclude_box;
+  const dib::asmb::AccArgs a{xyz, intensity, nullptr, n_pts, n_stride, T, frame_sample, frame_T16, S, r2, b != nullptr,
+                             b ? b[0] : 0.0f, b ? b[1] : 0.0f, b ? b[2] : 0.0f, b ? b[3] : 0.0f, nullptr,
+                             intensity_out, nullptr, xyz_out, out_stride};
+  return dib::asmb::accumulate<true>(a, count_out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 size_t assemble_resample_workspace_bytes(int S, int n_stride) {

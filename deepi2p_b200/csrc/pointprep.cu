@@ -3,8 +3,9 @@
 // DESIGN.md "Scan preparation" states the contract; oracle_prep/prep_oracle.cpp is its serial CPU restatement.
 //
 // voxel downsample (per call)
-//   bbox      (one CTA per cloud)  float bounding box; read back to the host, which rejects clouds of 2^21 or more
-//             voxels along an axis and sizes the sort key from the largest voxel index of the batch
+//   bbox      (one CTA per cloud)  bounding box in the coordinates' type (float32 or fp64); read back to the host,
+//             which rejects clouds of 2^21 or more voxels along an axis and sizes the sort key from the largest voxel
+//             index of the batch
 //   key       voxel (ix, iy, iz) = floor((p - min_bound) / v) in fp64, packed into bx + by + bz bits
 //   sort      stable cub radix sorts: by voxel key, then by cloud (padding last), so each voxel's points are
 //             contiguous and in ascending original index
@@ -46,7 +47,7 @@ inline size_t sort_reserve(size_t N) { return 8 * N + ((size_t)4 << 20); }
 // Voxel downsample.
 
 struct VoxWork {
-  float* bbox;                          // [S][6]
+  void* bbox;                           // [S][6] in the coordinates' type
   unsigned long long *key0, *key1;      // [N] voxel keys
   uint32_t *ck0, *ck1;                  // [N] cloud keys
   int32_t *val0, *val1;                 // [N] global point index s * n_stride + j
@@ -63,7 +64,7 @@ size_t carve_vox(char* base, int S, int n_stride, VoxWork* wk) {
   size_t off = 0;
   auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += align256(bytes); return p; };
   VoxWork w;
-  w.bbox = (float*)take((size_t)S * 6 * 4);
+  w.bbox = take((size_t)S * 6 * 8);
   w.key0 = (unsigned long long*)take(N * 8); w.key1 = (unsigned long long*)take(N * 8);
   w.ck0 = (uint32_t*)take(N * 4); w.ck1 = (uint32_t*)take(N * 4);
   w.val0 = (int32_t*)take(N * 4); w.val1 = (int32_t*)take(N * 4);
@@ -83,8 +84,8 @@ struct VoxKey {
 };
 
 // The voxel of point j of cloud s: floor(((double)p - min_bound) / v) per axis, min_bound = (double)lo - 0.5 * v.
-__device__ __forceinline__ unsigned long long voxel_key(const float* X, int n_stride, const float* bb, int j,
-                                                        const VoxKey& k) {
+template <typename T>
+__device__ __forceinline__ unsigned long long voxel_key(const T* X, int n_stride, const T* bb, int j, const VoxKey& k) {
   unsigned long long c[3];
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
@@ -95,8 +96,40 @@ __device__ __forceinline__ unsigned long long voxel_key(const float* X, int n_st
   return (c[0] << k.byz) | (c[1] << k.bz) | c[2];
 }
 
-__global__ void vox_key_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ n_pts, int n_stride, int S,
-                               const float* __restrict__ bbox, VoxKey k, unsigned long long* __restrict__ key,
+// The float32 clouds' box is icp.cu's bbox_kernel; fp64 clouds get this one (min / max are exact in any order).
+__global__ void __launch_bounds__(256) bbox_f64_kernel(const double* __restrict__ X, const int32_t* __restrict__ n_pts,
+                                                       int n_stride, double* __restrict__ bbox) {
+  const int s = blockIdx.x;
+  const int n = clamp_n(n_pts, s, n_stride);
+  const double* P = X + (size_t)s * 3 * n_stride;
+  double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
+  for (int j = threadIdx.x; j < n; j += blockDim.x)
+    for (int a = 0; a < 3; ++a) {
+      const double v = P[(size_t)a * n_stride + j];
+      lo[a] = fmin(lo[a], v);
+      hi[a] = fmax(hi[a], v);
+    }
+  __shared__ double red[6][8];
+  for (int a = 0; a < 3; ++a)
+    for (int o = 16; o > 0; o >>= 1) {
+      lo[a] = fmin(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
+      hi[a] = fmax(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
+    }
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0)
+    for (int a = 0; a < 3; ++a) red[a][w] = lo[a], red[3 + a][w] = hi[a];
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    double v = red[threadIdx.x][0];
+    for (int q = 1; q < (int)(blockDim.x >> 5); ++q)
+      v = threadIdx.x < 3 ? fmin(v, red[threadIdx.x][q]) : fmax(v, red[threadIdx.x][q]);
+    bbox[s * 6 + threadIdx.x] = v;
+  }
+}
+
+template <typename T>
+__global__ void vox_key_kernel(const T* __restrict__ xyz, const int32_t* __restrict__ n_pts, int n_stride, int S,
+                               const T* __restrict__ bbox, VoxKey k, unsigned long long* __restrict__ key,
                                int32_t* __restrict__ val) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= (long long)S * n_stride) return;
@@ -116,9 +149,9 @@ __global__ void vox_cloud_kernel(const int32_t* __restrict__ n_pts, int n_stride
   ck[g] = j < clamp_n(n_pts, s, n_stride) ? (uint32_t)s : (uint32_t)S;
 }
 
-__global__ void vox_head_kernel(const float* __restrict__ xyz, int n_stride, long long N,
-                                const float* __restrict__ bbox, VoxKey k, const int32_t* __restrict__ val,
-                                const int32_t* __restrict__ off, int S, int32_t* __restrict__ head) {
+template <typename T>
+__global__ void vox_head_kernel(const T* __restrict__ xyz, int n_stride, long long N, const T* __restrict__ bbox, VoxKey k,
+                                const int32_t* __restrict__ val, const int32_t* __restrict__ off, int S, int32_t* __restrict__ head) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   int h = 0;
@@ -127,7 +160,7 @@ __global__ void vox_head_kernel(const float* __restrict__ xyz, int n_stride, lon
     h = 1;
     if (i > off[s]) {
       const int u = val[i - 1], ju = u - s * n_stride;     // same cloud
-      const float* X = xyz + (size_t)s * 3 * n_stride;
+      const T* X = xyz + (size_t)s * 3 * n_stride;
       h = voxel_key(X, n_stride, bbox + s * 6, j, k) != voxel_key(X, n_stride, bbox + s * 6, ju, k);
     }
   }
@@ -135,7 +168,8 @@ __global__ void vox_head_kernel(const float* __restrict__ xyz, int n_stride, lon
 }
 
 // One thread per voxel head: sequential sums over the voxel's points in ascending original index, then / count.
-__global__ void vox_mean_kernel(const float* __restrict__ xyz, const double* __restrict__ attr, int C, int n_stride,
+template <typename T>
+__global__ void vox_mean_kernel(const T* __restrict__ xyz, const double* __restrict__ attr, int C, int n_stride,
                                 long long N, const int32_t* __restrict__ n_pts, const int32_t* __restrict__ val,
                                 const int32_t* __restrict__ off, const int32_t* __restrict__ head,
                                 const int32_t* __restrict__ rank, int S, double* __restrict__ xyz_out,
@@ -148,7 +182,7 @@ __global__ void vox_mean_kernel(const float* __restrict__ xyz, const double* __r
   int e = (int)i + 1;
   while (e < end && !head[e]) ++e;
   const double cnt = (double)(e - (int)i);
-  const float* X = xyz + (size_t)s * 3 * n_stride;
+  const T* X = xyz + (size_t)s * 3 * n_stride;
   for (int a = 0; a < 3; ++a) {
     double sum = 0.0;
     for (int t = (int)i; t < e; ++t) sum += (double)X[(size_t)a * n_stride + (val[t] - s * n_stride)];
@@ -184,7 +218,8 @@ int check_stride(int stride, int S, const char* name) {
   return DIB_OK;
 }
 
-int voxel_downsample(const float* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
+template <typename T>
+int voxel_downsample(const T* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
                      double voxel_size, double* xyz_out, double* attr_out, int32_t* m_pts_out, void* workspace,
                      size_t workspace_bytes, cudaStream_t st) {
   DIB_REQUIRE(xyz && xyz_out && m_pts_out, "NULL argument (xyz, xyz_out, m_pts_out)");
@@ -199,11 +234,15 @@ int voxel_downsample(const float* xyz, const int32_t* n_pts, int n_stride, int S
   if (S == 0) return DIB_OK;
   VoxWork wk;
   carve_vox((char*)workspace, S, n_stride, &wk);
-  icp::cloud_bbox(xyz, n_pts, n_stride, S, wk.bbox, st);
+  T* bbox = (T*)wk.bbox;
+  if constexpr (sizeof(T) == 4)
+    icp::cloud_bbox(xyz, n_pts, n_stride, S, bbox, st);
+  else
+    bbox_f64_kernel<<<S, 256, 0, st>>>(xyz, n_pts, n_stride, bbox);
   DIB_CHECK_CUDA(cudaGetLastError());
   // The limit on the voxel count depends on the data, so the boxes come back to the host before the sort.
-  std::vector<float> bb((size_t)S * 6);
-  DIB_CHECK_CUDA(cudaMemcpyAsync(bb.data(), wk.bbox, bb.size() * 4, cudaMemcpyDeviceToHost, st));
+  std::vector<T> bb((size_t)S * 6);
+  DIB_CHECK_CUDA(cudaMemcpyAsync(bb.data(), bbox, bb.size() * sizeof(T), cudaMemcpyDeviceToHost, st));
   DIB_CHECK_CUDA(cudaStreamSynchronize(st));
   unsigned long long top[3] = {0, 0, 0};
   for (int s = 0; s < S; ++s) {
@@ -222,7 +261,7 @@ int voxel_downsample(const float* xyz, const int32_t* n_pts, int n_stride, int S
   const int kb = bits_of(top[0]) + k.byz;
   const long long N = (long long)S * n_stride;
   const int nb = (int)((N + 255) / 256);
-  vox_key_kernel<<<nb, 256, 0, st>>>(xyz, n_pts, n_stride, S, wk.bbox, k, wk.key0, wk.val0);
+  vox_key_kernel<T><<<nb, 256, 0, st>>>(xyz, n_pts, n_stride, S, bbox, k, wk.key0, wk.val0);
   DIB_CHECK_CUDA(cudaGetLastError());
   cub::DoubleBuffer<unsigned long long> keys(wk.key0, wk.key1);
   cub::DoubleBuffer<int32_t> vals(wk.val0, wk.val1);
@@ -249,12 +288,12 @@ int voxel_downsample(const float* xyz, const int32_t* n_pts, int n_stride, int S
   DIB_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp, wk.cnt, wk.off, S + 1, st));
   DIB_REQUIRE(tmp <= wk.tmp_bytes, "voxel_downsample: scan scratch %zu exceeds %zu", tmp, wk.tmp_bytes);
   DIB_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(wk.tmp, tmp, wk.cnt, wk.off, S + 1, st));
-  vox_head_kernel<<<nb, 256, 0, st>>>(xyz, n_stride, N, wk.bbox, k, vals.Current(), wk.off, S, wk.head);
+  vox_head_kernel<T><<<nb, 256, 0, st>>>(xyz, n_stride, N, bbox, k, vals.Current(), wk.off, S, wk.head);
   DIB_CHECK_CUDA(cudaGetLastError());
   DIB_CHECK_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp, wk.head, wk.rank, (int)N, st));
   DIB_REQUIRE(tmp <= wk.tmp_bytes, "voxel_downsample: scan scratch %zu exceeds %zu", tmp, wk.tmp_bytes);
   DIB_CHECK_CUDA(cub::DeviceScan::InclusiveSum(wk.tmp, tmp, wk.head, wk.rank, (int)N, st));
-  vox_mean_kernel<<<nb, 256, 0, st>>>(xyz, attr, C, n_stride, N, n_pts, vals.Current(), wk.off, wk.head, wk.rank, S,
+  vox_mean_kernel<T><<<nb, 256, 0, st>>>(xyz, attr, C, n_stride, N, n_pts, vals.Current(), wk.off, wk.head, wk.rank, S,
                                       xyz_out, attr_out);
   vox_count_kernel<<<(S + 127) / 128, 128, 0, st>>>(n_pts, n_stride, S, wk.off, wk.rank, m_pts_out);
   DIB_CHECK_CUDA(cudaGetLastError());
@@ -438,8 +477,15 @@ size_t voxel_downsample_workspace_bytes(int S, int n_stride, int C) {
 int voxel_downsample_batch_f32(const float* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
                                double voxel_size, double* xyz_out, double* attr_out, int32_t* m_pts_out,
                                void* workspace, size_t workspace_bytes, dib_stream_t stream) {
-  return dib::prep::voxel_downsample(xyz, n_pts, n_stride, S, attr, C, voxel_size, xyz_out, attr_out, m_pts_out,
-                                     workspace, workspace_bytes, (cudaStream_t)stream);
+  return dib::prep::voxel_downsample<float>(xyz, n_pts, n_stride, S, attr, C, voxel_size, xyz_out, attr_out,
+                                            m_pts_out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int voxel_downsample_batch_f64(const double* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
+                               double voxel_size, double* xyz_out, double* attr_out, int32_t* m_pts_out,
+                               void* workspace, size_t workspace_bytes, dib_stream_t stream) {
+  return dib::prep::voxel_downsample<double>(xyz, n_pts, n_stride, S, attr, C, voxel_size, xyz_out, attr_out,
+                                             m_pts_out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 size_t estimate_normals_workspace_bytes(int S, int m_stride) {

@@ -7,8 +7,8 @@ pack_images packs ragged HWC uint8 frames into one device buffer, and decode_jpe
 loaders' JPEG frames (Image.open(path).convert("RGB"), bit for bit; csrc/jpeg.cu, DESIGN.md 4.19) into the same
 buffer on the device; image_params draws the per-sample crop offsets and
 jitter on the host; assemble_images runs csrc/imageprep.cu and composes K in fp64.  kitti_image_args /
-oxford_image_args are the two loaders' options; nuScenes is crop_top_rows=100, img_scale=0.2, 160 x 320,
-jitter_prob=0.5.  augment_img is a host drop-in for the loaders' augment_img that works on current torchvision.
+oxford_image_args / nuscenes_image_args are the loaders' options (nuScenes: crop_top_rows=100, img_scale=0.2, 160 x
+320, jitter_prob=0.5).  augment_img is a host drop-in for the loaders' augment_img that works on current torchvision.
 DESIGN.md 4.13 states the contract.  There is no CPU fallback.
 """
 import numpy as np
@@ -32,6 +32,12 @@ def kitti_image_args():
 def oxford_image_args():
     """oxford/options.py: no row cut, scale 0.5, 384 x 640; a train sample is jittered with probability 1/2."""
     return dict(img_H=384, img_W=640, img_scale=0.5, crop_top_rows=0, crop_bottom_rows=0, jitter_prob=0.5)
+
+
+def nuscenes_image_args():
+    """nuscenes_t/options.py: cut 100 top rows, scale 0.2, 160 x 320; a train sample is jittered with probability
+    1/2."""
+    return dict(img_H=160, img_W=320, img_scale=0.2, crop_top_rows=100, crop_bottom_rows=0, jitter_prob=0.5)
 
 
 def resize_dims(h, w, s):

@@ -54,15 +54,15 @@ def _cloud_batch(xyz, n_pts, name="xyz"):
 
 
 def voxel_downsample(xyz, n_pts, voxel_size, attr=None, stream=None):
-    """Open3D voxel_down_sample for S clouds.  xyz [S,3,N] f32, n_pts [S] int32 or None (= N), attr [S,C,N] f64 or
-    None.  Returns dict(xyz [S,3,N] f64, m_pts [S] int32, attr [S,C,N] f64 when given): per cloud, the mean of each
-    occupied voxel's points (and attributes) in ascending (ix, iy, iz) order; entries past m_pts are zero.  Raises
-    ValueError when a cloud spans 2^21 or more voxels along an axis.  The call waits for the stream's earlier work."""
+    """Open3D voxel_down_sample for S clouds.  xyz [S,3,N] f32 or f64, n_pts [S] int32 or None (= N), attr [S,C,N]
+    f64 or None.  Returns dict(xyz [S,3,N] f64, m_pts [S] int32, attr [S,C,N] f64 when given): per cloud, the mean of
+    each occupied voxel's points (and attributes) in ascending (ix, iy, iz) order; entries past m_pts are zero.
+    Raises ValueError when a cloud spans 2^21 or more voxels along an axis.  The call waits for the stream's earlier
+    work."""
     voxel_size = _positive(voxel_size, "voxel_size")
     _require_cuda()
     lib = _native.load()
-    S, N = _cloud_batch(xyz, n_pts)
-    _check(xyz, "xyz", torch.float32, (S, 3, N), None)
+    S, N = _cloud_batch(xyz, n_pts)             # float32 or float64
     C = 0
     if attr is not None:
         if not (isinstance(attr, torch.Tensor) and attr.dim() == 3):
@@ -79,8 +79,9 @@ def voxel_downsample(xyz, n_pts, voxel_size, attr=None, stream=None):
             res["attr"] = torch.zeros((S, C, N), dtype=torch.float64, device=dev)
         sp = _stream_ptr(stream)
         ws = _workspace(max(lib.voxel_downsample_workspace_bytes(S, N, C), 1), dev, sp)
-        rc = lib.voxel_downsample_batch_f32(_ptr(xyz), _ptr(n_pts), N, S, _ptr(attr), C, voxel_size, _ptr(res["xyz"]),
-                                            _ptr(res.get("attr")), _ptr(res["m_pts"]), _ptr(ws), ws.numel(), sp)
+        fn = lib.voxel_downsample_batch_f32 if xyz.dtype == torch.float32 else lib.voxel_downsample_batch_f64
+        rc = fn(_ptr(xyz), _ptr(n_pts), N, S, _ptr(attr), C, voxel_size, _ptr(res["xyz"]), _ptr(res.get("attr")),
+                _ptr(res["m_pts"]), _ptr(ws), ws.numel(), sp)
     if rc == -22:                   # the only data-dependent rejection: too many voxels along an axis
         raise ValueError(lib.dib_last_error().decode("utf-8", "replace"))
     _native.check(rc, "voxel_downsample")

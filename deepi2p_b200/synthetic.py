@@ -8,6 +8,7 @@ loader's crop/scale (data/kitti_pc_img_pose_loader.py:329-349, kitti/options.py:
 Oxford-shaped: H=384, W=640 (data/oxford_pc_img_pose_loader.py:221-259).
 """
 import math
+import os
 
 import numpy as np
 
@@ -239,6 +240,104 @@ def make_loader_sample(seed, shape="kitti", n_rings=64, n_azimuth=512):
         return dict(frames=[(cam, sc["intensity"], None)], frame_T=np.eye(4)[None], K=K,
                     P_cam_pc=_rigid(rng, 0.1, 5.0))
     raise ValueError(f"shape must be 'kitti' or 'oxford' (got {shape!r})")
+
+
+NUSCENES_CAMERAS = ("CAM_FRONT", "CAM_FRONT_LEFT", "CAM_FRONT_RIGHT", "CAM_BACK", "CAM_BACK_LEFT", "CAM_BACK_RIGHT")
+EGO_POINTS = 512
+
+
+def make_nuscenes_sweep(seed, n_rings=32, n_azimuth=1085):
+    """One seeded LIDAR_TOP-shaped sweep as the .pcd.bin records hold it: [n, 5] float32 (x, y, z, intensity, ring),
+    a make_lidar_scan of n_rings x n_azimuth rays (intensity 0-255) followed by EGO_POINTS points drawn in and around
+    the ego-vehicle box (-0.8 < x < 0.8, -2.7 < y < 2.7)."""
+    sc = make_lidar_scan(seed, n_rings=n_rings, n_azimuth=n_azimuth, ground=-1.84)
+    rng = np.random.default_rng(seed + 0xE60)
+    ego = rng.uniform([-1.0, -3.0, -1.5], [1.0, 3.0, 0.5], (EGO_POINTS, 3)).T
+    xyz = np.concatenate([sc["xyz"], ego.astype(np.float32)], 1)
+    inten = np.concatenate([sc["intensity"] * 255.0, rng.uniform(0.0, 255.0, EGO_POINTS)])
+    ring = np.concatenate([np.repeat(np.arange(n_rings), n_azimuth), np.zeros(EGO_POINTS)])
+    return np.stack([xyz[0], xyz[1], xyz[2], inten, ring], 1).astype(np.float32)
+
+
+def make_nuscenes_sample(seed, n_sweeps=7, n_rings=32, n_azimuth=1085):
+    """One seeded nuScenes sample for assemble_batch(**nuscenes_args): n_sweeps make_nuscenes_sweep frames (the anchor
+    first with the identity, the others moved by small rigid frame_T as the sweep chain composes them) and P_cam_pc.
+    Returns dict(frames [(xyz [3,n] f32, intensity [n] f32, None)], frame_T [T,4,4], P_cam_pc [4,4])."""
+    rng = np.random.default_rng(seed + 0x4E5)
+    frames, Ts = [], []
+    for t in range(n_sweeps):
+        r = make_nuscenes_sweep(seed * 16 + t, n_rings, n_azimuth)
+        frames.append((np.ascontiguousarray(r[:, :3].T), np.ascontiguousarray(r[:, 3]), None))
+        Ts.append(np.eye(4) if t == 0 else _rigid(rng, 0.02, 4.0))
+    P = np.eye(4)
+    P[:3, :3] = np.array([[0.0, -1.0, 0.0], [0.0, 0.0, -1.0], [1.0, 0.0, 0.0]]) @ _rigid(rng, 0.05, 0.0)[:3, :3]
+    P[:3, 3] = rng.uniform(-1.0, 1.0, 3)
+    return dict(frames=frames, frame_T=np.stack(Ts), P_cam_pc=P)
+
+
+def _quaternion(rng, yaw, tilt=0.01):
+    """A near-unit (w, x, y, z) list: yaw about z plus small tilts, not renormalised."""
+    return [math.cos(yaw / 2), float(rng.normal(0.0, tilt)), float(rng.normal(0.0, tilt)), math.sin(yaw / 2)]
+
+
+def write_nuscenes_dataroot(root, chains, seed=0, jpeg=None, version="v1.0-mini", n_rings=8, n_azimuth=128,
+                            sweeps=True):
+    """A seeded devkit-layout dataroot for deepi2p_b200.nuscenes: <root>/<version>/{sample_data, ego_pose,
+    calibrated_sensor}.json, <root>/dataset_info.list and, with `sweeps`, one make_nuscenes_sweep .pcd.bin per
+    LIDAR_TOP record.  chains: [(length, anchor)] -- one scene per entry, `length` LIDAR_TOP sweeps linked by next /
+    prev, the dataset entry at sweep `anchor`.  Each scene has one record per camera whose file holds `jpeg` (bytes)
+    when given.  Returns the dataset_info list."""
+    import json
+    import pickle
+    rng = np.random.default_rng(seed + 0x4E5C)
+    sd, ego, cal = [], [], []
+    cal.append(dict(token="calib-LIDAR_TOP", sensor_token="LIDAR_TOP", translation=[0.943713, 0.0, 1.84023],
+                    rotation=_quaternion(rng, -math.pi / 2), camera_intrinsic=[]))
+    for k, name in enumerate(NUSCENES_CAMERAS):
+        yaw = [0.0, 0.95, -0.95, math.pi, 1.9, -1.9][k]
+        cal.append(dict(token=f"calib-{name}", sensor_token=name, translation=[1.7, 0.0 + 0.1 * k, 1.5],
+                        rotation=_quaternion(rng, yaw - math.pi / 2),
+                        camera_intrinsic=[[1266.4, 0.0, 816.3 + k], [0.0, 1266.4, 491.5], [0.0, 0.0, 1.0]]))
+    items = []
+    for c, (length, anchor) in enumerate(chains):
+        x0 = rng.uniform(300.0, 900.0, 2)
+        heading = rng.uniform(-math.pi, math.pi)
+        for i in range(length):
+            tok = f"lidar-{c}-{i}"
+            fn = f"sweeps/LIDAR_TOP/scene{c}_{i:03d}.pcd.bin"
+            sd.append(dict(token=tok, filename=fn, ego_pose_token=f"ego-{c}-{i}",
+                           calibrated_sensor_token="calib-LIDAR_TOP",
+                           next=f"lidar-{c}-{i + 1}" if i + 1 < length else "",
+                           prev=f"lidar-{c}-{i - 1}" if i > 0 else ""))
+            yaw = heading + 0.01 * i
+            ego.append(dict(token=f"ego-{c}-{i}", rotation=_quaternion(rng, yaw),
+                            translation=[x0[0] + 0.45 * i * math.cos(heading), x0[1] + 0.45 * i * math.sin(heading),
+                                         float(rng.normal(0.0, 0.02))]))
+            if sweeps:
+                os.makedirs(os.path.join(root, os.path.dirname(fn)), exist_ok=True)
+                make_nuscenes_sweep(seed * 4096 + c * 64 + i, n_rings, n_azimuth).tofile(os.path.join(root, fn))
+        cams = {}
+        for name in NUSCENES_CAMERAS:
+            tok = f"cam-{c}-{name}"
+            fn = f"samples/{name}/scene{c}.jpg"
+            sd.append(dict(token=tok, filename=fn, ego_pose_token=f"ego-{tok}", calibrated_sensor_token=f"calib-{name}",
+                           next="", prev=""))
+            ego.append(dict(token=f"ego-{tok}", rotation=_quaternion(rng, heading + 0.01 * anchor),
+                            translation=[x0[0] + 0.45 * anchor * math.cos(heading) + float(rng.normal(0.0, 0.1)),
+                                         x0[1] + 0.45 * anchor * math.sin(heading), 0.0]))
+            if jpeg is not None:
+                os.makedirs(os.path.join(root, os.path.dirname(fn)), exist_ok=True)
+                with open(os.path.join(root, fn), "wb") as f:
+                    f.write(jpeg)
+            cams[name] = [tok]
+        items.append((f"lidar-{c}-{anchor}", cams))
+    os.makedirs(os.path.join(root, version), exist_ok=True)
+    for name, recs in (("sample_data", sd), ("ego_pose", ego), ("calibrated_sensor", cal)):
+        with open(os.path.join(root, version, name + ".json"), "w") as f:
+            json.dump(recs, f)
+    with open(os.path.join(root, "dataset_info.list"), "wb") as f:
+        pickle.dump(items, f)
+    return items
 
 
 def write_icp_handoff(data_dir, monodepth_dir, seeds, shape="oxford"):

@@ -346,6 +346,8 @@ int icp_build_index_f32(const float* tgt, const int32_t* m_pts, int m_stride, in
  *   Returns DIB_EINVAL when a cloud spans 2^21 or more voxels along an axis.  The call reads the clouds' boxes back
  *   to the host, so it waits for the work queued on the stream before it.
  *   workspace >= voxel_downsample_workspace_bytes(S, n_stride, C), 256-byte aligned (about 44 B per point).
+ * voxel_downsample_batch_f64: the same with fp64 coordinates xyz [S][3][n_stride] f64 (min_bound from the fp64 box).
+ *   Same workspace.
  * estimate_normals_batch_f32: xyz [S][3][m_stride] f32.  Per point i: the min(max_nn, c) nearest points of the cloud
  *   with d2 < radius^2 (itself included, ties -> lower index; 1 <= max_nn <= 64); fewer than 3 -> (0, 0, 1); else the
  *   unit eigenvector of the smallest eigenvalue of the covariance about p_i (zero covariance -> 0); then a zero normal
@@ -362,6 +364,9 @@ int icp_build_index_f32(const float* tgt, const int32_t* m_pts, int m_stride, in
  * ------------------------------------------------------------------------------------------ */
 size_t voxel_downsample_workspace_bytes(int S, int n_stride, int C);
 int voxel_downsample_batch_f32(const float* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
+                               double voxel_size, double* xyz_out, double* attr_out, int32_t* m_pts_out,
+                               void* workspace, size_t workspace_bytes, dib_stream_t stream);
+int voxel_downsample_batch_f64(const double* xyz, const int32_t* n_pts, int n_stride, int S, const double* attr, int C,
                                double voxel_size, double* xyz_out, double* attr_out, int32_t* m_pts_out,
                                void* workspace, size_t workspace_bytes, dib_stream_t stream);
 size_t estimate_normals_workspace_bytes(int S, int m_stride);
@@ -386,6 +391,10 @@ int sym3_eig_batch_f64(const double* C, int n, double* lam, double* E, dib_strea
  *   points with x'^2 + z'^2 < range_max^2 in float32.  Each sample's kept points are written in (frame, index) order to
  *   xyz_out [S][3][out_stride], intensity_out [S][out_stride], sn_out [S][3][out_stride] (with sn); count_out [S] i32.
  *   workspace >= assemble_accumulate_workspace_bytes(T, n_stride, S), 256-byte aligned.
+ * assemble_accumulate_f64 (data/nuscenes_pc_img_pose_loader.py:194-267): as assemble_accumulate_f32 without sn, with
+ *   the coordinates kept in fp64, xyz_out [S][3][out_stride] f64.  exclude_box [host, 4 f32] (x_lo, x_hi, y_lo, y_hi)
+ *   or NULL drops points with x_lo < x < x_hi and y_lo < y < y_hi, compared in float32 on the frame's own (source)
+ *   coordinates before the transform.  workspace >= assemble_accumulate_f64_workspace_bytes(T, n_stride, S).
  * assemble_resample_f32: S clouds as above (stride n_stride, counts n_pts [S]) to input_pt_num = N points each
  *   (data/kitti_pc_img_pose_loader.py:158-171): with n >= N points, the N smallest (key, index); otherwise index o < r n
  *   takes o mod n (r >= 1 the smallest with (r + 1) n >= N) and the rest the N - r n smallest keys, in ascending key
@@ -406,6 +415,11 @@ size_t assemble_accumulate_workspace_bytes(int T, int n_stride, int S);
 int assemble_accumulate_f32(const float* xyz, const float* intensity, const float* sn, const int32_t* n_pts,
                             int n_stride, int T, const int32_t* frame_sample, const double* frame_T16, int S,
                             double range_max, float* xyz_out, float* intensity_out, float* sn_out, int out_stride,
+                            int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+size_t assemble_accumulate_f64_workspace_bytes(int T, int n_stride, int S);
+int assemble_accumulate_f64(const float* xyz, const float* intensity, const int32_t* n_pts, int n_stride, int T,
+                            const int32_t* frame_sample, const double* frame_T16, int S, double range_max,
+                            const float* exclude_box, double* xyz_out, float* intensity_out, int out_stride,
                             int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream);
 size_t assemble_resample_workspace_bytes(int S, int n_stride);
 int assemble_resample_f32(const float* xyz, const float* intensity, const float* sn, const int32_t* n_pts,
