@@ -308,8 +308,126 @@ def predict(coarse, fine=None):
     return coarse_pred, fine_pred
 
 
+def fold_pointnet(pointnet, dtype=torch.float32):
+    """The layers of a _PointNet as plain affine maps for inference: [(W [C_out,C_in], b [C_out], relu)] with each
+    layer's eval-mode BatchNorm folded in float64, W' = W * gamma / sqrt(var + eps) per output row and b' = (b - mean)
+    * gamma / sqrt(var + eps) + beta, then rounded once to `dtype`.  Dropout is the identity in eval mode.  The
+    tensors are new (detached) and live on the pointnet's device: what point_ops.pointwise_mlp takes."""
+    out = []
+    for layer in pointnet.layers:
+        conv, norm = layer.conv, layer.norm
+        W = conv.weight.detach().double().reshape(conv.out_channels, conv.in_channels)
+        b = conv.bias.detach().double() if conv.bias is not None else W.new_zeros(conv.out_channels)
+        if norm is not None:
+            scale = norm.weight.detach().double() / torch.sqrt(norm.running_var.detach().double() + norm.eps)
+            W = W * scale.unsqueeze(1)
+            b = (b - norm.running_mean.detach().double()) * scale + norm.bias.detach().double()
+        out.append((W.to(dtype).contiguous(), b.to(dtype).contiguous(), layer.act is not None))
+    return out
+
+
+class FusedInference:
+    """Inference through KeypointDetector with its per-point layers fused (DESIGN.md 4.21): first_pointnet,
+    second_pointnet and the decoder's two per-point interpolations + concatenation + per_point_pn + predict each run
+    as one point_ops.pointwise_mlp call, so no [B,C,N] tensor wider than 64 channels is built.  Everything else (the
+    node-level layers, the kNN module, ResNet) is the model's own code.
+
+    The fused layers compute in TF32 whatever torch's TF32 flags say, with BatchNorm folded into the weights, so the
+    scores differ from model.forward's at rounding level and a prediction can differ where the top two scores nearly
+    tie.  Inference only: classify raises under grad mode.  The folded layers are cached and rebuilt when a parameter
+    or buffer they were read from has changed (load_state_dict, an optimizer step, .to())."""
+
+    _CHAINS = (("first", lambda m: m.pc_encoder.first_pointnet, ((3, 0, 0), (1, 0, 0), (3, 0, 0))),
+               ("second", lambda m: m.pc_encoder.second_pointnet, ((32, 0, 0), (32, 0, 0))),
+               ("head", lambda m: m.per_point_pn, None))
+
+    def __init__(self, model):
+        if not isinstance(model, KeypointDetector):
+            raise TypeError("FusedInference wraps a network.KeypointDetector")
+        self.model = model
+        self._packed, self._stamp = {}, {}
+
+    def _chain(self, name):
+        model = self.model
+        _, get, spec = next(c for c in self._CHAINS if c[0] == name)
+        if spec is None:
+            spec = ((128, model.node_a_num, model.k_interp_point_a), (512, model.node_b_num, model.k_interp_point_b),
+                    (32, 0, 0), (64, 0, 0))
+        pn = get(model)
+        tensors = list(pn.parameters()) + list(pn.buffers())
+        stamp = tuple((t.data_ptr(), t._version) for t in tensors)
+        if self._stamp.get(name) != stamp:
+            self._packed[name] = point_ops.pack_pointwise_mlp(spec, fold_pointnet(pn))
+            self._stamp[name] = stamp
+        return self._packed[name]
+
+    def classify(self, pc, intensity, sn, node_a, node_b, img, return_scores=False):
+        """(pc [B,3,N], intensity [B,1,N], sn [B,3,N], node_a [B,3,Ma], node_b [B,3,Mb], img [B,3,H,W]) float32 CUDA ->
+        (coarse_pred int8 [B,N], fine_pred int32 [B,N] or None for a coarse-only model), the dtypes
+        frustum.register_batch and pnp.pnp_ransac_batch take; with return_scores=True the scores [B,2+L,N] come third.
+        Runs the model's layers in eval mode (the training flag is restored) under no_grad."""
+        if torch.is_grad_enabled():
+            raise RuntimeError("FusedInference.classify is inference only: call it under torch.no_grad()")
+        model = self.model
+        was_training = model.training
+        model.eval()
+        try:
+            return self._classify(pc, intensity, sn, node_a, node_b, img, return_scores)
+        finally:
+            model.train(was_training)
+
+    def _classify(self, pc, intensity, sn, node_a, node_b, img, return_scores):
+        model, enc = self.model, self.model.pc_encoder
+        B, Ma, Mb = pc.shape[0], node_a.shape[2], node_b.shape[2]
+        if (Ma, Mb) != (model.node_a_num, model.node_b_num):
+            raise ValueError(f"node_a / node_b have {Ma} / {Mb} nodes, the model was built for {model.node_a_num} / "
+                             f"{model.node_b_num}")
+        pc, node_a, node_b = (t.detach().contiguous() for t in (pc, node_a, node_b))
+        ca = point_ops.cluster_assign_forward(pc, node_a, k=model.k_interp_point_a)
+        min_idx = ca["min_idx"]
+        first_pn_out = point_ops.pointwise_mlp([ca["pc_decentered"], intensity, sn], self._chain("first"))
+        _, scattered = point_ops.cluster_max_pool(first_pn_out, min_idx, Ma, broadcast=True)
+        second_pn_out = point_ops.pointwise_mlp([first_pn_out, scattered], self._chain("second"))
+        del scattered
+        node_a_features = point_ops.cluster_max_pool(second_pn_out, min_idx, Ma)
+        node_b_features = enc.knnlayer(node_b, ca["cluster_mean"], node_a_features, model.k_ab)
+        final_pn_out = enc.final_pointnet(torch.cat((node_b, node_b_features), dim=1))
+        global_feature = torch.max(final_pn_out, dim=2, keepdim=True)[0]
+
+        s16, s32 = model.img_encoder.backbone(img)
+        img_global = s32.mean(dim=(2, 3))
+        C_img = img_global.shape[1]
+        s16 = s16.reshape(B, s16.shape[1], -1).contiguous()
+        s32 = s32.reshape(B, C_img, -1).contiguous()
+        img_global_a = img_global.unsqueeze(2).expand(B, C_img, Ma)
+        img_global_b = img_global.unsqueeze(2).expand(B, C_img, Mb)
+
+        att_b = model.node_b_attention_pn(torch.cat((node_b_features, img_global_b), dim=1))
+        weighted_s32 = point_ops.attention_fusion(s32, att_b)
+        up_node_b_features = model.node_b_pn(torch.cat((node_b_features, global_feature.expand(B, -1, Mb),
+                                                        weighted_s32, img_global_b), dim=1))
+        pb_idx = point_ops.cluster_assign_forward(pc, node_b, k=model.k_interp_point_b,
+                                                  want_centers=False)["min_k_idx"]
+        att_a = model.node_a_attention_pn(torch.cat((node_a_features, img_global_a), dim=1))
+        weighted_s16 = point_ops.attention_fusion(s16, att_a)
+        ab_idx = point_ops.cluster_assign_forward(node_a, node_b, k=model.k_interp_ab,
+                                                  want_centers=False)["min_k_idx"]
+        ab = point_ops.upsample_by_interpolation(ab_idx, node_a, node_b, up_node_b_features)
+        up_node_a_features = model.node_a_pn(torch.cat((node_a_features, ab, weighted_s16), dim=1))
+
+        # the decoder's per-point half in one call: rows (pa, pb, first_pn_out, second_pn_out) of per_point_pn's input
+        wa, ia = point_ops.interpolation_weights(ca["min_k_idx"], pc, node_a)
+        wb, ib = point_ops.interpolation_weights(pb_idx, pc, node_b)
+        return point_ops.pointwise_mlp([(up_node_a_features, wa, ia), (up_node_b_features, wb, ib), first_pn_out,
+                                        second_pn_out], self._chain("head"), output="argmax", c_split=2,
+                                       return_scores=return_scores)
+
+
+HEADS = ("torch", "fused")
+
+
 def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chunk=DEFAULT_CHUNK, n_inits=60, seed=0,
-                          t_lb=frustum.DEFAULT_T_LB, t_ub=frustum.DEFAULT_T_UB):
+                          t_lb=frustum.DEFAULT_T_LB, t_ub=frustum.DEFAULT_T_UB, head="torch"):
     """Classify an assembled batch and register every sample: visualize_and_save_data.py's forward and
     registration_lsq.py's solve in one call, with nothing going to the host or to files.
 
@@ -320,12 +438,20 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
     changes rounding only); the model's training flag is restored afterwards.  The coarse predictions go to
     frustum.register_batch with registration_lsq.py's settings (n_inits starts, 2-D, the t bounds of :340).
 
+    head selects a numeric contract, not a tuning.  "torch" (the default) is model.forward and network.predict: the
+    convolutions are cuDNN's and honour torch's TF32 flags.  "fused" is FusedInference.classify per chunk: the
+    per-point layers run as fused TF32 tensor-core kernels whatever the flags say, so predictions can differ from
+    "torch" at points whose top two scores nearly tie.
+
     Returns dict(P [S,4,4] f64, cost [S] f64, coarse_pred int8 [S,N], fine_pred int32 [S,N] or None, degenerate
     int32 [S]); a sample with no point predicted inside gets P = I, cost 1e4 and degenerate = 1."""
     S, N = pc.shape[0], pc.shape[2]
     chunk = int(chunk)
     if chunk < 1:
         raise ValueError(f"chunk must be >= 1, got {chunk}")
+    if head not in HEADS:
+        raise ValueError(f"head must be one of {HEADS}, got {head!r}")
+    fused = FusedInference(model) if head == "fused" else None
     for t, name in ((intensity, "intensity"), (sn, "sn"), (node_a, "node_a"), (node_b, "node_b"), (img, "img")):
         if t.shape[0] != S:
             raise ValueError(f"{name} has {t.shape[0]} samples, pc has {S}")
@@ -338,8 +464,13 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
             fine_pred = torch.empty((S, N), dtype=torch.int32, device=pc.device) if model.fine else None
             for a in range(0, S, chunk):
                 b = min(a + chunk, S)
-                out = model(pc[a:b], intensity[a:b], sn[a:b], node_a[a:b], node_b[a:b], img[a:b])
-                c, f = predict(*out) if model.fine else predict(out)
+                args = (pc[a:b], intensity[a:b], sn[a:b], node_a[a:b], node_b[a:b], img[a:b])
+                if head == "fused":
+                    out = None
+                    c, f = fused.classify(*args)
+                else:
+                    out = model(*args)
+                    c, f = predict(*out) if model.fine else predict(out)
                 coarse_pred[a:b] = c
                 if fine_pred is not None:
                     fine_pred[a:b] = f

@@ -512,3 +512,234 @@ def attention_fusion(img_features, attention):
     for attention); an input that needs no gradient costs nothing in the backward."""
     _check_fusion_args(img_features, attention)
     return _AttentionFusion.apply(img_features, attention)
+
+
+def interpolation_weights(topk_idx, query, node):
+    """The weights half of upsample_by_interpolation: topk_idx [B,Nq,k], query [B,3,Nq], node [B,3,M] -> (w float32
+    [B,Nq,k], idx int32 [B,Nq,k]) with w_j = 1 - d_j / sum_j d_j; a point with an index outside [0, M) gets w = NaN and
+    idx = -1 in every slot.  pointwise_mlp takes these for an interpolated source.  No gradient."""
+    _check_interp_args(topk_idx, query, node, query.new_empty((query.shape[0], 1, node.shape[2])))
+    lib = _native.load()
+    B, Nq, k = topk_idx.shape
+    dev = query.device
+    with torch.cuda.device(dev):
+        w = torch.empty((B, Nq, k), dtype=torch.float32, device=dev)
+        idx = torch.empty((B, Nq, k), dtype=torch.int32, device=dev)
+        if w.numel():
+            rc = lib.interp_weights_f32(topk_idx.data_ptr(), topk_idx.element_size(), query.data_ptr(),
+                                        node.data_ptr(), B, Nq, node.shape[2], k, w.data_ptr(), idx.data_ptr(),
+                                        torch.cuda.current_stream().cuda_stream)
+            _native.check(rc, "interp_weights_f32")
+    return w, idx
+
+
+MLP_MAX_SOURCES = 4
+MLP_MAX_LAYERS = 3
+MLP_MAX_WIDTH = 256
+MLP_MAX_IN = 1024
+MLP_MAX_BATCH = 65535
+_MLP_SRC, _MLP_LAYER = 8, 4       # int64 slots per source / layer (DIB_MLP_SRC, DIB_MLP_LAYER)
+_mlp_ws = {}
+
+
+def _mlp_source_shapes(sources):
+    """[(C, M, k)] per source (M = k = 0: dense) and (B, N), from shapes alone; ValueError on a mismatch."""
+    if not isinstance(sources, (list, tuple)) or not 1 <= len(sources) <= MLP_MAX_SOURCES:
+        raise ValueError(f"sources: need a list of 1 to {MLP_MAX_SOURCES} sources")
+    spec, B, N = [], None, None
+    for i, s in enumerate(sources):
+        if isinstance(s, torch.Tensor):
+            if s.dim() != 3:
+                raise ValueError(f"sources[{i}]: a dense source must be [B,C,N]")
+            b, C, n, M, k = s.shape[0], s.shape[1], s.shape[2], 0, 0
+        else:
+            if not isinstance(s, (list, tuple)) or len(s) != 3 or not all(isinstance(t, torch.Tensor) for t in s):
+                raise ValueError(f"sources[{i}]: need a tensor [B,C,N] or a tuple (features [B,C,M], w, idx)")
+            F, w, idx = s
+            if F.dim() != 3 or w.dim() != 3 or idx.shape != w.shape or w.shape[0] != F.shape[0]:
+                raise ValueError(f"sources[{i}]: need features [B,C,M] and w, idx [B,N,k]")
+            b, C, M, n, k = F.shape[0], F.shape[1], F.shape[2], w.shape[1], w.shape[2]
+            if not 1 <= k <= INTERP_MAX_K:
+                raise ValueError(f"sources[{i}]: need 1 <= k <= {INTERP_MAX_K}, got {k}")
+            if not 1 <= M <= INTERP_MAX_NODES:
+                raise ValueError(f"sources[{i}]: need 1 <= M <= {INTERP_MAX_NODES}, got {M}")
+        if C < 1:
+            raise ValueError(f"sources[{i}]: need at least one channel")
+        if B is None:
+            B, N = b, n
+        elif (b, n) != (B, N):
+            raise ValueError(f"sources[{i}] has B, N = {b}, {n}; sources[0] has {B}, {N}")
+        spec.append((C, M, k))
+    if sum(c for c, _, _ in spec) > MLP_MAX_IN:
+        raise ValueError(f"the concatenated input has {sum(c for c, _, _ in spec)} rows, more than {MLP_MAX_IN}")
+    if N < 1 or not 1 <= B <= MLP_MAX_BATCH:
+        raise ValueError(f"need N >= 1 and 1 <= B <= {MLP_MAX_BATCH}, got B = {B}, N = {N}")
+    return spec, B, N
+
+
+def _mlp_layer_widths(layers, c_in):
+    """[(C_out, relu)] of a list of (W [C_out,C_in], b [C_out] or None, relu); ValueError on a bad width."""
+    if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= MLP_MAX_LAYERS:
+        raise ValueError(f"layers: need a list of 1 to {MLP_MAX_LAYERS} layers")
+    meta = []
+    for i, layer in enumerate(layers):
+        if not isinstance(layer, (list, tuple)) or len(layer) != 3:
+            raise ValueError(f"layers[{i}]: need (W, b, relu)")
+        W, b, relu = layer
+        if not isinstance(W, torch.Tensor) or W.dim() != 2 or W.shape[1] != c_in:
+            raise ValueError(f"layers[{i}]: W must be [C_out, {c_in}]")
+        if not 1 <= W.shape[0] <= MLP_MAX_WIDTH:
+            raise ValueError(f"layers[{i}]: need 1 <= C_out <= {MLP_MAX_WIDTH}, got {W.shape[0]}")
+        if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (W.shape[0],)):
+            raise ValueError(f"layers[{i}]: b must be [{W.shape[0]}] or None")
+        c_in = W.shape[0]
+        meta.append((c_in, bool(relu)))
+    return meta
+
+
+def _mlp_tables(spec, meta):
+    import numpy as np
+    src = np.zeros((len(spec), _MLP_SRC), dtype=np.int64)
+    for i, (C, M, k) in enumerate(spec):
+        src[i, 2], src[i, 3], src[i, 6] = C, M, k
+    lay = np.zeros((len(meta), _MLP_LAYER), dtype=np.int64)
+    for i, (C, relu) in enumerate(meta):
+        lay[i, 2], lay[i, 3] = C, int(relu)
+    return src, lay
+
+
+class PackedPointwiseMLP:
+    """The layers of one pointwise_mlp chain in the kernel's order on the device (weights rounded to TF32 once), for
+    sources of the widths `spec` = [(C, M, k)] (M = k = 0 for a dense source).  pack_pointwise_mlp builds it."""
+
+    def __init__(self, spec, meta, packed):
+        self.spec, self.meta, self.packed = list(spec), list(meta), packed
+
+
+def pack_pointwise_mlp(spec, layers):
+    """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] for sources of the widths `spec`
+    (as PackedPointwiseMLP.spec); pointwise_mlp does this itself when given the raw layers."""
+    spec = [tuple(int(v) for v in s) for s in spec]
+    meta = _mlp_layer_widths(layers, sum(c for c, _, _ in spec))
+    dev = layers[0][0].device
+    keep = []
+    for W, b, _ in layers:
+        for t in (W, b):
+            if t is None:
+                continue
+            if t.requires_grad and torch.is_grad_enabled():
+                raise RuntimeError("pointwise_mlp has no backward: call it under torch.no_grad() or detach the layers")
+            if not t.is_cuda or t.device != dev or t.dtype != torch.float32:
+                raise RuntimeError("the layers must be float32 CUDA tensors on one device")
+        keep.append((W.detach().contiguous(), None if b is None else b.detach().contiguous()))
+    src, lay = _mlp_tables(spec, meta)
+    for i, (W, b) in enumerate(keep):
+        lay[i, 0], lay[i, 1] = W.data_ptr(), 0 if b is None else b.data_ptr()
+    lib = _native.load()
+    need = lib.pointwise_mlp_packed_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta))
+    if need == 0:
+        raise ValueError("pointwise_mlp: " + lib.dib_last_error().decode("utf-8", "replace"))
+    with torch.cuda.device(dev):
+        packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
+        rc = lib.pointwise_mlp_pack_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.data_ptr(), need,
+                                        torch.cuda.current_stream().cuda_stream)
+    _native.check(rc, "pointwise_mlp_pack_f32")
+    return PackedPointwiseMLP(spec, meta, packed)
+
+
+def pointwise_mlp(sources, layers, output="activations", c_split=None, return_scores=False):
+    """A chain of one to three 1x1-convolution layers y = act(W x + b) over every point, in one kernel, for inference
+    (DESIGN.md 4.21): the PointNets the classifier applies per point, with BatchNorm already folded into W and b
+    (network.fold_pointnet) and the input concatenation never built.
+
+    sources: 1 to 4 of, in the order of layer 1's input rows, a dense float32 CUDA tensor [B,C,N] (a channel slice of
+    a wider contiguous tensor is read in place) or a tuple (features [B,C,M], w [B,N,k], idx [B,N,k]) whose rows are
+    the interpolation upsample_by_interpolation computes (w, idx from interpolation_weights; k <= 8, M <= 2048, a
+    point with idx = -1 has NaN rows).  At most 1024 rows in all.  layers: [(W [C_out,C_in], b [C_out] or None, relu)]
+    with every C_out in [1, 256], or a PackedPointwiseMLP.
+
+    output="activations" returns the last layer [B,C_out,N].  output="argmax" returns (int8 [B,N], int32 [B,N] or
+    None): the arg-max over channels [0, c_split) and over [c_split, C_out) (None when that range is empty) by
+    torch.max's rule, so c_split = 2 is network.predict; with return_scores=True the scores [B,C_out,N] come third.
+
+    The products run on the tensor cores in TF32 with float32 accumulation whatever torch's TF32 flags say: weights,
+    source values and the activations between layers are rounded to TF32 (nearest, ties away from zero); bias, ReLU
+    (NaN stays NaN) and the arg-max are float32.  No backward: an input that requires grad raises RuntimeError unless
+    grad mode is off.  Shape and bound errors raise ValueError before anything is launched."""
+    spec, B, N = _mlp_source_shapes(sources)
+    if isinstance(layers, PackedPointwiseMLP):
+        if layers.spec != spec:
+            raise ValueError(f"the layers were packed for sources {layers.spec}, got {spec}")
+        packed = layers
+    else:
+        packed = None
+    meta = packed.meta if packed is not None else _mlp_layer_widths(layers, sum(c for c, _, _ in spec))
+    C_out = meta[-1][0]
+    if output not in ("activations", "argmax"):
+        raise ValueError(f"output must be 'activations' or 'argmax', got {output!r}")
+    if output == "argmax":
+        if c_split is None or isinstance(c_split, bool) or int(c_split) != c_split \
+                or not 1 <= c_split <= min(C_out, 128):
+            raise ValueError(f"c_split: need an integer in [1, min(C_out, 128)] with C_out = {C_out}, got {c_split}")
+        c_split = int(c_split)
+    elif c_split is not None or return_scores:
+        raise ValueError("c_split and return_scores go with output='argmax'")
+    flat = [t for s in sources for t in ((s,) if isinstance(s, torch.Tensor) else s)]
+    dev = flat[0].device
+    for t in flat:
+        if t.requires_grad and torch.is_grad_enabled():
+            raise RuntimeError("pointwise_mlp has no backward: call it under torch.no_grad() or detach the inputs")
+        if not t.is_cuda:
+            raise RuntimeError("pointwise_mlp: every source must be a CUDA tensor")
+        if t.device != dev:
+            raise RuntimeError(f"pointwise_mlp: every source must be on {dev}")
+    src, lay = _mlp_tables(spec, meta)
+    keep = []
+    for i, s in enumerate(sources):
+        if isinstance(s, torch.Tensor):
+            if s.dtype != torch.float32:
+                raise RuntimeError(f"sources[{i}] must have dtype {torch.float32}")
+            C = s.shape[1]
+            if (N > 1 and s.stride(2) != 1) or (C > 1 and s.stride(1) != N) or (B > 1 and s.stride(0) < C * N):
+                s = s.contiguous()
+            keep.append(s)
+            src[i, 0], src[i, 1] = s.data_ptr(), s.stride(0) if B > 1 else C * N
+        else:
+            F, w, idx = s
+            if F.dtype != torch.float32 or w.dtype != torch.float32 or idx.dtype != torch.int32:
+                raise RuntimeError(f"sources[{i}] must be (float32 features, float32 w, int32 idx)")
+            F, w, idx = F.contiguous(), w.contiguous(), idx.contiguous()
+            keep.append((F, w, idx))
+            src[i, 0], src[i, 1], src[i, 4], src[i, 5] = F.data_ptr(), F.shape[1] * F.shape[2], w.data_ptr(), \
+                idx.data_ptr()
+    if packed is None:
+        packed = pack_pointwise_mlp(spec, layers)
+    if packed.packed.device != dev:
+        raise RuntimeError(f"the layers must be on {dev}")
+    lib = _native.load()
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream().cuda_stream
+        need = lib.pointwise_mlp_workspace_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), B)
+        ws = None
+        if need:
+            key = (dev.index, stream)
+            ws = _mlp_ws.get(key)
+            if ws is None or ws.numel() < need:
+                ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                _mlp_ws[key] = ws
+        want_out = output == "activations" or return_scores
+        out = torch.empty((B, C_out, N), dtype=torch.float32, device=dev) if want_out else None
+        pred_a = torch.empty((B, N), dtype=torch.int8, device=dev) if output == "argmax" else None
+        pred_b = torch.empty((B, N), dtype=torch.int32, device=dev) if output == "argmax" and c_split < C_out else None
+        rc = lib.pointwise_mlp_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.packed.data_ptr(),
+                                   packed.packed.numel() * 4, B, N, c_split or 0,
+                                   out.data_ptr() if out is not None else None,
+                                   pred_a.data_ptr() if pred_a is not None else None,
+                                   pred_b.data_ptr() if pred_b is not None else None,
+                                   ws.data_ptr() if ws is not None else None, ws.numel() if ws is not None else 0,
+                                   stream)
+    _native.check(rc, "pointwise_mlp_f32")
+    del keep
+    if output == "activations":
+        return out
+    return (pred_a, pred_b, out) if return_scores else (pred_a, pred_b)

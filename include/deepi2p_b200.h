@@ -623,6 +623,58 @@ int jpeg_decode_batch_u8(const uint8_t* data, size_t data_bytes, const int64_t* 
                          const int32_t* quant, int S, int window_bits, uint8_t* out, size_t out_bytes,
                          int32_t* status, void* workspace, size_t workspace_bytes, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Fused inference of the classifier's per-point layers (the PointNets of models/layers_pc.py:345-408 applied per
+ * point in models/networks_united.py:193-197 and networks_pc.py:86-103; SURVEY.md 8f N16).  DESIGN.md 4.21 states the
+ * contract.  A chain of 1..3 layers y = act(W x + b) over the N points of each of B samples, inference only, with
+ * BatchNorm already folded into W and b by the caller.  The rows of layer 1's input are the concatenation, in order,
+ * of 1..4 sources that is never written to memory; the total is at most 1024 rows, every C_out is in [1, 256].
+ *
+ * sources: [host] int64 [n_sources][DIB_MLP_SRC]; pointers are [dev] addresses stored as integers.
+ *   dense source (NODES = 0): DATA f32, element (b, c, n) at b * BSTRIDE + c * N + n (BSTRIDE >= CHANNELS * N: a
+ *     channel slice of a wider tensor passes the wider tensor's batch stride).
+ *   interpolated source (NODES = M in [1, 2048]): DATA node features f32, element (b, c, m) at b * BSTRIDE + c * M + m;
+ *     W f32 [B][N][K] and IDX int32 [B][N][K] as interp_weights_f32 writes them, 1 <= K <= 8.  Its rows are
+ *     sum_j w_j F[c][idx_j]; a point with an index outside [0, M) has NaN in all of them.
+ * layers: [host] int64 [n_layers][DIB_MLP_LAYER]: W [dev] f32 [C_out][C_in] contiguous, B [dev] f32 [C_out] or 0 (no
+ *   bias), COUT, RELU (1: ReLU that keeps NaN, 0: identity).  pointwise_mlp_f32 reads only COUT and RELU.
+ *
+ * pointwise_mlp_pack_f32 writes the layers in the kernel's order into packed ([dev] 16-byte aligned, >=
+ *   pointwise_mlp_packed_bytes): every weight rounded to TF32 (nearest, ties away from zero) once.  It depends on the
+ *   sources' CHANNELS, NODES and K only.
+ * pointwise_mlp_f32 evaluates the chain.  The products run on the tensor cores in TF32 with f32 accumulation; source
+ *   values and the activations fed to the next layer are rounded to TF32 like the weights; bias, ReLU and the
+ *   arg-max are f32.  An interpolated source's block of W1 is applied to its node features first (a TF32 product
+ *   per node, kept in f32 in the workspace) and the projected rows are interpolated per point in f32.
+ *   c_split = 0: out [B][C_out][N] f32, the last layer's activations.
+ *   1 <= c_split <= min(C_out, 128): pred_a int8 [B][N] = arg-max over channels [0, c_split) and pred_b int32 [B][N]
+ *     = arg-max over [c_split, C_out) minus c_split (not written, and may be NULL, when c_split = C_out), both by
+ *     torch.max's rule (NaN is maximal, the first maximal index wins); out, when not NULL, also receives the scores.
+ *   workspace: [dev] 16-byte aligned, >= pointwise_mlp_workspace_bytes (0 without interpolated sources).
+ *   Deterministic: no atomics; 0 <= B <= 65535, N >= 0.
+ * ------------------------------------------------------------------------------------------ */
+#define DIB_MLP_SRC 8
+#define DIB_MLP_SRC_DATA 0
+#define DIB_MLP_SRC_BSTRIDE 1
+#define DIB_MLP_SRC_CHANNELS 2
+#define DIB_MLP_SRC_NODES 3
+#define DIB_MLP_SRC_W 4
+#define DIB_MLP_SRC_IDX 5
+#define DIB_MLP_SRC_K 6
+#define DIB_MLP_LAYER 4
+#define DIB_MLP_LAYER_W 0
+#define DIB_MLP_LAYER_B 1
+#define DIB_MLP_LAYER_COUT 2
+#define DIB_MLP_LAYER_RELU 3
+size_t pointwise_mlp_packed_bytes(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers);
+int pointwise_mlp_pack_f32(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, void* packed,
+                           size_t packed_bytes, dib_stream_t stream);
+size_t pointwise_mlp_workspace_bytes(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers,
+                                     int B);
+int pointwise_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, const void* packed,
+                      size_t packed_bytes, int B, int N, int c_split, float* out, int8_t* pred_a, int32_t* pred_b,
+                      void* workspace, size_t workspace_bytes, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
