@@ -27,6 +27,7 @@ EXPORTS = (
     "estimate_normals_workspace_bytes",
     "estimate_normals_batch_f32", "nearest_batch_f32", "sym3_eig_batch_f64",
     "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32",
+    "assemble_accumulate_gather_workspace_bytes", "assemble_accumulate_gather_f32",
     "assemble_accumulate_f64_workspace_bytes", "assemble_accumulate_f64", "assemble_resample_workspace_bytes",
     "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
     "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
@@ -177,6 +178,11 @@ def load():
     lib.assemble_accumulate_f32.restype = i32
     lib.assemble_accumulate_f32.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp, vp, i32, vp, vp, sz,
                                             vp]
+    lib.assemble_accumulate_gather_workspace_bytes.restype = sz
+    lib.assemble_accumulate_gather_workspace_bytes.argtypes = [i32, i32, i32]
+    lib.assemble_accumulate_gather_f32.restype = i32
+    lib.assemble_accumulate_gather_f32.argtypes = [vp, vp, vp, _c.c_int64, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp,
+                                                   vp, i32, vp, vp, sz, vp]
     lib.assemble_accumulate_f64_workspace_bytes.restype = sz
     lib.assemble_accumulate_f64_workspace_bytes.argtypes = [i32, i32, i32]
     lib.assemble_accumulate_f64.restype = i32

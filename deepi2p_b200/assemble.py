@@ -218,6 +218,197 @@ def accumulate(xyz, intensity, sn, n_pts, frame_sample, frame_T, range_max=None,
     return out_x, out_i, out_n, cnt, cnt_h
 
 
+STORE_LOCATIONS = ("cuda", "pinned")
+STAGE_POINTS = 1 << 21        # points per host-to-device transfer while a device ScanStore is filled
+
+
+def store_layout(shapes):
+    """The ragged layout of records of `shapes` ([rows, n] each, every rows 4 or every rows 7): returns (rows, offsets
+    int64 [R] (running sums of n, from 0), counts int32 [R])."""
+    shapes = [tuple(sh) for sh in shapes]
+    if not shapes:
+        raise ValueError("a scan store needs at least one record")
+    rows = {sh[0] if len(sh) == 2 else None for sh in shapes}
+    if len(rows) != 1 or next(iter(rows)) not in (4, 7):
+        raise ValueError("every record must be [4, n] (xyz, intensity) or every record [7, n] (xyz, intensity, sn)")
+    counts = np.array([sh[1] for sh in shapes], dtype=np.int64)
+    if counts.max() >= 2**31:
+        raise ValueError("a record has 2^31 or more points")
+    offsets = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
+    return int(shapes[0][0]), offsets, counts.astype(np.int32)
+
+
+def unique_records(keys):
+    """Deduplicate a batch's frame keys: returns (distinct keys in first-use order, ids [T] int64 into them)."""
+    first, ids = {}, []
+    for k in keys:
+        ids.append(first.setdefault(k, len(first)))
+    return list(first), np.array(ids, dtype=np.int64)
+
+
+class ScanStore:
+    """A ragged scan store: R records [rows, n_r] (rows 0-2 xyz, 3 intensity, 4-6 surface normals when rows == 7),
+    rounded to float32 and laid end to end in SoA planes data [rows, total] (plane stride `total`), in device memory
+    (location "cuda") or in pinned host memory ("pinned", read by the device through its mapped address).  No record
+    is padded.  keys (optional, one hashable per record) name the records for index().  offsets int64 [R] and counts
+    int32 [R] (host) locate record r at data[:, offsets[r]:offsets[r] + counts[r]]; nbytes is the planes' size.
+    Records may be numpy memory maps: they are read once, record by record."""
+
+    def __init__(self, records, location="cuda", keys=None, device=None):
+        if location not in STORE_LOCATIONS:
+            raise ValueError(f"location must be one of {STORE_LOCATIONS} (got {location!r})")
+        records = list(records)
+        self.rows, self.offsets, self.counts = store_layout([np.shape(r) for r in records])
+        self.total = int(self.counts.astype(np.int64).sum())
+        self.location = location
+        device = torch.device("cuda" if device is None else device)
+        self.device = device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
+        if keys is not None:
+            keys = list(keys)
+            if len(keys) != len(records) or len(set(keys)) != len(keys):
+                raise ValueError("keys needs one distinct key per record")
+        self.keys = keys
+        self._index = None if keys is None else {k: r for r, k in enumerate(keys)}
+        width = max(self.total, 1)
+        on_device = location == "cuda"
+        self.data = (torch.empty((self.rows, width), dtype=torch.float32, device=self.device) if on_device else
+                     torch.empty((self.rows, width), dtype=torch.float32, pin_memory=True))
+        # Each record is rounded to float32 and checked on the host.  A pinned store takes it in place; a device store
+        # gets it through a pinned staging buffer, copied over in transfers of up to STAGE_POINTS points.
+        stage = (torch.empty((self.rows, min(width, STAGE_POINTS)), dtype=torch.float32, pin_memory=True)
+                 if on_device else self.data)
+        host = stage.numpy()
+        base, fill = 0, 0                       # the staged columns are store columns [base, base + fill)
+        for r, rec in enumerate(records):
+            a = np.asarray(rec, dtype=np.float32)
+            if not np.isfinite(a[:3]).all():
+                raise ValueError(f"record {r} has a non-finite coordinate")
+            if not on_device:
+                host[:, self.offsets[r]:self.offsets[r] + self.counts[r]] = a
+                continue
+            pos = 0
+            while pos < a.shape[1]:
+                if fill == host.shape[1]:
+                    self.data[:, base:base + fill].copy_(stage)
+                    base, fill = base + fill, 0
+                k = min(a.shape[1] - pos, host.shape[1] - fill)
+                host[:, fill:fill + k] = a[:, pos:pos + k]
+                fill, pos = fill + k, pos + k
+        if on_device and fill:
+            self.data[:, base:base + fill].copy_(stage[:, :fill])
+
+    def __len__(self):
+        return len(self.counts)
+
+    @property
+    def nbytes(self):
+        return self.data.numel() * 4
+
+    @property
+    def has_sn(self):
+        return self.rows == 7
+
+    def index(self, key):
+        if self._index is None:
+            raise ValueError("this store has no keys")
+        try:
+            return self._index[key]
+        except KeyError:
+            raise KeyError(f"no record {key!r} in the scan store") from None
+
+    def to(self, location, stream=None):
+        """A copy of the store in `location` ("cuda" or "pinned") with the same keys, offsets and counts; a pinned
+        store goes to the device asynchronously on `stream`."""
+        if location not in STORE_LOCATIONS:
+            raise ValueError(f"location must be one of {STORE_LOCATIONS} (got {location!r})")
+        out = ScanStore.__new__(ScanStore)
+        out.__dict__.update(self.__dict__)
+        out.location = location
+        with torch.cuda.device(self.device), torch.cuda.stream(stream):
+            if location == "cuda":
+                out.data = self.data.to(self.device, non_blocking=self.location == "pinned")
+            else:
+                out.data = self.data.to("cpu").pin_memory()
+        return out
+
+    def plane_ptrs(self):
+        """(xyz, intensity, sn or 0) addresses of the planes."""
+        base, ps = self.data.data_ptr(), self.data.stride(0) * 4
+        return base, base + 3 * ps, (base + 4 * ps if self.has_sn else 0)
+
+
+class StoreFrames:
+    """Store-backed frames for assemble_batch (store_frames builds them)."""
+
+    def __init__(self, store, ids, frame_sample, frame_T):
+        self.store, self.ids, self.frame_sample, self.frame_T = store, ids, frame_sample, frame_T
+
+
+def store_frames(store, ids, frame_sample, frame_T):
+    """assemble_batch's frames from a ScanStore: frame t is record ids[t] (a record may back several frames, in any
+    order), frame_sample [T] non-decreasing from 0 without gaps (anchor frame first), frame_T [T,4,4] float64 (host).
+    assemble_batch gives the same bits as on pack_frames of the same records."""
+    if not isinstance(store, ScanStore):
+        raise ValueError("store must be an assemble.ScanStore")
+    ids = np.asarray(ids, dtype=np.int64).reshape(-1)
+    fs = np.asarray(frame_sample, dtype=np.int64).reshape(-1)
+    T = ids.shape[0]
+    if T == 0 or fs.shape != (T,):
+        raise ValueError("ids and frame_sample need one entry per frame (T >= 1)")
+    if ids.min() < 0 or ids.max() >= len(store):
+        raise ValueError(f"record ids must be in [0, {len(store)})")
+    if fs[0] != 0 or np.any(np.diff(fs) < 0) or np.any(np.diff(fs) > 1):
+        raise ValueError("frame_sample must be non-decreasing from 0 without gaps")
+    FT = np.ascontiguousarray(frame_T, dtype=np.float64)
+    if FT.shape != (T, 4, 4) or not np.isfinite(FT).all():
+        raise ValueError("frame_T must be [T,4,4] finite")
+    return StoreFrames(store, ids, fs, FT)
+
+
+def batch_frames(records, ids, frame_sample, frame_T, device="cuda", stream=None):
+    """Store-backed frames without a long-lived store: the batch's distinct records (each once, unpadded) go to a
+    pinned ScanStore, which is copied to the device in one transfer on `stream`; frame t is records[ids[t]].  Returns
+    store_frames' frames."""
+    staged = ScanStore(records, "pinned", device=device)
+    return store_frames(staged.to("cuda", stream), ids, frame_sample, frame_T)
+
+
+
+def accumulate_gather(frames, range_max=None, stream=None):
+    """accumulate() on store_frames' frames (float32, with sn when the store has it): the same outputs, bit for bit,
+    as accumulate on the frames padded into [T,3,n]."""
+    _require_cuda()
+    lib = _native.load()
+    st = frames.store
+    dev = st.device
+    npts = st.counts[frames.ids].astype(np.int64)
+    T = frames.ids.shape[0]
+    n_max = max(int(npts.max()), 1)
+    r = 0.0 if range_max is None else pointprep._positive(range_max, "range_max")
+    fs = frames.frame_sample
+    S = int(fs[-1]) + 1
+    A = round_up(max(int(np.bincount(fs, weights=npts).max()), 1), 16)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):
+        meta = torch.from_numpy(np.concatenate([st.offsets[frames.ids], npts, fs]).astype(np.int64)).to(dev)
+        off_d = meta[:T]
+        n_d = meta[T:2 * T].to(torch.int32)
+        fs_d = meta[2 * T:].to(torch.int32)
+        FT_d = torch.from_numpy(frames.frame_T).to(dev)
+        out_x = torch.zeros((S, 3, A), dtype=torch.float32, device=dev)
+        out_i = torch.zeros((S, A), dtype=torch.float32, device=dev)
+        out_n = torch.zeros((S, 3, A), dtype=torch.float32, device=dev) if st.has_sn else None
+        cnt = torch.zeros((S,), dtype=torch.int32, device=dev)
+        sp = _stream_ptr(stream)
+        ws = _workspace(lib.assemble_accumulate_gather_workspace_bytes(T, n_max, S), dev, sp)
+        px, pi, pn = st.plane_ptrs()
+        rc = lib.assemble_accumulate_gather_f32(px, pi, pn or None, st.data.stride(0), _ptr(off_d), _ptr(n_d), n_max,
+                                                T, _ptr(fs_d), _ptr(FT_d), S, r, _ptr(out_x), _ptr(out_i),
+                                                _ptr(out_n), A, _ptr(cnt), _ptr(ws), ws.numel(), sp)
+        _native.check(rc, "assemble_accumulate_gather")
+        cnt_h = cnt.cpu().numpy()
+    return out_x, out_i, out_n, cnt, cnt_h
+
+
 def _voxel_step(xyz, inten, sn, cnt, cnt_h, N, voxel_size, stream):
     """The loaders' `if n > 2 N` branch: downsample_with_intensity_sn / downsample_with_reflectance on the samples that
     take it, with the drop-ins' arithmetic (intensity / max in float32, means in float64, times max, then float32).
@@ -384,7 +575,8 @@ def assemble_batch(frames, mode, seed, input_pt_num=INPUT_PT_NUM, node_a_num=NOD
                    val_amplitudes=None):
     """The loaders' point side for S samples.  frames: dict(xyz [T,3,n] f32, intensity [T,n] f32, sn [T,3,n] f32 or
     None -- CUDA; n_pts [T], frame_sample [T] (non-decreasing from 0, anchor frame first) and frame_T [T,4,4] float64
-    on the host).  kitti_args / oxford_args / nuscenes_args give pre, P_base and the rest as the loaders compose them.
+    on the host), or store_frames' / batch_frames' frames gathered from a ScanStore (float32 accumulation only; the
+    same bits as the dict of the same records).  kitti_args / oxford_args / nuscenes_args give pre, P_base and the rest as the loaders compose them.
     Steps: accumulate (exclusion box, range mask; fp64 with accumulate_f64), the voxel step for clouds above 2
     input_pt_num points (on the fp64 cloud with accumulate_f64; every cloud is then rounded to float32), downsample_np,
     Pr from random_transforms(mode, amplitudes, rng, flip, val_amplitudes) with jitter in train mode, points -> (Pr
@@ -403,9 +595,14 @@ def assemble_batch(frames, mode, seed, input_pt_num=INPUT_PT_NUM, node_a_num=NOD
         raise ValueError(f"accumulate_f64 must be a bool (got {accumulate_f64!r})")
     if _exclude_box(exclude_box) is not None and not accumulate_f64:
         raise ValueError("exclude_box needs accumulate_f64=True")
-    xyz, inten, sn, cnt, cnt_h = accumulate(frames["xyz"], frames["intensity"], frames.get("sn"), frames["n_pts"],
-                                            frames["frame_sample"], frames["frame_T"], range_max, stream, exclude_box,
-                                            accumulate_f64)
+    if isinstance(frames, StoreFrames):
+        if accumulate_f64 or exclude_box is not None:
+            raise ValueError("store-backed frames take the float32 accumulation (no accumulate_f64, no exclude_box)")
+        xyz, inten, sn, cnt, cnt_h = accumulate_gather(frames, range_max, stream)
+    else:
+        xyz, inten, sn, cnt, cnt_h = accumulate(frames["xyz"], frames["intensity"], frames.get("sn"),
+                                                frames["n_pts"], frames["frame_sample"], frames["frame_T"], range_max,
+                                                stream, exclude_box, accumulate_f64)
     if cnt_h.min() < 1:
         raise ValueError(f"sample {int(np.argmin(cnt_h))} has no point left to assemble")
     S = cnt_h.shape[0]

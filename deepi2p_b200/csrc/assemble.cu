@@ -5,7 +5,9 @@
 // accumulate  one thread per (frame, point): p' = T p in fp64 with a fixed association, rounded once to float32 (or
 //             kept in fp64: assemble_accumulate_f64); normals get the rotation only; an optional float32 x / y
 //             exclusion box on the source coordinates and an optional float32 range mask (x'^2 + z'^2 < r^2); a scan
-//             over the keep flags compacts every sample's frames into one cloud in (frame, index) order
+//             over the keep flags compacts every sample's frames into one cloud in (frame, index) order.  Frames are
+//             rows of a padded [T][3][n] block, or (assemble_accumulate_gather_f32) ranges of a ragged scan store
+//             addressed by int64 offsets; only the frame's base address differs, so both compute the same bits
 // resample    a 64-bit Philox key per point, a stable segmented radix sort by key (ties: ascending index); output o
 //             takes o mod n while o < r n (the fixed repeats of downsample_np) and the (o - r n)-th point in key order
 //             after that; float32 jitter from Box-Muller on Philox words; p' = M p in fp64, rounded to float32
@@ -122,15 +124,40 @@ struct AccArgs {
   float *xyz_out, *intensity_out, *sn_out;
   double* xyz64_out;         // the fp64 variant's coordinates (instead of xyz_out; no sn)
   int out_stride;
+  // Gather addressing (GATHER = true): frame t is points [frame_offset[t], frame_offset[t] + n_pts[t]) of store
+  // planes xyz [3][plane_stride], intensity [plane_stride], sn [3][plane_stride]; n_stride is then the largest
+  // frame length, so the (frame, index) iteration space is the padded entry's.
+  const int64_t* frame_offset;
+  int64_t plane_stride;
 };
 
+// Frame t's first coordinate (plane 0), its plane stride and its first intensity.
+template <bool GATHER>
+__device__ __forceinline__ size_t frame_base(const AccArgs& a, int t) {
+  if constexpr (GATHER) return (size_t)a.frame_offset[t];
+  else return (size_t)t * 3 * a.n_stride;
+}
+template <bool GATHER>
+__device__ __forceinline__ size_t plane(const AccArgs& a) {
+  if constexpr (GATHER) return (size_t)a.plane_stride;
+  else return (size_t)a.n_stride;
+}
+template <bool GATHER>
+__device__ __forceinline__ size_t intensity_base(const AccArgs& a, int t) {
+  if constexpr (GATHER) return (size_t)a.frame_offset[t];
+  else return (size_t)t * a.n_stride;
+}
+
+template <bool GATHER>
 __device__ __forceinline__ void acc_point(const AccArgs& a, int t, int j, double p[3]) {
   const double* M = a.frame_T + (size_t)t * 16;
-  const float* X = a.xyz + (size_t)t * 3 * a.n_stride;
-  const double x = X[j], y = X[(size_t)a.n_stride + j], z = X[(size_t)2 * a.n_stride + j];
+  const float* X = a.xyz + frame_base<GATHER>(a, t);
+  const size_t ps = plane<GATHER>(a);
+  const double x = X[j], y = X[ps + j], z = X[2 * ps + j];
   for (int r = 0; r < 3; ++r) p[r] = affine_row(M, r, x, y, z);
 }
 
+template <bool GATHER>
 __global__ void acc_flag_kernel(AccArgs a, int32_t* __restrict__ flag) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long N = (long long)a.T * a.n_stride;
@@ -142,13 +169,13 @@ __global__ void acc_flag_kernel(AccArgs a, int32_t* __restrict__ flag) {
     if (j < clamp_count(a.n_pts, t, a.n_stride) && s >= 0 && s < a.S) {
       f = 1;
       if (a.box) {
-        const float* X = a.xyz + (size_t)t * 3 * a.n_stride;
-        const float x = X[j], y = X[(size_t)a.n_stride + j];
+        const float* X = a.xyz + frame_base<GATHER>(a, t);
+        const float x = X[j], y = X[plane<GATHER>(a) + j];
         f = !(x > a.x_lo && x < a.x_hi && y > a.y_lo && y < a.y_hi);
       }
       if (f && a.range2 > 0.0f) {
         double p[3];
-        acc_point(a, t, j, p);
+        acc_point<GATHER>(a, t, j, p);
         const float px = (float)p[0], pz = (float)p[2];
         f = px * px + pz * pz < a.range2;
       }
@@ -169,7 +196,7 @@ __global__ void acc_first_kernel(const int32_t* __restrict__ frame_sample, int T
   first[s] = s == S ? T : lo;
 }
 
-template <bool F64>
+template <bool F64, bool GATHER>
 __global__ void acc_scatter_kernel(AccArgs a, const int32_t* __restrict__ flag, const int32_t* __restrict__ pos,
                                    const int32_t* __restrict__ first, int32_t* __restrict__ count_out) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -183,27 +210,30 @@ __global__ void acc_scatter_kernel(AccArgs a, const int32_t* __restrict__ flag, 
   const int o = pos[g] - pos[(size_t)first[s] * a.n_stride];
   if (o < 0 || o >= a.out_stride) return;
   double p[3];
-  acc_point(a, t, j, p);
+  acc_point<GATHER>(a, t, j, p);
   for (int r = 0; r < 3; ++r) {
     if constexpr (F64)
       a.xyz64_out[((size_t)s * 3 + r) * a.out_stride + o] = p[r];
     else
       a.xyz_out[((size_t)s * 3 + r) * a.out_stride + o] = (float)p[r];
   }
-  a.intensity_out[(size_t)s * a.out_stride + o] = a.intensity[(size_t)t * a.n_stride + j];
+  a.intensity_out[(size_t)s * a.out_stride + o] = a.intensity[intensity_base<GATHER>(a, t) + j];
   if (a.sn) {
     const double* M = a.frame_T + (size_t)t * 16;
-    const float* Nn = a.sn + (size_t)t * 3 * a.n_stride;
-    const double x = Nn[j], y = Nn[(size_t)a.n_stride + j], z = Nn[(size_t)2 * a.n_stride + j];
+    const float* Nn = a.sn + frame_base<GATHER>(a, t);
+    const size_t ps = plane<GATHER>(a);
+    const double x = Nn[j], y = Nn[ps + j], z = Nn[2 * ps + j];
     for (int r = 0; r < 3; ++r) a.sn_out[((size_t)s * 3 + r) * a.out_stride + o] = (float)rot_row(M, r, x, y, z);
   }
 }
 
-template <bool F64>
+template <bool F64, bool GATHER = false>
 int accumulate(const AccArgs& a, int32_t* count_out, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   DIB_REQUIRE(a.xyz && a.intensity && a.frame_sample && a.frame_T && (F64 ? (void*)a.xyz64_out : (void*)a.xyz_out) &&
               a.intensity_out && count_out,
               "NULL argument (xyz, intensity, frame_sample, frame_T, xyz_out, intensity_out, count_out)");
+  DIB_REQUIRE(!GATHER || (a.frame_offset && a.n_pts && a.plane_stride >= 1),
+              "NULL argument (frame_offset, frame_n) or plane_stride < 1");
   DIB_REQUIRE(!a.sn || a.sn_out, "NULL argument (sn_out with sn)");
   DIB_REQUIRE(!a.box || (std::isfinite(a.x_lo) && std::isfinite(a.x_hi) && std::isfinite(a.y_lo) &&
                          std::isfinite(a.y_hi) && a.x_lo <= a.x_hi && a.y_lo <= a.y_hi),
@@ -220,7 +250,7 @@ int accumulate(const AccArgs& a, int32_t* count_out, void* workspace, size_t wor
   carve_acc((char*)workspace, a.T, a.n_stride, a.S, &wk);
   const long long N = (long long)a.T * a.n_stride + 1;
   const int nb = (int)((N + 255) / 256);
-  acc_flag_kernel<<<nb, 256, 0, st>>>(a, wk.flag);
+  acc_flag_kernel<GATHER><<<nb, 256, 0, st>>>(a, wk.flag);
   acc_first_kernel<<<(a.S + 1 + 127) / 128, 128, 0, st>>>(a.frame_sample, a.T, a.S, wk.first);
   DIB_CHECK_CUDA(cudaGetLastError());
   size_t tmp = 0;
@@ -228,7 +258,7 @@ int accumulate(const AccArgs& a, int32_t* count_out, void* workspace, size_t wor
   DIB_REQUIRE(tmp <= kScratch, "accumulate: scan scratch %zu exceeds %zu", tmp, kScratch);
   DIB_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(wk.tmp, tmp, wk.flag, wk.pos, (int)N, st));
   const long long M = N - 1 > a.S ? N - 1 : a.S;
-  acc_scatter_kernel<F64><<<(int)((M + 255) / 256), 256, 0, st>>>(a, wk.flag, wk.pos, wk.first, count_out);
+  acc_scatter_kernel<F64, GATHER><<<(int)((M + 255) / 256), 256, 0, st>>>(a, wk.flag, wk.pos, wk.first, count_out);
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
 }
@@ -597,8 +627,41 @@ int assemble_accumulate_f32(const float* xyz, const float* intensity, const floa
   DIB_REQUIRE(std::isfinite(range_max), "range_max must be finite (<= 0: no range mask)");
   const float r2 = range_max > 0.0 ? (float)(range_max * range_max) : 0.0f;
   const dib::asmb::AccArgs a{xyz, intensity, sn, n_pts, n_stride, T, frame_sample, frame_T16, S, r2, false,
-                             0.0f, 0.0f, 0.0f, 0.0f, xyz_out, intensity_out, sn_out, nullptr, out_stride};
+                             0.0f, 0.0f, 0.0f, 0.0f, xyz_out, intensity_out, sn_out, nullptr, out_stride, nullptr, 0};
   return dib::asmb::accumulate<false>(a, count_out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t assemble_accumulate_gather_workspace_bytes(int T, int n_max, int S) {
+  return assemble_accumulate_workspace_bytes(T, n_max, S);
+}
+
+int assemble_accumulate_gather_f32(const float* xyz, const float* intensity, const float* sn, int64_t plane_stride,
+                                   const int64_t* frame_offset, const int32_t* frame_n, int n_max, int T,
+                                   const int32_t* frame_sample, const double* frame_T16, int S, double range_max,
+                                   float* xyz_out, float* intensity_out, float* sn_out, int out_stride,
+                                   int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream) {
+  DIB_REQUIRE(std::isfinite(range_max), "range_max must be finite (<= 0: no range mask)");
+  // The store planes are device memory or pinned (page-locked) host memory, read through its mapped device address.
+  const float* planes[3] = {xyz, intensity, sn};
+  for (int k = 0; k < 3; ++k) {
+    if (!planes[k]) continue;
+    cudaPointerAttributes at;
+    DIB_CHECK_CUDA(cudaPointerGetAttributes(&at, planes[k]));
+    if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) continue;
+    DIB_REQUIRE(at.type == cudaMemoryTypeHost, "the scan store (%s) must be device or pinned host memory",
+                k == 0 ? "xyz" : (k == 1 ? "intensity" : "sn"));
+    void* dp = nullptr;
+    const cudaError_t e = cudaHostGetDevicePointer(&dp, const_cast<float*>(planes[k]), 0);
+    if (e != cudaSuccess) (void)cudaGetLastError();
+    DIB_REQUIRE(e == cudaSuccess && dp, "the pinned scan store (%s) has no mapped device address (%s)",
+                k == 0 ? "xyz" : (k == 1 ? "intensity" : "sn"), cudaGetErrorString(e));
+    planes[k] = static_cast<const float*>(dp);
+  }
+  const float r2 = range_max > 0.0 ? (float)(range_max * range_max) : 0.0f;
+  const dib::asmb::AccArgs a{planes[0], planes[1], planes[2], frame_n, n_max, T, frame_sample, frame_T16, S, r2, false,
+                             0.0f, 0.0f, 0.0f, 0.0f, xyz_out, intensity_out, sn_out, nullptr, out_stride,
+                             frame_offset, plane_stride};
+  return dib::asmb::accumulate<false, true>(a, count_out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 size_t assemble_accumulate_f64_workspace_bytes(int T, int n_stride, int S) {
@@ -614,7 +677,7 @@ int assemble_accumulate_f64(const float* xyz, const float* intensity, const int3
   const float* b = exclude_box;
   const dib::asmb::AccArgs a{xyz, intensity, nullptr, n_pts, n_stride, T, frame_sample, frame_T16, S, r2, b != nullptr,
                              b ? b[0] : 0.0f, b ? b[1] : 0.0f, b ? b[2] : 0.0f, b ? b[3] : 0.0f, nullptr,
-                             intensity_out, nullptr, xyz_out, out_stride};
+                             intensity_out, nullptr, xyz_out, out_stride, nullptr, 0};
   return dib::asmb::accumulate<true>(a, count_out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 

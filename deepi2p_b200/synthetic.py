@@ -422,3 +422,148 @@ def make_ball_query_inputs(seed, B=64, M=64, N=16384, K=64, cube=20.0):
     kth = np.partition(dist, K - 1, axis=2)[:, :, K - 1]
     radius = float(np.median(kth))
     return dist, radius
+
+
+def _link_or_copy(src, dst):
+    try:
+        os.link(src, dst)
+    except OSError:
+        import shutil
+        shutil.copyfile(src, dst)
+
+
+def _kitti_record(seed, n_rings, n_azimuth):
+    """A [7, n] float32 KITTI scan record (xyz, intensity, unit normals) of a make_lidar_scan with a seeded fraction of
+    the rays dropped, so record lengths differ."""
+    sc = make_lidar_scan(seed, n_rings=n_rings, n_azimuth=n_azimuth)
+    rng = np.random.default_rng(seed + 0x7EC)
+    keep = rng.random(sc["xyz"].shape[1]) < rng.uniform(0.6, 0.95)
+    nrm = rng.normal(0.0, 0.2, sc["xyz"].shape) + np.array([[0.0], [0.0], [1.0]])
+    nrm /= np.linalg.norm(nrm, axis=0)
+    return np.concatenate([sc["xyz"], sc["intensity"][None], nrm], 0)[:, keep].astype(np.float32)
+
+
+def write_kitti_root(root, seqs=(0, 9, 10), n_frames=90, seed=0, n_rings=8, n_azimuth=256, image_hw=(376, 1241),
+                     n_images=4):
+    """A seeded KITTI odometry root in the loader's layout for deepi2p_b200.kitti: calib/<seq>/calib.txt (P0-P3 and
+    Tr as KITTI writes them), poses/<seq>/<frame>.npz ['pose'] along a gently turning drive of about 1 m per frame,
+    data_odometry_velodyne_NWU/sequences/<seq>/voxel0.1-SNr0.6/<frame>.npy records ([7, n], n differing per frame) and
+    data_odometry_color_npy/sequences/<seq>/image_{2,3}/<frame>.npy images (n_images distinct uint8 frames of
+    image_hw, linked by frame number).  Returns {seq: n_frames}."""
+    rng = np.random.default_rng(seed + 0x4B17)
+    os.makedirs(root, exist_ok=True)
+    for seq in seqs:
+        s = "%02d" % seq
+        os.makedirs(os.path.join(root, "calib", s), exist_ok=True)
+        fx, cx, cy = 718.856 + seq, 607.1928, 185.2157
+        lines = []
+        for k, tx in enumerate((0.0, -0.537, 0.06, -0.47)):
+            tz = (0.0, 0.0, 2.7e-3, 3.4e-3)[k]
+            ty = (0.0, 0.0, -1.2e-5, 2.0e-5)[k]
+            m = [fx, 0.0, cx, fx * tx + cx * tz, 0.0, fx, cy, fx * ty + cy * tz, 0.0, 0.0, 1.0, tz]
+            lines.append(f"P{k}: " + " ".join("%.12e" % v for v in m))
+        R = np.array([[0.0, -1.0, 0.0], [0.0, 0.0, -1.0], [1.0, 0.0, 0.0]]) @ _rigid(rng, 0.01, 0.0)[:3, :3]
+        Tr = np.concatenate([R, np.array([[-4.07e-3], [-7.63e-2], [-2.72e-1]])], 1)
+        lines.append("Tr: " + " ".join("%.12e" % v for v in Tr.reshape(-1)))
+        with open(os.path.join(root, "calib", s, "calib.txt"), "w") as f:
+            f.write("\n".join(lines) + "\n")
+        pdir = os.path.join(root, "poses", s)
+        rdir = os.path.join(root, "data_odometry_velodyne_NWU", "sequences", s, "voxel0.1-SNr0.6")
+        for d in (pdir, rdir):
+            os.makedirs(d, exist_ok=True)
+        yaw, pos = rng.uniform(-math.pi, math.pi), np.zeros(3)
+        for i in range(n_frames):
+            yaw += rng.normal(0.0, 0.01)
+            pos = pos + np.array([math.sin(yaw), 0.0, math.cos(yaw)]) * rng.uniform(0.8, 1.2)
+            P = np.eye(4)
+            P[:3, :3] = ry_matrix(yaw) @ _rigid(rng, 0.002, 0.0)[:3, :3]
+            P[:3, 3] = pos + rng.normal(0.0, 0.01, 3)
+            np.savez(os.path.join(pdir, "%06d.npz" % i), pose=P)
+            np.save(os.path.join(rdir, "%06d.npy" % i), _kitti_record(seed * 65536 + seq * 1024 + i, n_rings,
+                                                                      n_azimuth))
+        for cam in ("image_2", "image_3"):
+            idir = os.path.join(root, "data_odometry_color_npy", "sequences", s, cam)
+            os.makedirs(idir, exist_ok=True)
+            srcs = []
+            for k in range(n_images):
+                h, w = image_hw
+                yy, xx = np.mgrid[0:h, 0:w]
+                img = np.stack([(xx * (3 + k) + yy) % 256, (yy * (2 + k)) % 256, (xx + 7 * yy * k) % 256], -1)
+                img = (img + rng.integers(0, 24, img.shape)).clip(0, 255).astype(np.uint8)
+                srcs.append(os.path.join(idir, "%06d.npy" % k))
+                np.save(srcs[-1], img)
+            for i in range(n_images, n_frames):
+                _link_or_copy(srcs[i % n_images], os.path.join(idir, "%06d.npy" % i))
+    return {seq: n_frames for seq in seqs}
+
+
+def write_oxford_root(root, train=("2014-05-19-13-20-57", "2014-06-26-08-53-56"), val=("2014-07-14-14-49-50",),
+                      n_clouds=24, cams_per_cloud=3, seed=0, n_rings=8, n_azimuth=256, image_hw=(960, 1280),
+                      n_images=3, quality=90):
+    """A seeded Oxford root in the loader's layout for deepi2p_b200.oxford: train.txt / val.txt, and per traversal
+    pc_timestamps.npy / camera_timestamps.npy (int64 microseconds, cams_per_cloud camera frames per cloud),
+    pc_poses.npy / camera_poses.npy ([n,4,4] float64 along a drive, 2 m between clouds, in the frame the loader
+    conjugates by P_convert), lms_front/<ts>.npy records ([4, n] in camera axes, n differing per cloud) and
+    stereo/centre/<ts>.jpg frames (n_images distinct Pillow JPEGs of image_hw, linked by timestamp).  Returns
+    {traversal: n_clouds}."""
+    from PIL import Image
+    rng = np.random.default_rng(seed + 0x0CF)
+    os.makedirs(root, exist_ok=True)
+    for name, trs in (("train.txt", train), ("val.txt", val)):
+        with open(os.path.join(root, name), "w") as f:
+            f.write("".join(t + "\n" for t in trs))
+    jpegs = []
+    for k in range(n_images):
+        h, w = image_hw
+        yy, xx = np.mgrid[0:h, 0:w]
+        img = np.stack([(xx // (2 + k) + yy // 3) % 256, (yy // (1 + k)) % 256, (xx // 5 + 11 * k) % 256], -1)
+        img = (img + rng.integers(0, 16, img.shape)).clip(0, 255).astype(np.uint8)
+        jpegs.append(img)
+
+    def pose(yaw, p):
+        P = np.eye(4)
+        c, s = math.cos(yaw), math.sin(yaw)
+        P[:3, :3] = np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]]) @ _rigid(rng, 0.003, 0.0)[:3, :3]
+        P[:3, 3] = p
+        return P
+
+    for t_i, tr in enumerate(tuple(train) + tuple(val)):
+        d = os.path.join(root, tr)
+        for sub in ("lms_front", os.path.join("stereo", "centre")):
+            os.makedirs(os.path.join(d, sub), exist_ok=True)
+        t0 = 1400000000000000 + t_i * 10**9
+        yaw, pos = rng.uniform(-math.pi, math.pi), np.array([rng.uniform(-500, 500), rng.uniform(-500, 500), 0.0])
+        pc_ts, pc_P, cam_ts, cam_P = [], [], [], []
+        for i in range(n_clouds):
+            ts = t0 + i * 250000 + int(rng.integers(0, 1000))
+            for c in range(cams_per_cloud):
+                cts = ts - 100000 + c * (250000 // cams_per_cloud) + int(rng.integers(0, 500))
+                cyaw = yaw + rng.normal(0.0, 0.01)
+                cp = pos + np.array([math.cos(yaw), math.sin(yaw), 0.0]) * (c * 2.0 / cams_per_cloud - 0.8)
+                cam_ts.append(cts)
+                cam_P.append(pose(cyaw, cp))
+            pc_ts.append(ts)
+            pc_P.append(pose(yaw, pos))
+            sc = make_lidar_scan(seed * 65536 + t_i * 1024 + i, n_rings=n_rings, n_azimuth=n_azimuth)
+            keep = rng.random(sc["xyz"].shape[1]) < rng.uniform(0.6, 0.95)
+            x, y, z = sc["xyz"]
+            rec = np.stack([-y, -z, x, sc["intensity"]])[:, keep].astype(np.float32)
+            np.save(os.path.join(d, "lms_front", "%d.npy" % ts), rec)
+            yaw += rng.normal(0.0, 0.02)
+            pos = pos + np.array([math.cos(yaw), math.sin(yaw), 0.0]) * 2.0
+        order = np.argsort(cam_ts, kind="stable")
+        cam_ts = [cam_ts[k] for k in order]
+        cam_P = [cam_P[k] for k in order]
+        np.save(os.path.join(d, "pc_timestamps.npy"), np.array(pc_ts, dtype=np.int64))
+        np.save(os.path.join(d, "pc_poses.npy"), np.stack(pc_P))
+        np.save(os.path.join(d, "camera_timestamps.npy"), np.array(cam_ts, dtype=np.int64))
+        np.save(os.path.join(d, "camera_poses.npy"), np.stack(cam_P))
+        srcs = []
+        for k, cts in enumerate(cam_ts):
+            p = os.path.join(d, "stereo", "centre", "%d.jpg" % cts)
+            if k < n_images:
+                Image.fromarray(jpegs[k]).save(p, quality=quality)
+                srcs.append(p)
+            else:
+                _link_or_copy(srcs[k % n_images], p)
+    return {tr: n_clouds for tr in tuple(train) + tuple(val)}

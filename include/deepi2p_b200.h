@@ -391,6 +391,13 @@ int sym3_eig_batch_f64(const double* C, int n, double* lam, double* E, dib_strea
  *   points with x'^2 + z'^2 < range_max^2 in float32.  Each sample's kept points are written in (frame, index) order to
  *   xyz_out [S][3][out_stride], intensity_out [S][out_stride], sn_out [S][3][out_stride] (with sn); count_out [S] i32.
  *   workspace >= assemble_accumulate_workspace_bytes(T, n_stride, S), 256-byte aligned.
+ * assemble_accumulate_gather_f32: assemble_accumulate_f32 on frames gathered from a ragged scan store: SoA planes
+ *   xyz [3][plane_stride], intensity [plane_stride], sn [3][plane_stride] (may be NULL) f32, in device memory or in
+ *   pinned host memory (read through its mapped device address; other host memory is an error).  Frame t is store
+ *   points [frame_offset[t], frame_offset[t] + frame_n[t]) (frame_offset [T] i64, frame_n [T] i32 clamped to
+ *   [0, n_max], both device; the caller keeps every range inside the store).  A store range may back several frames,
+ *   in any order.  The outputs equal assemble_accumulate_f32's bit for bit on the same frames padded into
+ *   [T][3][n_max] with n_pts = frame_n.  workspace >= assemble_accumulate_gather_workspace_bytes(T, n_max, S).
  * assemble_accumulate_f64 (data/nuscenes_pc_img_pose_loader.py:194-267): as assemble_accumulate_f32 without sn, with
  *   the coordinates kept in fp64, xyz_out [S][3][out_stride] f64.  exclude_box [host, 4 f32] (x_lo, x_hi, y_lo, y_hi)
  *   or NULL drops points with x_lo < x < x_hi and y_lo < y < y_hi, compared in float32 on the frame's own (source)
@@ -416,6 +423,12 @@ int assemble_accumulate_f32(const float* xyz, const float* intensity, const floa
                             int n_stride, int T, const int32_t* frame_sample, const double* frame_T16, int S,
                             double range_max, float* xyz_out, float* intensity_out, float* sn_out, int out_stride,
                             int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+size_t assemble_accumulate_gather_workspace_bytes(int T, int n_max, int S);
+int assemble_accumulate_gather_f32(const float* xyz, const float* intensity, const float* sn, int64_t plane_stride,
+                                   const int64_t* frame_offset, const int32_t* frame_n, int n_max, int T,
+                                   const int32_t* frame_sample, const double* frame_T16, int S, double range_max,
+                                   float* xyz_out, float* intensity_out, float* sn_out, int out_stride,
+                                   int32_t* count_out, void* workspace, size_t workspace_bytes, dib_stream_t stream);
 size_t assemble_accumulate_f64_workspace_bytes(int T, int n_stride, int S);
 int assemble_accumulate_f64(const float* xyz, const float* intensity, const int32_t* n_pts, int n_stride, int T,
                             const int32_t* frame_sample, const double* frame_T16, int S, double range_max,
