@@ -37,6 +37,7 @@ EXPORTS = (
     "knn_group_forward_f32", "knn_group_backward_workspace_bytes", "knn_group_backward_f32",
     "attn_fusion_forward_f32", "attn_fusion_backward_f32", "jpeg_decode_workspace_bytes", "jpeg_decode_batch_u8",
     "pointwise_mlp_packed_bytes", "pointwise_mlp_pack_f32", "pointwise_mlp_workspace_bytes", "pointwise_mlp_f32",
+    "png_decode_workspace_bytes", "png_decode_batch_u8",
 )
 
 
@@ -249,6 +250,10 @@ def load():
     lib.pointwise_mlp_workspace_bytes.argtypes = [vp, i32, vp, i32, i32]
     lib.pointwise_mlp_f32.restype = i32
     lib.pointwise_mlp_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, i32, vp, vp, vp, vp, sz, vp]
+    lib.png_decode_workspace_bytes.restype = sz
+    lib.png_decode_workspace_bytes.argtypes = [vp, i32, vp, i32, sz]
+    lib.png_decode_batch_u8.restype = i32
+    lib.png_decode_batch_u8.argtypes = [vp, sz, vp, i32, vp, i32, vp, sz, vp, vp, sz, vp]
     _lib = lib
     return lib
 

@@ -5,7 +5,8 @@ loader), for S samples at once and bit for bit against cv2 and Pillow.
 
 pack_images packs ragged HWC uint8 frames into one device buffer, and decode_jpeg_batch / read_jpeg_batch decode the
 loaders' JPEG frames (Image.open(path).convert("RGB"), bit for bit; csrc/jpeg.cu, DESIGN.md 4.19) into the same
-buffer on the device; image_params draws the per-sample crop offsets and
+buffer on the device, and decode_png_batch / read_png_batch do the same for KITTI's official PNG frames
+(cv2.imread(path)[:, :, ::-1], bit for bit; csrc/png.cu, DESIGN.md 4.23); image_params draws the per-sample crop offsets and
 jitter on the host; assemble_images runs csrc/imageprep.cu and composes K in fp64.  kitti_image_args /
 oxford_image_args / nuscenes_image_args are the loaders' options (nuScenes: crop_top_rows=100, img_scale=0.2, 160 x
 320, jitter_prob=0.5).  augment_img is a host drop-in for the loaders' augment_img that works on current torchvision.
@@ -16,6 +17,7 @@ import torch
 
 from . import _native
 from . import jpeg as _jpeg
+from . import png as _png
 from .assemble import MODES
 from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace
 
@@ -132,6 +134,61 @@ def read_jpeg_batch(paths, device="cuda", stream=None):
         with open(p, "rb") as f:
             blobs.append(f.read())
     return decode_jpeg_batch(blobs, device=device, stream=stream)
+
+
+def decode_png_batch(blobs, device="cuda", stream=None):
+    """Decode S PNG streams (bytes-like) on the GPU into pack_images' dict: data uint8 [sum 3 h w] on `device` (HWC
+    RGB, each image equal to cv2.imdecode(np.frombuffer(b, np.uint8), cv2.IMREAD_COLOR)[:, :, ::-1] on OpenCV 4.13),
+    offsets int64 [S], shapes int64 [S,2] (h, w), so assemble_images takes it as it is.
+
+    Supported: 8-bit truecolour (colour type 2), not interlaced, from 1 x 1 up to OpenCV's limits (2^20 per side,
+    2^30 pixels); the zlib stream split over any number of IDAT chunks (empty ones included), stored, fixed and
+    dynamic Deflate blocks, any declared window, all five row filters; ancillary chunks are skipped (a bad CRC on one is ignored, as libpng does).  Other colour types,
+    bit depths and Adam7 raise ValueError("image i: unsupported ...").  Every stream OpenCV rejects raises too: a bad
+    signature, chunk structure or critical-chunk CRC, a bad zlib header, corrupt or truncated Deflate data, a bad
+    Adler-32, too little image data or a filter byte above 4.  Beyond OpenCV, a stream whose inflated data is longer
+    than the image or that uses a distance beyond its declared window is rejected (DESIGN.md 4.23).  The error names
+    the first bad image, ValueError("image i: <reason>"), and no output is returned for any image.  The call waits for
+    the decode to finish (the per-image status is read back)."""
+    _require_cuda()
+    lib = _native.load()
+    dev = torch.device(device)
+    S = len(blobs)
+    pk = _png.pack_batch(blobs)
+    bad = dict(pk["errors"])
+    with torch.cuda.device(dev), torch.cuda.stream(stream):
+        out = torch.empty(pk["out_bytes"], dtype=torch.uint8, device=dev)
+        if S and len(bad) < S:
+            sp = _stream_ptr(stream)
+            data = torch.from_numpy(pk["data"]).to(dev)
+            status = torch.empty((S, 4), dtype=torch.int32, device=dev)
+            desc = np.ascontiguousarray(pk["desc"])
+            chunks = np.ascontiguousarray(pk["chunks"])
+            nws = lib.png_decode_workspace_bytes(desc.ctypes.data, S, chunks.ctypes.data, len(chunks), data.numel())
+            if nws == 0:
+                raise _native.NativeError("png_decode_workspace_bytes rejected the batch")
+            ws = _workspace(nws, dev, sp)
+            rc = lib.png_decode_batch_u8(_ptr(data), data.numel(), desc.ctypes.data, S, chunks.ctypes.data,
+                                         len(chunks), _ptr(out), out.numel(), _ptr(status), _ptr(ws), ws.numel(), sp)
+            _native.check(rc, "png_decode")
+            st = status.cpu().numpy()
+            for i in np.flatnonzero(st.any(1)):
+                code = int(st[i][np.flatnonzero(st[i])[0]])
+                bad.setdefault(int(i), _png.STATUS.get(code, f"status {code}"))
+    if bad:
+        i = min(bad)
+        raise ValueError(f"image {i}: {bad[i]}")
+    return dict(data=out, offsets=pk["offsets"], shapes=pk["shapes"])
+
+
+def read_png_batch(paths, device="cuda", stream=None):
+    """cv2.imread(path)[:, :, ::-1] for S PNG files (the frames kitti_png_to_npy.py converts): reads the files on the
+    host and decodes them with decode_png_batch."""
+    blobs = []
+    for p in paths:
+        with open(p, "rb") as f:
+            blobs.append(f.read())
+    return decode_png_batch(blobs, device=device, stream=stream)
 
 
 def image_params(shapes, mode, rng=None, img_H=160, img_W=512, img_scale=0.5, crop_top_rows=0, crop_bottom_rows=0,

@@ -46,12 +46,29 @@ def record_path(root, seq, i):
     return os.path.join(record_dir(root, seq), "%06d.npy" % i)
 
 
+def image_dirs(root, seq, key):
+    """The two folders a sequence's camera frames may be in: the .npy conversion (kitti_png_to_npy.py's output, the
+    loader's layout) and KITTI's official .png layout."""
+    cam = "image_" + key[1]
+    return (os.path.join(root, "data_odometry_color_npy", "sequences", "%02d" % seq, cam),
+            os.path.join(root, "data_odometry_color", "sequences", "%02d" % seq, cam))
+
+
 def image_dir(root, seq, key):
-    return os.path.join(root, "data_odometry_color_npy", "sequences", "%02d" % seq, "image_" + key[1])
+    """The sequence's frame folder: the .npy folder when it exists, otherwise the official PNG folder; raises
+    FileNotFoundError naming both when neither exists."""
+    npy, png = image_dirs(root, seq, key)
+    if os.path.isdir(npy):
+        return npy
+    if os.path.isdir(png):
+        return png
+    raise FileNotFoundError(f"KITTI image folder not found: neither {npy} nor {png}")
 
 
 def image_path(root, seq, key, i):
-    return os.path.join(image_dir(root, seq, key), "%06d.npy" % i)
+    """Frame i of the camera: <frame>.npy in the .npy folder when it exists, otherwise <frame>.png."""
+    d = image_dir(root, seq, key)
+    return os.path.join(d, "%06d.%s" % (i, "npy" if d == image_dirs(root, seq, key)[0] else "png"))
 
 
 def parse_calib(text, path="calib.txt"):
@@ -108,7 +125,7 @@ def mode_seqs(mode):
 
 
 def sequence_length(root, seq):
-    """The loader's sample count: the number of entries of the sequence's image_2 folder."""
+    """The loader's sample count: the number of entries of the sequence's image_2 folder (the one image_dir picks)."""
     d = _require(image_dir(root, seq, "P2"), "image folder")
     n = len(os.listdir(d))
     if n == 0:
@@ -296,8 +313,18 @@ def kitti_batch(root, items, mode, seed, rng=None, store=None, input_pt_num=asse
     Pji = np.stack([p["Pji"] for p in plan])
     out = assemble.assemble_batch(frames, mode, seed, input_pt_num=input_pt_num, node_a_num=node_a_num,
                                   node_b_num=node_b_num, rng=rng, stream=stream, **assemble.kitti_args(Pc, Pji))
-    imgs = [np.load(_require(image_path(ds.root, p["seq"], p["key"], p["j"]), "image")) for p in plan]
-    images = imageprep.pack_images(imgs, device)
+    paths = [_require(image_path(ds.root, p["seq"], p["key"], p["j"]), "image") for p in plan]
+    png = [k for k, q in enumerate(paths) if q.endswith(".png")]
+    if len(png) == len(paths):
+        images = imageprep.read_png_batch(paths, device, stream)
+    else:                                   # .npy frames, or sequences of both kinds in one batch
+        imgs = [None if k in png else np.load(q) for k, q in enumerate(paths)]
+        if png:
+            dec = imageprep.read_png_batch([paths[k] for k in png], device, stream)
+            data = dec["data"].cpu().numpy()
+            for k, o, (h, w) in zip(png, dec["offsets"], dec["shapes"]):
+                imgs[k] = data[o:o + 3 * h * w].reshape(h, w, 3)
+        images = imageprep.pack_images(imgs, device)
     K = np.stack([p["K"] for p in plan])
     im = imageprep.assemble_images(images, K, mode, rng=rng, flip=out["flip"], stream=stream,
                                    **imageprep.kitti_image_args())

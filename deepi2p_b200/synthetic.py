@@ -9,6 +9,8 @@ Oxford-shaped: H=384, W=640 (data/oxford_pc_img_pose_loader.py:221-259).
 """
 import math
 import os
+import struct
+import zlib
 
 import numpy as np
 
@@ -444,12 +446,16 @@ def _kitti_record(seed, n_rings, n_azimuth):
 
 
 def write_kitti_root(root, seqs=(0, 9, 10), n_frames=90, seed=0, n_rings=8, n_azimuth=256, image_hw=(376, 1241),
-                     n_images=4):
+                     n_images=4, images="npy"):
     """A seeded KITTI odometry root in the loader's layout for deepi2p_b200.kitti: calib/<seq>/calib.txt (P0-P3 and
     Tr as KITTI writes them), poses/<seq>/<frame>.npz ['pose'] along a gently turning drive of about 1 m per frame,
     data_odometry_velodyne_NWU/sequences/<seq>/voxel0.1-SNr0.6/<frame>.npy records ([7, n], n differing per frame) and
     data_odometry_color_npy/sequences/<seq>/image_{2,3}/<frame>.npy images (n_images distinct uint8 frames of
-    image_hw, linked by frame number).  Returns {seq: n_frames}."""
+    image_hw, linked by frame number).  images="png" writes the same pixels in the official layout instead,
+    data_odometry_color/sequences/<seq>/image_{2,3}/<frame>.png (encode_png, the rows cycling through the five
+    filters).  Returns {seq: n_frames}."""
+    if images not in ("npy", "png"):
+        raise ValueError(f"images must be 'npy' or 'png' (got {images!r})")
     rng = np.random.default_rng(seed + 0x4B17)
     os.makedirs(root, exist_ok=True)
     for seq in seqs:
@@ -482,7 +488,8 @@ def write_kitti_root(root, seqs=(0, 9, 10), n_frames=90, seed=0, n_rings=8, n_az
             np.save(os.path.join(rdir, "%06d.npy" % i), _kitti_record(seed * 65536 + seq * 1024 + i, n_rings,
                                                                       n_azimuth))
         for cam in ("image_2", "image_3"):
-            idir = os.path.join(root, "data_odometry_color_npy", "sequences", s, cam)
+            folder = "data_odometry_color_npy" if images == "npy" else "data_odometry_color"
+            idir = os.path.join(root, folder, "sequences", s, cam)
             os.makedirs(idir, exist_ok=True)
             srcs = []
             for k in range(n_images):
@@ -490,10 +497,14 @@ def write_kitti_root(root, seqs=(0, 9, 10), n_frames=90, seed=0, n_rings=8, n_az
                 yy, xx = np.mgrid[0:h, 0:w]
                 img = np.stack([(xx * (3 + k) + yy) % 256, (yy * (2 + k)) % 256, (xx + 7 * yy * k) % 256], -1)
                 img = (img + rng.integers(0, 24, img.shape)).clip(0, 255).astype(np.uint8)
-                srcs.append(os.path.join(idir, "%06d.npy" % k))
-                np.save(srcs[-1], img)
+                srcs.append(os.path.join(idir, "%06d.%s" % (k, images)))
+                if images == "npy":
+                    np.save(srcs[-1], img)
+                else:
+                    with open(srcs[-1], "wb") as f:
+                        f.write(encode_png(img, filters=np.arange(h) % 5))
             for i in range(n_images, n_frames):
-                _link_or_copy(srcs[i % n_images], os.path.join(idir, "%06d.npy" % i))
+                _link_or_copy(srcs[i % n_images], os.path.join(idir, "%06d.%s" % (i, images)))
     return {seq: n_frames for seq in seqs}
 
 
@@ -567,3 +578,54 @@ def write_oxford_root(root, train=("2014-05-19-13-20-57", "2014-06-26-08-53-56")
             else:
                 _link_or_copy(srcs[k % n_images], p)
     return {tr: n_clouds for tr in tuple(train) + tuple(val)}
+
+
+def png_chunk(ctype, data, crc=None):
+    """One PNG chunk: length, type, data and CRC-32 (the correct one unless `crc` is given)."""
+    c = zlib.crc32(ctype + data) if crc is None else crc
+    return struct.pack(">I", len(data)) + ctype + data + struct.pack(">I", c & 0xFFFFFFFF)
+
+
+def png_filter(img, filters):
+    """The filtered scanlines of an HWC uint8 RGB image: each row prefixed by its filter type (filters: one int for
+    every row, or one per row) and filtered with 3 bytes per pixel, mod 256."""
+    h, w, _ = img.shape
+    x = img.reshape(h, 3 * w).astype(np.int64)
+    up = np.vstack([np.zeros((1, 3 * w), np.int64), x[:-1]])
+    left = np.hstack([np.zeros((h, 3), np.int64), x[:, :-3]])
+    ul = np.hstack([np.zeros((h, 3), np.int64), up[:, :-3]])
+    p = left + up - ul
+    pa, pb, pc = np.abs(p - left), np.abs(p - up), np.abs(p - ul)
+    paeth = np.where((pa <= pb) & (pa <= pc), left, np.where(pb <= pc, up, ul))
+    preds = [np.zeros_like(x), left, up, (left + up) >> 1, paeth]
+    f = np.broadcast_to(np.asarray(filters, np.int64), (h,))
+    out = np.empty((h, 3 * w + 1), np.uint8)
+    out[:, 0] = f
+    for k in range(5):
+        out[f == k, 1:] = (x - preds[k])[f == k] & 255
+    return out.tobytes()
+
+
+def encode_png(img, filters=4, level=6, wbits=15, idat=8192, zdata=None, ancillary=True):
+    """A PNG stream of an HWC uint8 RGB image from the standard library: png_filter's scanlines through zlib at
+    `level` with a 2^wbits window, split into IDAT chunks of `idat` bytes (an int, or a list of chunk lengths, the last
+    taking the rest); zdata replaces the zlib stream.  ancillary adds a tEXt chunk before the IDATs."""
+    img = np.ascontiguousarray(img, np.uint8)
+    h, w, _ = img.shape
+    if zdata is None:
+        co = zlib.compressobj(level, zlib.DEFLATED, wbits)
+        zdata = co.compress(png_filter(img, filters)) + co.flush()
+    parts = [b"\x89PNG\r\n\x1a\n", png_chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 2, 0, 0, 0))]
+    if ancillary:
+        parts.append(png_chunk(b"tEXt", b"Software\0deepi2p_b200"))
+    sizes = list(idat) if isinstance(idat, (list, tuple)) else None
+    p = 0
+    while p < len(zdata) or p == 0:
+        n = (sizes.pop(0) if sizes else len(zdata) - p) if sizes is not None else idat
+        parts.append(png_chunk(b"IDAT", zdata[p:p + n]))
+        p += n
+        if sizes is not None and not sizes and p < len(zdata):
+            parts.append(png_chunk(b"IDAT", zdata[p:]))
+            p = len(zdata)
+    parts.append(png_chunk(b"IEND", b""))
+    return b"".join(parts)

@@ -688,6 +688,48 @@ int pointwise_mlp_f32(const int64_t* sources, int n_sources, const int64_t* laye
                       size_t packed_bytes, int B, int N, int c_split, float* out, int8_t* pred_a, int32_t* pred_b,
                       void* workspace, size_t workspace_bytes, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Batched PNG decoding (KITTI's official odometry colour frames).  DESIGN.md 4.23 states the contract: 8-bit
+ * truecolour, not interlaced, decoded bit for bit as OpenCV 4.13's cv2.imdecode(..., IMREAD_COLOR)[:, :, ::-1]
+ * (HWC uint8 RGB).  deepi2p_b200/png.py walks the chunks, checks IHDR / PLTE / IEND and the zlib header, and fills
+ * the inputs.
+ *
+ * data: [dev] data_bytes bytes holding each image's IDAT payloads, each starting 16-byte aligned (no padding is
+ *   needed after the last).
+ *   desc: [host] int64 [S][DIB_PNG_DESC]: 0 data offset, 1 IDAT bytes, 2 out offset, 3 w, 4 h, 5 first chunk,
+ *   6 log2 of the zlib window, 7 skip (1: no work and no output for this image), 9 chunk count; slot 8 is the
+ *   library's.  chunks: [host] int64 [n_chunks][4]: image, data offset, payload length, stored CRC-32 of each IDAT
+ *   chunk, an image's chunks consecutive and covering its data.  out: [dev] out_bytes bytes, image s at its offset.
+ *   status: [dev] int32 [S][4]: the inflate code, the chunk CRC code, the Adler-32 code and the filter code of image s
+ *   (DIB_PNG_*, 0 = fine); the pixels of an image with any non-zero code are unspecified.  workspace: [dev] 256-byte
+ *   aligned, >= png_decode_workspace_bytes(desc, S, chunks, n_chunks, data_bytes) (0 for invalid descriptors).
+ *   Deterministic: no atomics touch the data.
+ * ------------------------------------------------------------------------------------------ */
+#define DIB_PNG_DESC 12
+#define DIB_PNG_OK 0
+#define DIB_PNG_TRUNCATED 1   /* the zlib stream needs more data than the IDAT chunks hold            */
+#define DIB_PNG_BLOCK_TYPE 2  /* Deflate block type 3                                                 */
+#define DIB_PNG_STORED 3      /* stored block LEN != ~NLEN                                            */
+#define DIB_PNG_LENGTHS 4     /* over-subscribed or incomplete code set                               */
+#define DIB_PNG_NO_EOB 5      /* the literal/length code has no end-of-block code                     */
+#define DIB_PNG_REPEAT 6      /* code-length repeat 16 with no previous length                        */
+#define DIB_PNG_OVERRUN 7     /* code lengths run past HLIT + HDIST                                   */
+#define DIB_PNG_SYMBOLS 8     /* HLIT > 286 or HDIST > 30                                             */
+#define DIB_PNG_LITLEN 9      /* an invalid literal/length code or symbol 286-287                     */
+#define DIB_PNG_DISTANCE 10   /* an invalid distance code or symbol 30-31                             */
+#define DIB_PNG_FAR 11        /* a distance before the start of the output                            */
+#define DIB_PNG_WINDOW 12     /* a distance beyond the window the zlib header declares                */
+#define DIB_PNG_TOO_MUCH 13   /* more inflated data than h x (1 + 3 w)                                */
+#define DIB_PNG_SHORT 14      /* the zlib stream ends before the image is complete                    */
+#define DIB_PNG_NO_ADLER 15   /* the Adler-32 trailer is missing                                      */
+#define DIB_PNG_ADLER 16      /* the Adler-32 of the inflated data does not match                     */
+#define DIB_PNG_CRC 17        /* an IDAT chunk's CRC-32 does not match                                */
+#define DIB_PNG_FILTER 18     /* a row filter byte above 4                                            */
+size_t png_decode_workspace_bytes(const int64_t* desc, int S, const int64_t* chunks, int n_chunks, size_t data_bytes);
+int png_decode_batch_u8(const uint8_t* data, size_t data_bytes, const int64_t* desc, int S, const int64_t* chunks,
+                        int n_chunks, uint8_t* out, size_t out_bytes, int32_t* status, void* workspace,
+                        size_t workspace_bytes, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
