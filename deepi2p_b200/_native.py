@@ -38,6 +38,8 @@ EXPORTS = (
     "attn_fusion_forward_f32", "attn_fusion_backward_f32", "jpeg_decode_workspace_bytes", "jpeg_decode_batch_u8",
     "pointwise_mlp_packed_bytes", "pointwise_mlp_pack_f32", "pointwise_mlp_workspace_bytes", "pointwise_mlp_f32",
     "png_decode_workspace_bytes", "png_decode_batch_u8",
+    "oxford_build_plan_f64", "oxford_build_count_workspace_bytes", "oxford_build_count_f64",
+    "oxford_build_scatter_f64", "oxford_build_pack_f32",
 )
 
 
@@ -254,6 +256,17 @@ def load():
     lib.png_decode_workspace_bytes.argtypes = [vp, i32, vp, i32, sz]
     lib.png_decode_batch_u8.restype = i32
     lib.png_decode_batch_u8.argtypes = [vp, sz, vp, i32, vp, i32, vp, sz, vp, vp, sz, vp]
+    i64 = _c.c_int64
+    lib.oxford_build_plan_f64.restype = i32
+    lib.oxford_build_plan_f64.argtypes = [vp, vp, i64, vp, vp, i32, vp, f64, i32, vp, vp, vp, vp, vp]
+    lib.oxford_build_count_workspace_bytes.restype = sz
+    lib.oxford_build_count_workspace_bytes.argtypes = [i32, i32]
+    lib.oxford_build_count_f64.restype = i32
+    lib.oxford_build_count_f64.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, f64, vp, vp, vp, vp, sz, vp]
+    lib.oxford_build_scatter_f64.restype = i32
+    lib.oxford_build_scatter_f64.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f64, i32, vp, vp, vp]
+    lib.oxford_build_pack_f32.restype = i32
+    lib.oxford_build_pack_f32.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, vp, vp]
     _lib = lib
     return lib
 

@@ -580,6 +580,88 @@ def write_oxford_root(root, train=("2014-05-19-13-20-57", "2014-06-26-08-53-56")
     return {tr: n_clouds for tr in tuple(train) + tuple(val)}
 
 
+OXFORD_CAMERA_MODEL = ("964.828979 964.828979 643.788025 484.407990\n"
+                       "0 0 1 0\n1 0 0 0\n0 1 0 0\n0 0 0 1\n")
+OXFORD_EXTRINSICS = {"lms_front": "1.7042 -0.021 0.1052 -0.0017 0.0152 -0.0001\n",
+                     "stereo": "0 0 0 0 0 0\n"}
+
+
+def write_oxford_sdk(sdk):
+    """The SDK text files the Oxford build reads: models/stereo_narrow_left.txt and extrinsics/{lms_front,stereo}.txt
+    (the loader's K_CENTRE, a camera-from-image permutation and plausible mounting offsets)."""
+    os.makedirs(os.path.join(sdk, "models"), exist_ok=True)
+    os.makedirs(os.path.join(sdk, "extrinsics"), exist_ok=True)
+    with open(os.path.join(sdk, "models", "stereo_narrow_left.txt"), "w") as f:
+        f.write(OXFORD_CAMERA_MODEL)
+    for name, line in OXFORD_EXTRINSICS.items():
+        with open(os.path.join(sdk, "extrinsics", name + ".txt"), "w") as f:
+            f.write(line)
+
+
+def write_oxford_raw(raw, lms, sdk, traversals=("2014-05-19-13-20-57",), night=("2014-12-10-18-10-50",), seconds=30.0,
+                     speed=5.0, stops=((8.0, 9.5), (14.0, 17.0)), curve=(6.0, 11.0), yaw_rate=0.15, zero_reflectance_after=None,
+                     n_returns=60, missing_scans=0.03, missing_images=0.05, vo_on_cameras=False, seed=0):
+    """Seeded raw RobotCar traversals in the layout build_dataset.py reads: <raw>/<t>/vo/vo.csv (16 Hz rows whose
+    chain abs_k = abs_{k-1} se3(row k) is the drive: `speed` m/s, standing still during each of `stops` (seconds from
+    the start), turning at yaw_rate rad/s during `curve`), <raw>/<t>/stereo.timestamps (16 Hz; with vo_on_cameras the
+    VO rows are sourced at the camera frames and end on the last one, as in a RobotCar download, otherwise they are
+    offset from them and run 120 ms past the last), empty placeholder
+    <raw>/<t>/stereo/centre/<ts>.png files (a fraction missing_images absent), <raw>/<t>/tags.csv, and
+    <lms>/<t>/lms_front.timestamps with 50 Hz <lms>/<t>/lms_front/<ts>.bin scans of n_returns float64 (x, y,
+    reflectance) triples (a fraction missing_scans absent; some x exactly 0.1; reflectance zero from
+    zero_reflectance_after seconds on).  night names traversals tagged night.  Also writes the SDK files into sdk.
+    Returns {traversal: dict(vo=..., lms=..., cameras=...)} of timestamp lists."""
+    write_oxford_sdk(sdk)
+    out = {}
+    for t_i, t in enumerate(tuple(traversals) + tuple(night)):
+        rng = np.random.default_rng(seed * 1000 + t_i + 0x0B5)
+        t0 = 1400000000000000 + t_i * 10**10
+        end = t0 + int(seconds * 1e6)
+        cams = list(range(t0 + 30002, end, 62500))
+        vo_ts = list(cams) if vo_on_cameras else list(range(t0 + 1, end + 120001, 60000))
+        rows = [[0.0] * 6]
+        for a, b in zip(vo_ts[:-1], vo_ts[1:]):
+            tm = (b - t0) / 1e6
+            dt = (b - a) / 1e6
+            moving = not any(a_ <= tm <= b_ for a_, b_ in stops)
+            v = speed * dt if moving else 0.0
+            w = yaw_rate * dt if (moving and curve[0] <= tm <= curve[1]) else 0.0
+            n = rng.normal(0.0, 1e-4, 4) if moving else np.zeros(4)
+            rows.append([v, n[0], n[1], n[2], n[3], w])
+        d = os.path.join(raw, t)
+        os.makedirs(os.path.join(d, "vo"), exist_ok=True)
+        os.makedirs(os.path.join(d, "stereo", "centre"), exist_ok=True)
+        with open(os.path.join(d, "vo", "vo.csv"), "w") as f:
+            f.write("source_timestamp,destination_timestamp,x,y,z,roll,pitch,yaw\n")
+            for k, (ts, r) in enumerate(zip(vo_ts, rows)):
+                f.write(",".join([str(ts), str(vo_ts[max(k - 1, 0)])] + [repr(float(x)) for x in r]) + "\n")
+        with open(os.path.join(d, "stereo.timestamps"), "w") as f:
+            f.write("".join("%d 1\n" % c for c in cams))
+        for c in cams:
+            if rng.random() >= missing_images:
+                open(os.path.join(d, "stereo", "centre", "%d.png" % c), "wb").close()
+        with open(os.path.join(d, "tags.csv"), "w") as f:
+            f.write("night,rain\n" if t in night else "overcast,roadworks\n")
+        ld = os.path.join(lms, t, "lms_front")
+        os.makedirs(ld, exist_ok=True)
+        lts = list(range(t0 + 10004, end, 20000))
+        with open(os.path.join(lms, t, "lms_front.timestamps"), "w") as f:
+            f.write("".join("%d 1\n" % x for x in lts))
+        for x in lts:
+            if rng.random() < missing_scans:
+                continue
+            s = np.empty((n_returns, 3))
+            s[:, 0] = rng.uniform(-3.0, 1.0, n_returns)
+            s[rng.random(n_returns) < 0.05, 0] = 0.1
+            s[:, 1] = rng.uniform(-25.0, 25.0, n_returns)
+            s[:, 2] = rng.uniform(0.0, 1500.0, n_returns)
+            if zero_reflectance_after is not None and x - t0 >= zero_reflectance_after * 1e6:
+                s[:, 2] = 0.0
+            s.astype(np.float64).tofile(os.path.join(ld, "%d.bin" % x))
+        out[t] = dict(vo=vo_ts, lms=lts, cameras=cams)
+    return out
+
+
 def png_chunk(ctype, data, crc=None):
     """One PNG chunk: length, type, data and CRC-32 (the correct one unless `crc` is given)."""
     c = zlib.crc32(ctype + data) if crc is None else crc

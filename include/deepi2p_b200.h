@@ -730,6 +730,49 @@ int png_decode_batch_u8(const uint8_t* data, size_t data_bytes, const int64_t* d
                         int n_chunks, uint8_t* out, size_t out_bytes, int32_t* status, void* workspace,
                         size_t workspace_bytes, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Oxford RobotCar point-cloud build (data/oxford/build_dataset.py: my_build_pointcloud, downsample and the output
+ * transform), S clouds of one traversal per call.  DESIGN.md 4.24 states the contract; deepi2p_b200/oxford_build.py
+ * plans the windows and chains the calls with voxel_downsample_batch_f64 (C = 1) between scatter and pack.  All
+ * arithmetic is fp64 without FMA, each sum in the association stated; all pointers [dev] unless marked [host].
+ *
+ * oxford_build_plan_f64: lms_poses [n_lms][16] row-major absolute poses, present [n_lms] u8 (0: no scan file),
+ *   windows [S][2] i64 LMS index range [lo, hi), centre_inv [S][16] the inverse of each centre's absolute pose,
+ *   G [host, 16] G_posesource_laser.  Per cloud, for i in [lo, hi) with present[i]: rel = M_c P_i (each entry
+ *   ((a0 b0 + a1 b1) + a2 b2) + a3 b3); unless it is the first kept scan, d = rows 0-2 of inv(prev) rel[:, 3] and
+ *   the scan is skipped when sqrt((d0 d0 + d1 d1) + d2 d2) < skip_threshold, prev being the last kept rel and inv a
+ *   Gauss-Jordan inverse with partial pivoting (first largest |pivot|; all eight columns of [A | I] updated, rows in
+ *   ascending order).  A kept scan writes kept_scan [S][w_stride] i32 = i and kept_T [S][w_stride][12] = rows 0-2
+ *   of rel G.  n_kept [S], n_skipped [S] i32.  A window outside [0, n_lms] or longer than w_stride gives n_kept = 0,
+ *   n_skipped = -1.
+ * oxford_build_count_f64: x, r [store] f64 planes, offsets [n_lms + 1] i64 (scan i = [offsets[i], offsets[i+1])).
+ *   A point is kept when use_mask is 0 or x < threshold.  pos [S][w_stride] i32 = first output index of each kept
+ *   scan, n_pts [S] i32 = kept points of the cloud, rmax [S] f64 = their largest reflectance (-inf when none).
+ *   workspace >= oxford_build_count_workspace_bytes(S, w_stride), 256-byte aligned.
+ * oxford_build_scatter_f64: the kept points in scan order, then point order: xyz_out [S][3][n_stride] =
+ *   ((T0 x + T1 y) + T2 0) + T3 per row, attr_out [S][n_stride] = r / rmax.  Entries past n_pts are not written;
+ *   n_stride % 16 == 0 and n_stride >= max n_pts.
+ * oxford_build_pack_f32: xyz [S][3][n_stride], attr [S][n_stride] (voxel_downsample_batch_f64's outputs), m_pts
+ *   [S] i32 <= m_stride, O [host, 16]: out [S][4][m_stride] f32 = (float)(((O0 x + O1 y) + O2 z) + O3) for rows
+ *   0-2 and (float)(attr * rmax) for row 3, zeros past m_pts.
+ * ------------------------------------------------------------------------------------------ */
+int oxford_build_plan_f64(const double* lms_poses, const uint8_t* present, int64_t n_lms, const int64_t* windows,
+                          const double* centre_inv, int S, const double* G, double skip_threshold, int w_stride,
+                          int32_t* kept_scan, double* kept_T, int32_t* n_kept, int32_t* n_skipped,
+                          dib_stream_t stream);
+size_t oxford_build_count_workspace_bytes(int S, int w_stride);
+int oxford_build_count_f64(const double* x, const double* r, const int64_t* offsets, const int32_t* kept_scan,
+                           const int32_t* n_kept, int S, int w_stride, int use_mask, double threshold, int32_t* pos,
+                           int32_t* n_pts, double* rmax, void* workspace, size_t workspace_bytes,
+                           dib_stream_t stream);
+int oxford_build_scatter_f64(const double* x, const double* y, const double* r, const int64_t* offsets,
+                             const int32_t* kept_scan, const double* kept_T, const int32_t* n_kept,
+                             const int32_t* pos, const double* rmax, int S, int w_stride, int use_mask,
+                             double threshold, int n_stride, double* xyz_out, double* attr_out,
+                             dib_stream_t stream);
+int oxford_build_pack_f32(const double* xyz, const double* attr, const int32_t* m_pts, const double* rmax,
+                          const double* O, int S, int n_stride, int m_stride, float* out, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
