@@ -40,6 +40,8 @@ EXPORTS = (
     "png_decode_workspace_bytes", "png_decode_batch_u8",
     "oxford_build_plan_f64", "oxford_build_count_workspace_bytes", "oxford_build_count_f64",
     "oxford_build_scatter_f64", "oxford_build_pack_f32",
+    "oxford_debayer_workspace_bytes", "oxford_debayer_undistort_u8",
+    "jpeg_encode_workspace_bytes", "jpeg_encode_entropy_u8", "jpeg_encode_stuff_u8",
 )
 
 
@@ -267,6 +269,16 @@ def load():
     lib.oxford_build_scatter_f64.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f64, i32, vp, vp, vp]
     lib.oxford_build_pack_f32.restype = i32
     lib.oxford_build_pack_f32.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, vp, vp]
+    lib.oxford_debayer_workspace_bytes.restype = sz
+    lib.oxford_debayer_workspace_bytes.argtypes = [i32]
+    lib.oxford_debayer_undistort_u8.restype = i32
+    lib.oxford_debayer_undistort_u8.argtypes = [vp, sz, vp, i64, vp, i32, vp, sz, vp, sz, vp]
+    lib.jpeg_encode_workspace_bytes.restype = sz
+    lib.jpeg_encode_workspace_bytes.argtypes = [vp, i32]
+    lib.jpeg_encode_entropy_u8.restype = i32
+    lib.jpeg_encode_entropy_u8.argtypes = [vp, sz, vp, i32, vp, vp, vp, vp, sz, vp]
+    lib.jpeg_encode_stuff_u8.restype = i32
+    lib.jpeg_encode_stuff_u8.argtypes = [vp, i32, vp, vp, sz, vp, sz, vp]
     _lib = lib
     return lib
 

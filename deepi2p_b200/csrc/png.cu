@@ -1,6 +1,8 @@
 // Batched PNG decoding (8-bit truecolour, not interlaced), bit for bit with OpenCV 4.13 / libpng, straight into
-// imageprep.pack_images' HWC buffer.  DESIGN.md 4.23 states the contract; oracle_png/ is its CPU restatement, and
-// deepi2p_b200/png.py walks the chunks, checks the small critical chunks and packs the IDAT payloads on the host.
+// imageprep.pack_images' HWC buffer; 8-bit greyscale too when the descriptor's bytes-per-pixel slot says 1 (the
+// RobotCar Bayer mosaics, imageprep.decode_grey_png_batch, DESIGN.md 4.25).  DESIGN.md 4.23 states the contract;
+// oracle_png/ is its CPU restatement, and deepi2p_b200/png.py walks the chunks, checks the small critical chunks and
+// packs the IDAT payloads on the host.
 //
 // png_crc_kernel       warp per piece (at most kPiece bytes of one IDAT chunk): CRC-32 of the piece, each lane over a
 //                      contiguous slice, the slices combined in GF(2) (x^(8n) mod P, as zlib's crc32_combine does)
@@ -16,7 +18,7 @@
 // png_unfilter_kernel  CTA per image: the Adler-32 of the inflated data (sum and position-weighted sum, exact in
 //                      64 bits per thread at any supported size, reduced mod 65521 before the block sum), the
 //                      filter-byte check, then a row wavefront (thread per row and channel, row r one pixel behind
-//                      row r - 1) that undoes the five filters into HWC RGB
+//                      row r - 1) that undoes the five filters into HWC RGB (or H x W grey)
 //
 // Every input read is bounded by the packed data, every output write by the image's descriptor; a corrupt stream ends
 // in a status code.  Integer arithmetic only and no atomics, so a decode is bit-identical across runs and streams.
@@ -40,9 +42,10 @@ constexpr int kStage = 2048;                   // input stage ring, loaded kStag
 constexpr uint32_t kPoly = 0xEDB88320u;
 constexpr uint32_t kCrcIdat = 0x35AF061Eu;     // CRC-32 of the chunk type "IDAT"
 
-// Descriptor slots (int64), DIB_PNG_DESC of them per image; the caller fills 0..7 and 9, the library 8.
-enum { kInOff = 0, kInLen, kOutOff, kW, kH, kChunk0, kWbits, kSkip, kRawOff, kNChunk };
-static_assert(kNChunk < DIB_PNG_DESC, "descriptor slots");
+// Descriptor slots (int64), DIB_PNG_DESC of them per image; the caller fills 0..7, 9 and 10, the library 8.  kBpp is
+// the bytes per pixel: 0 (the default) or 3 for RGB, 1 for grey.
+enum { kInOff = 0, kInLen, kOutOff, kW, kH, kChunk0, kWbits, kSkip, kRawOff, kNChunk, kBpp };
+static_assert(kBpp < DIB_PNG_DESC, "descriptor slots");
 // Library chunk records in the workspace: the caller's four slots, then the chunk's first piece and piece count.
 constexpr int kChunkSlots = 6;
 
@@ -52,7 +55,9 @@ struct Layout {
   size_t desc, chunks, pieces, piece_crc, adler, raw, total;
 };
 
-__host__ __device__ inline int64_t raw_bytes(const int64_t* q) { return q[kSkip] ? 0 : q[kH] * (1 + 3 * q[kW]); }
+__host__ __device__ inline int64_t bpp(const int64_t* q) { return q[kBpp] ? q[kBpp] : 3; }
+
+__host__ __device__ inline int64_t raw_bytes(const int64_t* q) { return q[kSkip] ? 0 : q[kH] * (1 + bpp(q) * q[kW]); }
 
 // Fills the library's slots (raw offsets) and the piece list, and returns the workspace layout.
 inline Layout layout(std::vector<int64_t>& d, int S, std::vector<int64_t>& ch, int C, std::vector<int64_t>& pieces) {
@@ -519,7 +524,7 @@ __global__ void __launch_bounds__(kUnfThreads) png_unfilter_kernel(const int64_t
   const int s = blockIdx.x;
   const int64_t* q = desc + (size_t)s * DIB_PNG_DESC;
   if (q[kSkip] || status[4 * s]) return;                            // block-uniform
-  const int64_t w = q[kW], h = q[kH], stride = 1 + 3 * w, n = h * stride;
+  const int64_t w = q[kW], h = q[kH], B = bpp(q), stride = 1 + B * w, n = h * stride;
   const uint8_t* raw = raw_all + q[kRawOff];
   unsigned long long s1 = 0, s2 = 0;
   for (int64_t i = threadIdx.x; i < n; i += kUnfThreads) {
@@ -543,20 +548,20 @@ __global__ void __launch_bounds__(kUnfThreads) png_unfilter_kernel(const int64_t
   }
   if (bad) return;
   uint8_t* o = out + q[kOutOff];
-  const int t = threadIdx.x, c = t % 3;
-  for (int64_t r0 = 0; r0 < h; r0 += kRows) {
-    const int64_t r = r0 + t / 3;
+  const int t = threadIdx.x, c = t % (int)B, rows = kUnfThreads / (int)B;   // kRows rows of RGB, 3 kRows of grey
+  for (int64_t r0 = 0; r0 < h; r0 += rows) {
+    const int64_t r = r0 + t / B;
     const bool live = r < h;
     const int f = live ? raw[r * stride] : 0;
     const uint8_t* src = raw + r * stride + 1 + c;
-    uint8_t* dst = o + r * 3 * w + c;
+    uint8_t* dst = o + r * B * w + c;
     int left = 0, upleft = 0;
-    const int64_t steps = w + min((int64_t)kRows, h - r0) - 1;
+    const int64_t steps = w + min((int64_t)rows, h - r0) - 1;
     for (int64_t k = 0; k < steps; ++k) {
-      const int64_t x = k - t / 3;
+      const int64_t x = k - t / B;
       if (live && x >= 0 && x < w) {
-        const int v = src[3 * x];
-        const int up = r > 0 ? dst[3 * x - 3 * w] : 0;
+        const int v = src[B * x];
+        const int up = r > 0 ? dst[B * x - B * w] : 0;
         int pred;
         switch (f) {
           case 0: pred = 0; break;
@@ -570,7 +575,7 @@ __global__ void __launch_bounds__(kUnfThreads) png_unfilter_kernel(const int64_t
           }
         }
         const int val = (v + pred) & 255;
-        dst[3 * x] = (uint8_t)val;
+        dst[B * x] = (uint8_t)val;
         left = val;
         upleft = up;
       }
@@ -586,7 +591,8 @@ int check_desc(const int64_t* q, int s, size_t data_bytes, size_t out_bytes, con
   DIB_REQUIRE(q[kInOff] >= 0 && q[kInOff] % 16 == 0 && q[kInLen] >= 2 && (size_t)(q[kInOff] + q[kInLen]) <= data_bytes,
               "image %d: IDAT data [%lld, +%lld) outside the %zu-byte stream or not 16-byte aligned", s,
               (long long)q[kInOff], (long long)q[kInLen], data_bytes);
-  DIB_REQUIRE(q[kOutOff] >= 0 && (size_t)(q[kOutOff] + 3 * q[kW] * q[kH]) <= out_bytes,
+  DIB_REQUIRE(q[kBpp] == 0 || q[kBpp] == 1 || q[kBpp] == 3, "image %d: bytes per pixel %lld", s, (long long)q[kBpp]);
+  DIB_REQUIRE(q[kOutOff] >= 0 && (size_t)(q[kOutOff] + bpp(q) * q[kW] * q[kH]) <= out_bytes,
               "image %d: output outside the %zu-byte buffer", s, out_bytes);
   DIB_REQUIRE(q[kWbits] >= 8 && q[kWbits] <= 15, "image %d: window bits %lld", s, (long long)q[kWbits]);
   DIB_REQUIRE(q[kChunk0] >= 0 && q[kNChunk] >= 1 && q[kChunk0] + q[kNChunk] <= C, "image %d: chunk range", s);

@@ -6,7 +6,9 @@ loader), for S samples at once and bit for bit against cv2 and Pillow.
 pack_images packs ragged HWC uint8 frames into one device buffer, and decode_jpeg_batch / read_jpeg_batch decode the
 loaders' JPEG frames (Image.open(path).convert("RGB"), bit for bit; csrc/jpeg.cu, DESIGN.md 4.19) into the same
 buffer on the device, and decode_png_batch / read_png_batch do the same for KITTI's official PNG frames
-(cv2.imread(path)[:, :, ::-1], bit for bit; csrc/png.cu, DESIGN.md 4.23); image_params draws the per-sample crop offsets and
+(cv2.imread(path)[:, :, ::-1], bit for bit; csrc/png.cu, DESIGN.md 4.23); decode_grey_png_batch decodes 8-bit grey
+PNGs (the RobotCar Bayer mosaics) and encode_jpeg_batch encodes pack_images' frames as baseline JPEG, bit for bit with
+cv2.imencode (csrc/jpeg_encode.cu, DESIGN.md 4.25); image_params draws the per-sample crop offsets and
 jitter on the host; assemble_images runs csrc/imageprep.cu and composes K in fp64.  kitti_image_args /
 oxford_image_args / nuscenes_image_args are the loaders' options (nuScenes: crop_top_rows=100, img_scale=0.2, 160 x
 320, jitter_prob=0.5).  augment_img is a host drop-in for the loaders' augment_img that works on current torchvision.
@@ -17,10 +19,12 @@ import torch
 
 from . import _native
 from . import jpeg as _jpeg
+from . import jpeg_encode as _jpege
 from . import png as _png
 from .assemble import MODES
 from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace
 
+_JPEGE_DESC = 8                   # include/deepi2p_b200.h DIB_JPEGE_DESC
 IMAGE_PARAMS = 16                 # include/deepi2p_b200.h DIB_IMAGE_PARAMS and the DIB_IMG_* slots below
 _H, _W, _ROW0, _ROWS, _DH, _DW, _DY, _DX, _FLIP, _JITTER, _ORDER, _SHIFT = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 14
 JITTER_RANGES = dict(brightness=(0.8, 1.2), contrast=(0.8, 1.2), saturation=(0.8, 1.2), hue=(-0.1, 0.1))
@@ -150,11 +154,25 @@ def decode_png_batch(blobs, device="cuda", stream=None):
     than the image or that uses a distance beyond its declared window is rejected (DESIGN.md 4.23).  The error names
     the first bad image, ValueError("image i: <reason>"), and no output is returned for any image.  The call waits for
     the decode to finish (the per-image status is read back)."""
+    return _decode_png(blobs, device, stream, grey=False)
+
+
+def decode_grey_png_batch(blobs, device="cuda", stream=None):
+    """Decode S 8-bit greyscale PNG streams (bytes-like; the RobotCar stereo Bayer mosaics) on the GPU: dict(data
+    uint8 [sum h w] on `device` (image s is h x w, row-major, at offsets[s] and equal to
+    np.asarray(PIL.Image.open(BytesIO(b))), mode "L"), offsets int64 [S], shapes int64 [S,2] (h, w)).  Supported:
+    colour type 0 with bit depth 8, not interlaced, with everything else decode_png_batch accepts about the chunks,
+    the zlib stream and the filters; any other colour type or depth, and every stream decode_png_batch would reject,
+    raise ValueError("image i: <reason>") for the first bad image.  The call waits for the decode to finish."""
+    return _decode_png(blobs, device, stream, grey=True)
+
+
+def _decode_png(blobs, device, stream, grey):
     _require_cuda()
     lib = _native.load()
     dev = torch.device(device)
     S = len(blobs)
-    pk = _png.pack_batch(blobs)
+    pk = _png.pack_batch(blobs, grey=grey)
     bad = dict(pk["errors"])
     with torch.cuda.device(dev), torch.cuda.stream(stream):
         out = torch.empty(pk["out_bytes"], dtype=torch.uint8, device=dev)
@@ -189,6 +207,62 @@ def read_png_batch(paths, device="cuda", stream=None):
         with open(p, "rb") as f:
             blobs.append(f.read())
     return decode_png_batch(blobs, device=device, stream=stream)
+
+
+def encode_jpeg_batch(images, quality=95, stream=None):
+    """Encode pack_images' frames (dict: data uint8 on a CUDA device, HWC RGB, offsets, shapes) as baseline JPEG on the
+    GPU.  Returns a list of S bytes objects, item s equal to cv2.imencode(".jpg", rgb_s[:, :, ::-1],
+    [cv2.IMWRITE_JPEG_QUALITY, quality])[1].tobytes() on OpenCV 4.13 / libjpeg-turbo 3.1: 4:2:0, islow DCT, the Annex K
+    tables scaled to `quality` (1..100, baseline-clamped), standard Huffman tables, no restart markers, any size from
+    1 x 1 to 65500 per side (DESIGN.md 4.25).  The call waits: the per-image sizes are read back once before the
+    stuffed bytes are packed, then the bytes are copied to the host."""
+    _require_cuda()
+    lib = _native.load()
+    q = int(quality)
+    if not 1 <= q <= 100:
+        raise ValueError(f"quality must be in 1..100 (got {quality})")
+    data = images["data"]
+    if not (isinstance(data, torch.Tensor) and data.is_cuda and data.dtype == torch.uint8 and data.dim() == 1):
+        raise ValueError("images['data'] must be a 1-D uint8 CUDA tensor (pack_images)")
+    shapes = np.asarray(images["shapes"], dtype=np.int64).reshape(-1, 2)
+    offsets = np.asarray(images["offsets"], dtype=np.int64).reshape(-1)
+    S = shapes.shape[0]
+    if offsets.shape != (S,):
+        raise ValueError("images needs one offset per shape")
+    for s in range(S):
+        _jpege.check_shape(int(shapes[s, 0]), int(shapes[s, 1]), f"image {s}")
+        if offsets[s] < 0 or offsets[s] + 3 * shapes[s, 0] * shapes[s, 1] > data.numel():
+            raise ValueError(f"image {s}: lies outside images['data']")
+    if S == 0:
+        return []
+    desc = np.zeros((S, _JPEGE_DESC), np.int64)
+    desc[:, 0], desc[:, 1], desc[:, 2] = offsets, shapes[:, 0], shapes[:, 1]
+    quant = np.ascontiguousarray(_jpege.quant_tables(q), dtype=np.int32)
+    huff = np.ascontiguousarray(_jpege.device_tables())
+    dev = data.device
+    with torch.cuda.device(dev), torch.cuda.stream(stream):
+        sp = _stream_ptr(stream)
+        nws = lib.jpeg_encode_workspace_bytes(desc.ctypes.data, S)
+        if nws == 0:
+            raise _native.NativeError("jpeg_encode_workspace_bytes rejected the batch")
+        ws = _workspace(nws, dev, sp)
+        counts = torch.empty((S, 2), dtype=torch.int64, device=dev)
+        rc = lib.jpeg_encode_entropy_u8(_ptr(data), data.numel(), desc.ctypes.data, S, quant.ctypes.data,
+                                        huff.ctypes.data, _ptr(counts), _ptr(ws), ws.numel(), sp)
+        _native.check(rc, "jpeg_encode_entropy")
+        n = counts.cpu().numpy()
+        sizes = n[:, 0] + n[:, 1]
+        out_off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64))
+        out = torch.empty(max(int(sizes.sum()), 1), dtype=torch.uint8, device=dev)
+        rc = lib.jpeg_encode_stuff_u8(desc.ctypes.data, S, out_off.ctypes.data, _ptr(out), out.numel(), _ptr(ws),
+                                      ws.numel(), sp)
+        _native.check(rc, "jpeg_encode_stuff")
+        host = out.cpu().numpy()
+    headers = {}
+    for h, w in shapes:
+        if (h, w) not in headers:
+            headers[h, w] = _jpege.header(int(h), int(w), q)
+    return [b"".join((headers[h, w], host[o:o + z].data, _jpege.EOI)) for (h, w), o, z in zip(shapes, out_off, sizes)]
 
 
 def image_params(shapes, mode, rng=None, img_H=160, img_W=512, img_scale=0.5, crop_top_rows=0, crop_bottom_rows=0,

@@ -510,14 +510,17 @@ def is_night(raw, t):
     return "night" in read_tags(os.path.join(raw, t, "tags.csv"))
 
 
-def build_traversal(raw, lms, out, t, sdk_dir, batch=64, device="cuda", stream=None, **params):
-    """save_pc_img_for_traversal (point clouds and both tables; images are not converted) for traversal t, writing
-    <out>/<t>/lms_front[_foreground]/<ts>.npy, pc_timestamps.npy, pc_poses.npy, camera_timestamps.npy,
-    camera_poses.npy and, as the last step, a copy of tags.csv.  Every built cloud is listed, whether or not its record
-    existed before.  The device work and its read-backs run on `stream` (the current stream when None).  Returns a
-    summary dict: clouds_built, clouds_skipped_velocity, scans_skipped (summed over the clouds), scans_missing (distinct
-    LMS timestamps without a scan file in the built clouds' windows), cameras_outside_vo, camera_frames, and per cloud
-    n_kept / n_skipped / m_pts."""
+def build_traversal(raw, lms, out, t, sdk_dir, batch=64, device="cuda", stream=None, images=False, **params):
+    """save_pc_img_for_traversal for traversal t, writing <out>/<t>/lms_front[_foreground]/<ts>.npy, pc_timestamps.npy,
+    pc_poses.npy, camera_timestamps.npy, camera_poses.npy and, as the last step, a copy of tags.csv.  Every built
+    cloud is listed, whether or not its record existed before.  With images=True the stereo-centre frames are
+    converted too (build_dataset.py:356-377, oxford_images.convert_frames with the SDK's
+    models/stereo_narrow_left_distortion_lut.bin): every frame of the camera table whose PNG exists and whose
+    <out>/<t>/stereo/centre/<ts>.jpg does not yet exist, before tags.csv is written.  The device work and its
+    read-backs run on `stream` (the current stream when None).  Returns a summary dict: clouds_built,
+    clouds_skipped_velocity, scans_skipped (summed over the clouds), scans_missing (distinct LMS timestamps without a
+    scan file in the built clouds' windows), cameras_outside_vo, camera_frames, per cloud n_kept / n_skipped / m_pts,
+    and with images=True images_converted and images_skipped (frames whose JPEG already existed)."""
     if int(batch) < 1:
         raise ValueError(f"batch must be positive (got {batch})")
     plan = plan_traversal(raw, lms, out, t, sdk_dir, **params)
@@ -547,11 +550,39 @@ def build_traversal(raw, lms, out, t, sdk_dir, batch=64, device="cuda", stream=N
     np.save(os.path.join(d, "pc_poses.npy"), np.asarray(plan["pc_poses"], dtype=np.float64))
     np.save(os.path.join(d, "camera_timestamps.npy"), plan["camera_timestamps"])
     np.save(os.path.join(d, "camera_poses.npy"), np.asarray(plan["camera_poses"], dtype=np.float64))
+    summary = dict(traversal=t, clouds_built=n, clouds_skipped_velocity=len(plan["skipped_velocity"]),
+                   scans_skipped=int(n_skipped.sum()), scans_missing=missing,
+                   cameras_outside_vo=plan["cameras_outside_vo"], camera_frames=len(plan["camera_timestamps"]),
+                   n_kept=n_kept, n_skipped=n_skipped, m_pts=m_pts)
+    if images:
+        summary.update(convert_images(raw, out, t, sdk_dir, plan["camera_timestamps"], batch, device, stream))
     shutil.copy(os.path.join(raw, t, "tags.csv"), os.path.join(d, "tags.csv"))
-    return dict(traversal=t, clouds_built=n, clouds_skipped_velocity=len(plan["skipped_velocity"]),
-                scans_skipped=int(n_skipped.sum()), scans_missing=missing,
-                cameras_outside_vo=plan["cameras_outside_vo"], camera_frames=len(plan["camera_timestamps"]),
-                n_kept=n_kept, n_skipped=n_skipped, m_pts=m_pts)
+    return summary
+
+
+def convert_images(raw, out, t, sdk_dir, cameras, batch=64, device="cuda", stream=None):
+    """build_dataset.py:356-377 for the frames `cameras` of traversal t: each <raw>/<t>/stereo/centre/<ts>.png without
+    a <out>/<t>/stereo/centre/<ts>.jpg is converted (oxford_images.convert_frames).  Returns dict(images_converted,
+    images_skipped)."""
+    from . import oxford_images
+    from .png import parse_png
+    src = os.path.join(raw, t, "stereo", "centre")
+    dst = os.path.join(out, t, "stereo", "centre")
+    todo = [c for c in cameras if not os.path.isfile(os.path.join(dst, "%d.jpg" % c))
+            and os.path.isfile(os.path.join(src, "%d.png" % c))]
+    skipped = len(cameras) - len(todo)
+    if todo:
+        first = os.path.join(src, "%d.png" % todo[0])
+        with open(first, "rb") as f:
+            try:
+                hd = parse_png(f.read(), grey=True)
+            except ValueError as e:
+                raise ValueError(f"{first}: {e}") from None
+        lut = oxford_images.read_distortion_lut(os.path.join(sdk_dir, "models", oxford_images.LUT_FILE), hd.H, hd.W)
+        oxford_images.convert_frames([os.path.join(src, "%d.png" % c) for c in todo],
+                                     [os.path.join(dst, "%d.jpg" % c) for c in todo], lut, batch=batch,
+                                     device=device, stream=stream)
+    return dict(images_converted=len(todo), images_skipped=skipped)
 
 
 def select_traversals(raw, out, traversals=None):
@@ -586,9 +617,9 @@ def write_train_split(out):
     return train
 
 
-def build_root(raw, lms, out, sdk_dir, traversals=None, batch=64, log=print, **params):
-    """main(): every selected traversal in turn on one GPU, then train.txt when val.txt exists.  Returns the
-    traversals' summaries."""
+def build_root(raw, lms, out, sdk_dir, traversals=None, batch=64, log=print, images=False, **params):
+    """main(): every selected traversal in turn on one GPU (converting the stereo-centre frames too with
+    images=True), then train.txt when val.txt exists.  Returns the traversals' summaries."""
     todo, night, done = select_traversals(raw, out, traversals)
     for t in night:
         log(f"{t} is night driving, skip.")
@@ -596,10 +627,12 @@ def build_root(raw, lms, out, sdk_dir, traversals=None, batch=64, log=print, **p
         log(f"{t} is already done, skip.")
     out_s = []
     for t in todo:
-        s = build_traversal(raw, lms, out, t, sdk_dir, batch=batch, **params)
+        s = build_traversal(raw, lms, out, t, sdk_dir, batch=batch, images=images, **params)
         log(f"{t}: {s['clouds_built']} clouds, {s['clouds_skipped_velocity']} skipped for velocity, "
             f"{s['scans_skipped']} scans skipped, {s['scans_missing']} scan files missing, {s['camera_frames']} camera "
-            f"frames ({s['cameras_outside_vo']} outside the VO span dropped)")
+            f"frames ({s['cameras_outside_vo']} outside the VO span dropped)"
+            + (f", {s['images_converted']} images converted, {s['images_skipped']} already converted or without a PNG"
+               if images else ""))
         out_s.append(s)
     write_train_split(out)
     return out_s

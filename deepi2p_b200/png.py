@@ -14,6 +14,7 @@ import numpy as np
 
 SIGNATURE = b"\x89PNG\r\n\x1a\n"
 DESC = 12                 # int64 slots of one image descriptor (the slot enum at the top of csrc/png.cu)
+BPP_SLOT = 10             # descriptor slot of the bytes per pixel: 0 (RGB) or 1 (grey)
 CHUNK = 4                 # int64 slots of one IDAT chunk record: image, data offset, length, expected CRC-32
 ALIGN = 16                # each image's IDAT payload starts at a multiple of ALIGN in the packed data
 MAX_SIDE = 1 << 20        # OpenCV's CV_IO_MAX_IMAGE_WIDTH / HEIGHT
@@ -29,8 +30,9 @@ class PngHeader(dict):
     __getattr__ = dict.__getitem__
 
 
-def parse_png(blob):
-    """Chunk structure of one PNG stream.  Returns a PngHeader with W, H, window (the LZ77 window the zlib header
+def parse_png(blob, grey=False):
+    """Chunk structure of one PNG stream.  With grey=True the supported colour type is 8-bit greyscale (0) instead of
+    8-bit truecolour (2).  Returns a PngHeader with W, H, window (the LZ77 window the zlib header
     declares, in bytes) and idat (a list of (payload offset in blob, payload length, expected CRC-32) of the IDAT
     chunks, in order).  Raises ValueError naming the reason for a stream outside the supported set or one libpng
     rejects before inflating: a bad signature, a truncated chunk, a bad IHDR, PLTE or IEND CRC, an unknown critical
@@ -70,7 +72,7 @@ def parse_png(blob):
             if ctype == b"IHDR":
                 if hdr is not None:
                     raise ValueError("IHDR: out of place")
-                hdr = _ihdr(bytes(b[data_off:data_off + length]))
+                hdr = _ihdr(bytes(b[data_off:data_off + length]), grey)
             elif ctype == b"PLTE":
                 if seen_idat or seen_plte or length % 3 or length == 0 or length > 768:
                     raise ValueError("PLTE: invalid or out of place")
@@ -102,7 +104,7 @@ def parse_png(blob):
     return PngHeader(W=hdr[0], H=hdr[1], window=1 << ((cmf >> 4) + 8), idat=idat, idat_bytes=total)
 
 
-def _ihdr(d):
+def _ihdr(d, grey=False):
     if len(d) != 13:
         raise ValueError("IHDR: invalid length")
     w, h, depth, ctype, comp, filt, interlace = struct.unpack(">IIBBBBB", d)
@@ -112,7 +114,9 @@ def _ihdr(d):
         raise ValueError(f"IHDR: invalid colour type {ctype} with bit depth {depth}")
     if comp != 0 or filt != 0 or interlace > 1:
         raise ValueError("IHDR: invalid compression, filter or interlace method")
-    if (ctype, depth) != (2, 8):
+    if grey and (ctype, depth) != (0, 8):
+        raise ValueError(f"unsupported colour type {ctype} with bit depth {depth} (only 8-bit grey is decoded here)")
+    if not grey and (ctype, depth) != (2, 8):
         raise ValueError(f"unsupported colour type {ctype} with bit depth {depth} (only 8-bit RGB is decoded)")
     if interlace:
         raise ValueError("unsupported interlace method (Adam7)")
@@ -121,8 +125,8 @@ def _ihdr(d):
     return w, h
 
 
-def pack_batch(blobs):
-    """Parse S streams and pack the decoder's inputs: dict(data uint8 (each image's concatenated IDAT payloads,
+def pack_batch(blobs, grey=False):
+    """Parse S streams (8-bit greyscale ones with grey=True, one output byte per pixel) and pack the decoder's inputs: dict(data uint8 (each image's concatenated IDAT payloads,
     ALIGN-aligned and zero-padded), desc int64 [S, DESC], chunks int64 [C, CHUNK], offsets int64 [S] (output byte
     offsets), shapes int64 [S, 2] (h, w), out_bytes, errors (a dict image -> reason of the streams the host already
     rejected; those images get empty descriptors and no output bytes))."""
@@ -133,14 +137,14 @@ def pack_batch(blobs):
     for s, blob in enumerate(blobs):
         mv = memoryview(blob).cast("B")
         try:
-            hd = parse_png(mv)
+            hd = parse_png(mv, grey)
         except ValueError as e:
             errors[s] = str(e)
             desc[s, 7] = 1
             continue
         d = desc[s]
         d[0], d[1], d[3], d[4], d[6] = pos, hd.idat_bytes, hd.W, hd.H, hd.window.bit_length() - 1
-        d[5], d[9] = len(chunks), len(hd.idat)
+        d[5], d[9], d[BPP_SLOT] = len(chunks), len(hd.idat), 1 if grey else 0
         p = pos
         for off, l, crc in hd.idat:
             chunks.append((s, p, l, crc))
@@ -152,7 +156,7 @@ def pack_batch(blobs):
     data = np.zeros(max(pos, ALIGN), np.uint8)
     for p, part in parts:
         data[p:p + len(part)] = np.frombuffer(part, np.uint8)
-    sizes = 3 * shapes[:, 0] * shapes[:, 1]
+    sizes = (1 if grey else 3) * shapes[:, 0] * shapes[:, 1]
     offsets = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64) if S else np.zeros(0, np.int64)
     desc[:, 2] = offsets
     chunks = np.array(chunks, np.int64).reshape(-1, CHUNK)

@@ -600,7 +600,8 @@ def write_oxford_sdk(sdk):
 
 def write_oxford_raw(raw, lms, sdk, traversals=("2014-05-19-13-20-57",), night=("2014-12-10-18-10-50",), seconds=30.0,
                      speed=5.0, stops=((8.0, 9.5), (14.0, 17.0)), curve=(6.0, 11.0), yaw_rate=0.15, zero_reflectance_after=None,
-                     n_returns=60, missing_scans=0.03, missing_images=0.05, vo_on_cameras=False, seed=0):
+                     n_returns=60, missing_scans=0.03, missing_images=0.05, vo_on_cameras=False, seed=0,
+                     image_shape=None):
     """Seeded raw RobotCar traversals in the layout build_dataset.py reads: <raw>/<t>/vo/vo.csv (16 Hz rows whose
     chain abs_k = abs_{k-1} se3(row k) is the drive: `speed` m/s, standing still during each of `stops` (seconds from
     the start), turning at yaw_rate rad/s during `curve`), <raw>/<t>/stereo.timestamps (16 Hz; with vo_on_cameras the
@@ -610,8 +611,14 @@ def write_oxford_raw(raw, lms, sdk, traversals=("2014-05-19-13-20-57",), night=(
     <lms>/<t>/lms_front.timestamps with 50 Hz <lms>/<t>/lms_front/<ts>.bin scans of n_returns float64 (x, y,
     reflectance) triples (a fraction missing_scans absent; some x exactly 0.1; reflectance zero from
     zero_reflectance_after seconds on).  night names traversals tagged night.  Also writes the SDK files into sdk.
-    Returns {traversal: dict(vo=..., lms=..., cameras=...)} of timestamp lists."""
+    With image_shape=(h, w) the PNGs are seeded 8-bit GBRG Bayer mosaics of that size (oxford_mosaic) and the SDK gets
+    a seeded radial models/stereo_narrow_left_distortion_lut.bin (oxford_distortion_lut); the other files are the same
+    as without.  Returns {traversal: dict(vo=..., lms=..., cameras=...)} of timestamp lists."""
     write_oxford_sdk(sdk)
+    if image_shape is not None:
+        h, w = (int(v) for v in image_shape)
+        lut = oxford_distortion_lut(h, w, seed)
+        np.concatenate([lut[:, 0], lut[:, 1]]).tofile(os.path.join(sdk, "models", "stereo_narrow_left_distortion_lut.bin"))
     out = {}
     for t_i, t in enumerate(tuple(traversals) + tuple(night)):
         rng = np.random.default_rng(seed * 1000 + t_i + 0x0B5)
@@ -639,7 +646,12 @@ def write_oxford_raw(raw, lms, sdk, traversals=("2014-05-19-13-20-57",), night=(
             f.write("".join("%d 1\n" % c for c in cams))
         for c in cams:
             if rng.random() >= missing_images:
-                open(os.path.join(d, "stereo", "centre", "%d.png" % c), "wb").close()
+                path = os.path.join(d, "stereo", "centre", "%d.png" % c)
+                if image_shape is None:
+                    open(path, "wb").close()
+                else:
+                    with open(path, "wb") as f:
+                        f.write(encode_png(oxford_mosaic(image_shape, c)))
         with open(os.path.join(d, "tags.csv"), "w") as f:
             f.write("night,rain\n" if t in night else "overcast,roadworks\n")
         ld = os.path.join(lms, t, "lms_front")
@@ -662,6 +674,33 @@ def write_oxford_raw(raw, lms, sdk, traversals=("2014-05-19-13-20-57",), night=(
     return out
 
 
+def oxford_mosaic(shape, seed):
+    """A seeded 8-bit Bayer mosaic of shape (h, w): smooth gradients and a disc under noise, with saturated and black
+    specks, so that demosaicing, the borders and the JPEG encoder's 0xFF bytes all get exercised."""
+    h, w = (int(v) for v in shape)
+    rng = np.random.default_rng(int(seed) & 0xFFFFFFFF)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    a, b, c = rng.uniform(0.5, 3.0, 3)
+    img = 128 + 60 * np.sin(a * xx / w * 6.28 + b) * np.cos(c * yy / h * 6.28)
+    cy, cx, r = rng.uniform(0, h), rng.uniform(0, w), rng.uniform(0.1, 0.4) * min(h, w)
+    img += np.where((yy - cy) ** 2 + (xx - cx) ** 2 < r * r, 70.0, 0.0)
+    img += rng.normal(0.0, 12.0, (h, w))
+    img[rng.random((h, w)) < 0.01] = 255
+    img[rng.random((h, w)) < 0.01] = 0
+    return np.clip(np.rint(img), 0, 255).astype(np.uint8)
+
+
+def oxford_distortion_lut(h, w, seed=0):
+    """A seeded radial undistortion LUT in the SDK's layout: float64 [h w, 2] of (x, y) source coordinates, (x - cx)
+    scaled by 1 + k r^2 about a centre near the middle; the corners map slightly outside the image."""
+    rng = np.random.default_rng(int(seed) + 0x1C7)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    cx, cy = (w - 1) / 2 + rng.uniform(-2, 2), (h - 1) / 2 + rng.uniform(-2, 2)
+    k = rng.uniform(0.05, 0.15) / ((w / 2) ** 2 + (h / 2) ** 2)
+    r2 = (xx - cx) ** 2 + (yy - cy) ** 2
+    return np.stack([(cx + (xx - cx) * (1 + k * r2)).ravel(), (cy + (yy - cy) * (1 + k * r2)).ravel()], 1)
+
+
 def png_chunk(ctype, data, crc=None):
     """One PNG chunk: length, type, data and CRC-32 (the correct one unless `crc` is given)."""
     c = zlib.crc32(ctype + data) if crc is None else crc
@@ -669,19 +708,20 @@ def png_chunk(ctype, data, crc=None):
 
 
 def png_filter(img, filters):
-    """The filtered scanlines of an HWC uint8 RGB image: each row prefixed by its filter type (filters: one int for
-    every row, or one per row) and filtered with 3 bytes per pixel, mod 256."""
-    h, w, _ = img.shape
-    x = img.reshape(h, 3 * w).astype(np.int64)
-    up = np.vstack([np.zeros((1, 3 * w), np.int64), x[:-1]])
-    left = np.hstack([np.zeros((h, 3), np.int64), x[:, :-3]])
-    ul = np.hstack([np.zeros((h, 3), np.int64), up[:, :-3]])
+    """The filtered scanlines of an HWC uint8 RGB image (or an HW grey one): each row prefixed by its filter type
+    (filters: one int for every row, or one per row) and filtered with 3 (grey: 1) bytes per pixel, mod 256."""
+    h, w = img.shape[:2]
+    bpp = 1 if img.ndim == 2 else 3
+    x = img.reshape(h, bpp * w).astype(np.int64)
+    up = np.vstack([np.zeros((1, bpp * w), np.int64), x[:-1]])
+    left = np.hstack([np.zeros((h, bpp), np.int64), x[:, :-bpp]])
+    ul = np.hstack([np.zeros((h, bpp), np.int64), up[:, :-bpp]])
     p = left + up - ul
     pa, pb, pc = np.abs(p - left), np.abs(p - up), np.abs(p - ul)
     paeth = np.where((pa <= pb) & (pa <= pc), left, np.where(pb <= pc, up, ul))
     preds = [np.zeros_like(x), left, up, (left + up) >> 1, paeth]
     f = np.broadcast_to(np.asarray(filters, np.int64), (h,))
-    out = np.empty((h, 3 * w + 1), np.uint8)
+    out = np.empty((h, bpp * w + 1), np.uint8)
     out[:, 0] = f
     for k in range(5):
         out[f == k, 1:] = (x - preds[k])[f == k] & 255
@@ -689,15 +729,17 @@ def png_filter(img, filters):
 
 
 def encode_png(img, filters=4, level=6, wbits=15, idat=8192, zdata=None, ancillary=True):
-    """A PNG stream of an HWC uint8 RGB image from the standard library: png_filter's scanlines through zlib at
-    `level` with a 2^wbits window, split into IDAT chunks of `idat` bytes (an int, or a list of chunk lengths, the last
-    taking the rest); zdata replaces the zlib stream.  ancillary adds a tEXt chunk before the IDATs."""
+    """A PNG stream of an HWC uint8 RGB image (an HW one: 8-bit grey) from the standard library: png_filter's
+    scanlines through zlib at `level` with a 2^wbits window, split into IDAT chunks of `idat` bytes (an int, or a list
+    of chunk lengths, the last taking the rest); zdata replaces the zlib stream.  ancillary adds a tEXt chunk before
+    the IDATs."""
     img = np.ascontiguousarray(img, np.uint8)
-    h, w, _ = img.shape
+    h, w = img.shape[:2]
     if zdata is None:
         co = zlib.compressobj(level, zlib.DEFLATED, wbits)
         zdata = co.compress(png_filter(img, filters)) + co.flush()
-    parts = [b"\x89PNG\r\n\x1a\n", png_chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 2, 0, 0, 0))]
+    ctype = 0 if img.ndim == 2 else 2
+    parts = [b"\x89PNG\r\n\x1a\n", png_chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, ctype, 0, 0, 0))]
     if ancillary:
         parts.append(png_chunk(b"tEXt", b"Software\0deepi2p_b200"))
     sizes = list(idat) if isinstance(idat, (list, tuple)) else None

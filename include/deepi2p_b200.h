@@ -697,9 +697,10 @@ int pointwise_mlp_f32(const int64_t* sources, int n_sources, const int64_t* laye
  * data: [dev] data_bytes bytes holding each image's IDAT payloads, each starting 16-byte aligned (no padding is
  *   needed after the last).
  *   desc: [host] int64 [S][DIB_PNG_DESC]: 0 data offset, 1 IDAT bytes, 2 out offset, 3 w, 4 h, 5 first chunk,
- *   6 log2 of the zlib window, 7 skip (1: no work and no output for this image), 9 chunk count; slot 8 is the
- *   library's.  chunks: [host] int64 [n_chunks][4]: image, data offset, payload length, stored CRC-32 of each IDAT
- *   chunk, an image's chunks consecutive and covering its data.  out: [dev] out_bytes bytes, image s at its offset.
+ *   6 log2 of the zlib window, 7 skip (1: no work and no output for this image), 9 chunk count, 10 bytes per pixel
+ *   (0 or 3: RGB; 1: 8-bit grey, h x w output bytes); slot 8 is the library's.  chunks: [host] int64 [n_chunks][4]:
+ *   image, data offset, payload length, stored CRC-32 of each IDAT chunk, an image's chunks consecutive and covering
+ *   its data.  out: [dev] out_bytes bytes, image s at its offset.
  *   status: [dev] int32 [S][4]: the inflate code, the chunk CRC code, the Adler-32 code and the filter code of image s
  *   (DIB_PNG_*, 0 = fine); the pixels of an image with any non-zero code are unspecified.  workspace: [dev] 256-byte
  *   aligned, >= png_decode_workspace_bytes(desc, S, chunks, n_chunks, data_bytes) (0 for invalid descriptors).
@@ -772,6 +773,42 @@ int oxford_build_scatter_f64(const double* x, const double* y, const double* r, 
                              dib_stream_t stream);
 int oxford_build_pack_f32(const double* xyz, const double* attr, const int32_t* m_pts, const double* rmax,
                           const double* O, int S, int n_stride, int m_stride, float* out, dib_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Oxford RobotCar stereo-centre frames (the SDK's load_image for the stereo camera).  DESIGN.md 4.25 states the
+ * contract: GBRG bilinear demosaicing (colour_demosaicing, float64, scipy 'reflect' borders) and the undistortion LUT
+ * through scipy's map_coordinates(order=1, mode 'constant'), then numpy's uint8 cast, bit for bit.
+ *
+ * oxford_debayer_undistort_u8: grey [dev] grey_bytes bytes, image s an h x w mosaic at desc offset 0; lut [dev]
+ *   16-byte aligned float64 (x, y) pairs, lut_pairs of them, image s reading the h w pairs from desc slot 4; desc
+ *   [host] int64 [S][DIB_OXIMG_DESC]: 0 mosaic offset, 1 output offset, 2 h, 3 w, 4 first LUT pair (h, w in
+ *   2..65536); out [dev] HWC RGB uint8, image s at its offset.  workspace [dev] >= oxford_debayer_workspace_bytes(S).
+ *
+ * Batched baseline JPEG encoding (4:2:0, quality tables given, Annex K Huffman tables, no restart markers), bit for
+ * bit with OpenCV 4.13's cv2.imencode(".jpg") on libjpeg-turbo 3.1; deepi2p_b200/jpeg_encode.py builds the tables
+ * and the markers around the entropy-coded data.
+ *
+ * jpeg_encode_entropy_u8: rgb [dev] HWC uint8; desc [host] int64 [S][DIB_JPEGE_DESC]: 0 input offset, 1 h, 2 w
+ *   (1..65500), the other slots the library's; quant [host] int32 [2][64] luma and chroma quantisers in natural order
+ *   (1..255); huff [host] int32 [4][256] (length << 16) | code per symbol of the DC luma, AC luma, DC chroma and AC
+ *   chroma tables.  Codes every image into the workspace and writes counts [dev] int64 [S][2]: the entropy-coded
+ *   bytes before stuffing (padded with 1 bits) and their number of 0xFF bytes.
+ * jpeg_encode_stuff_u8: the same desc and workspace, after jpeg_encode_entropy_u8 on the same stream: writes image s's
+ *   bytes, each 0xFF followed by 0x00, to out [dev] at out_off[s] [host] (its bytes + 0xFF count long).
+ *   workspace [dev] 256-byte aligned, >= jpeg_encode_workspace_bytes(desc, S) (0 for invalid descriptors).
+ * ------------------------------------------------------------------------------------------ */
+#define DIB_OXIMG_DESC 8
+size_t oxford_debayer_workspace_bytes(int S);
+int oxford_debayer_undistort_u8(const uint8_t* grey, size_t grey_bytes, const double* lut, int64_t lut_pairs,
+                                const int64_t* desc, int S, uint8_t* out, size_t out_bytes, void* workspace,
+                                size_t workspace_bytes, dib_stream_t stream);
+#define DIB_JPEGE_DESC 8
+size_t jpeg_encode_workspace_bytes(const int64_t* desc, int S);
+int jpeg_encode_entropy_u8(const uint8_t* rgb, size_t rgb_bytes, const int64_t* desc, int S, const int32_t* quant,
+                           const int32_t* huff, int64_t* counts, void* workspace, size_t workspace_bytes,
+                           dib_stream_t stream);
+int jpeg_encode_stuff_u8(const int64_t* desc, int S, const int64_t* out_off, uint8_t* out, size_t out_bytes,
+                         void* workspace, size_t workspace_bytes, dib_stream_t stream);
 
 #ifdef __cplusplus
 }

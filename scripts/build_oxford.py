@@ -1,7 +1,7 @@
 """Build an Oxford RobotCar root from the raw downloads (data/oxford/build_dataset.py's main(), one GPU, traversals in
 turn):
 
-    python scripts/build_oxford.py RAW LMS OUT --sdk DIR [--traversals T ...] [--batch 64]
+    python scripts/build_oxford.py RAW LMS OUT --sdk DIR [--traversals T ...] [--batch 64] [--images]
 
 RAW holds <t>/vo/vo.csv, <t>/stereo.timestamps, <t>/stereo/centre/<ts>.png and <t>/tags.csv; LMS holds
 <t>/lms_front.timestamps and <t>/lms_front/<ts>.bin; DIR is the RobotCar SDK, of which only models/ and extrinsics/
@@ -28,10 +28,12 @@ def main(argv=None):
     ap.add_argument("out", metavar="OUT")
     ap.add_argument("--sdk", required=True, help="RobotCar SDK directory (models/, extrinsics/)")
     ap.add_argument("--traversals", nargs="+", default=None, help="only these traversals (default: all of RAW)")
-    ap.add_argument("--batch", type=positive, default=64, help="clouds per device call")
+    ap.add_argument("--batch", type=positive, default=64, help="clouds (and images) per device call")
+    ap.add_argument("--images", action="store_true", help="also convert the stereo-centre PNGs to JPEG")
     a = ap.parse_args(argv)
     from deepi2p_b200 import oxford_build
-    oxford_build.build_root(a.raw, a.lms, a.out, a.sdk, traversals=a.traversals, batch=a.batch)
+    oxford_build.build_root(a.raw, a.lms, a.out, a.sdk, traversals=a.traversals, batch=a.batch,
+                            images=a.images)
 
 
 if __name__ == "__main__":
