@@ -42,6 +42,8 @@ EXPORTS = (
     "oxford_build_scatter_f64", "oxford_build_pack_f32",
     "oxford_debayer_workspace_bytes", "oxford_debayer_undistort_u8",
     "jpeg_encode_workspace_bytes", "jpeg_encode_entropy_u8", "jpeg_encode_stuff_u8",
+    "knn_fusion_packed_bytes", "knn_fusion_pack_f32", "knn_fusion_f32", "pointwise_mlp_max_packed_bytes",
+    "pointwise_mlp_max_pack_f32", "pointwise_mlp_max_workspace_bytes", "pointwise_mlp_max_f32",
 )
 
 
@@ -254,6 +256,20 @@ def load():
     lib.pointwise_mlp_workspace_bytes.argtypes = [vp, i32, vp, i32, i32]
     lib.pointwise_mlp_f32.restype = i32
     lib.pointwise_mlp_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, i32, vp, vp, vp, vp, sz, vp]
+    lib.knn_fusion_packed_bytes.restype = sz
+    lib.knn_fusion_packed_bytes.argtypes = [i32, vp, i32, i32]
+    lib.knn_fusion_pack_f32.restype = i32
+    lib.knn_fusion_pack_f32.argtypes = [i32, vp, i32, i32, vp, sz, vp]
+    lib.knn_fusion_f32.restype = i32
+    lib.knn_fusion_f32.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, sz, vp, vp, vp]
+    lib.pointwise_mlp_max_packed_bytes.restype = sz
+    lib.pointwise_mlp_max_packed_bytes.argtypes = [i32, vp, i32]
+    lib.pointwise_mlp_max_pack_f32.restype = i32
+    lib.pointwise_mlp_max_pack_f32.argtypes = [i32, vp, i32, vp, sz, vp]
+    lib.pointwise_mlp_max_workspace_bytes.restype = sz
+    lib.pointwise_mlp_max_workspace_bytes.argtypes = [i32, i32, i32]
+    lib.pointwise_mlp_max_f32.restype = i32
+    lib.pointwise_mlp_max_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, vp, vp, sz, vp]
     lib.png_decode_workspace_bytes.restype = sz
     lib.png_decode_workspace_bytes.argtypes = [vp, i32, vp, i32, sz]
     lib.png_decode_batch_u8.restype = i32

@@ -101,6 +101,24 @@ __global__ void __launch_bounds__(kKnnThreads)
     if (j < K) o[j] = bi[j];
 }
 
+// knn_idx [B][M][K] of knn_group_forward_f32 (also the indices knn_fusion.cu groups by); the caller checks the shape
+int knn_search_launch(const float* query, const float* database, int B, int M, int N, int K, int32_t* knn_idx,
+                      cudaStream_t stream) {
+  const size_t smem = (size_t)3 * N * sizeof(float);            // <= 24 KB
+  dim3 grid((M + kKnnThreads - 1) / kKnnThreads, B);
+#define DIB_KS_LAUNCH(KK) \
+  knn_search_kernel<KK><<<grid, kKnnThreads, smem, stream>>>(query, database, M, N, K, knn_idx)
+  if (K <= 1) DIB_KS_LAUNCH(1);
+  else if (K <= 2) DIB_KS_LAUNCH(2);
+  else if (K <= 4) DIB_KS_LAUNCH(4);
+  else if (K <= 8) DIB_KS_LAUNCH(8);
+  else if (K <= 16) DIB_KS_LAUNCH(16);
+  else DIB_KS_LAUNCH(32);
+#undef DIB_KS_LAUNCH
+  DIB_CHECK_CUDA(cudaGetLastError());
+  return DIB_OK;
+}
+
 // grid (ceil(M * K / 256), ceil((3 + C) / 16), B)
 __global__ void __launch_bounds__(kGroupThreads)
     knn_group_kernel(const float* __restrict__ query, const float* __restrict__ database,
@@ -345,18 +363,8 @@ int knn_group_forward_f32(const float* query, const float* database, const float
   DIB_REQUIRE(query && database && knn_idx && grouped && (C == 0 || features), "knn_group: NULL argument");
   DIB_REQUIRE((3 + C + kGroupRows - 1) / kGroupRows <= 65535, "knn_group: too many channels");
   DIB_REQUIRE((long long)M * K <= 0x7fffffffLL, "knn_group: M * K must fit in int32");
-  const size_t smem = (size_t)3 * N * sizeof(float);            // <= 24 KB
-  dim3 grid((M + kKnnThreads - 1) / kKnnThreads, B);
-#define DIB_KS_LAUNCH(KK) \
-  knn_search_kernel<KK><<<grid, kKnnThreads, smem, stream>>>(query, database, M, N, K, knn_idx)
-  if (K <= 1) DIB_KS_LAUNCH(1);
-  else if (K <= 2) DIB_KS_LAUNCH(2);
-  else if (K <= 4) DIB_KS_LAUNCH(4);
-  else if (K <= 8) DIB_KS_LAUNCH(8);
-  else if (K <= 16) DIB_KS_LAUNCH(16);
-  else DIB_KS_LAUNCH(32);
-#undef DIB_KS_LAUNCH
-  DIB_CHECK_CUDA(cudaGetLastError());
+  const int rc = knn_search_launch(query, database, B, M, N, K, knn_idx, stream);
+  if (rc != DIB_OK) return rc;
   const long long MK = (long long)M * K;
   dim3 ggrid((unsigned)((MK + kGroupThreads - 1) / kGroupThreads), (3 + C + kGroupRows - 1) / kGroupRows, B);
   knn_group_kernel<<<ggrid, kGroupThreads, 0, stream>>>(query, database, features, knn_idx, C, M, N, K, grouped);

@@ -4,6 +4,9 @@
 //   key d2 = ((dx*dx + dy*dy) + dz*dz), float32 without fma, d = point - node; ties -> lower node index; +inf after
 //   every finite key and NaN after +inf, so the K slots always hold K distinct nodes (K <= M).
 #pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
 #include <type_traits>
 
 namespace dib {
@@ -43,5 +46,10 @@ __device__ __forceinline__ bool nearest_k(float x, float y, float z, const float
   }
   if constexpr (kAll) return true; else return bd[K - 1] < __int_as_float(0x7f800000);
 }
+
+// knn_idx [B][M][K] int32: nearest_k of every query [B][3][M] among the database [B][3][N], K <= min(32, N) <= 2048
+// (encoder_ops.cu's knn_search_kernel, launched on `stream`).  knn_group and knn_fusion group by these indices.
+int knn_search_launch(const float* query, const float* database, int B, int M, int N, int K, int32_t* knn_idx,
+                      cudaStream_t stream);
 
 }  // namespace dib

@@ -16,13 +16,14 @@
 //                     arg-max over [0, c_split) and [c_split, C) by torch.max's rule, or (the projection launches)
 //                     transposed as [B][N][C_pad].
 //
-// Operand rounding is defined, not left to the instruction: tf32_rna is round-to-nearest, ties away from zero, onto
-// 10 mantissa bits (cvt.rna.tf32.f32's rule for every finite value that stays finite), written with integer
-// operations so that overflow (-> inf) and NaN (unchanged) are defined too.  Products accumulate in f32 in the tensor
-// core; bias, ReLU (NaN stays NaN) and the arg-max are f32.  oracle_pointwise restates this formulation.
+// Operand rounding is defined, not left to the instruction: tf32_rna (tf32_mma.cuh) is round-to-nearest, ties away
+// from zero, onto 10 mantissa bits, with overflow (-> inf) and NaN (unchanged) defined too.  Products accumulate in
+// f32 in the tensor core; bias, ReLU (NaN stays NaN) and the arg-max are f32.  oracle_pointwise restates this
+// formulation.
 #include <math.h>
 
 #include "common.cuh"
+#include "tf32_mma.cuh"
 
 namespace dib {
 
@@ -51,58 +52,6 @@ struct MlpParams {
   int8_t* pred_a;
   int32_t* pred_b;
 };
-
-__host__ __device__ __forceinline__ uint32_t tf32_rna_bits(uint32_t u) {
-  if ((u & 0x7fffffffu) > 0x7f800000u) return u;                 // NaN
-  return (u + 0x1000u) & 0xffffe000u;
-}
-__device__ __forceinline__ float tf32_rna(float x) { return __uint_as_float(tf32_rna_bits(__float_as_uint(x))); }
-
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const float4& a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(__float_as_uint(a.x)), "r"(__float_as_uint(a.y)), "r"(__float_as_uint(a.z)), "r"(__float_as_uint(a.w)),
-        "r"(b0), "r"(b1));
-}
-
-// acc += W[warp's 64 rows][k tiles kt0 .. kt0 + nkt) . xin[nkt * 8][kMlpStride] over the warp's 32 points.  The next
-// step's A fragments are loaded while the current step's products are issued.
-__device__ __forceinline__ void mlp_mma_block(float (&acc)[4][4][4], const float* __restrict__ xin,
-                                              const float4* __restrict__ Wp, int KT, int MT, int kt0, int nkt,
-                                              int wm, int n_base, int lane) {
-  const int g = lane >> 2, t = lane & 3;
-  float4 a[4], an[4];
-#pragma unroll
-  for (int mt = 0; mt < 4; ++mt) {
-    const int m = wm * 4 + mt;
-    a[mt] = m < MT && nkt > 0 ? __ldg(Wp + ((size_t)m * KT + kt0) * 32 + lane) : make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  for (int kt = 0; kt < nkt; ++kt) {
-#pragma unroll
-    for (int mt = 0; mt < 4; ++mt) {
-      const int m = wm * 4 + mt;
-      an[mt] = m < MT && kt + 1 < nkt ? __ldg(Wp + ((size_t)m * KT + kt0 + kt + 1) * 32 + lane)
-                                      : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    const float* x0 = xin + (kt * 8 + t) * kMlpStride + n_base + g;
-    uint32_t b0[4], b1[4];
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt) {
-      b0[nt] = __float_as_uint(x0[nt * 8]);
-      b1[nt] = __float_as_uint(x0[4 * kMlpStride + nt * 8]);
-    }
-#pragma unroll
-    for (int mt = 0; mt < 4; ++mt) {
-      if (wm * 4 + mt < MT) {
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) mma_tf32(acc[mt][nt], a[mt], b0[nt], b1[nt]);
-      }
-    }
-#pragma unroll
-    for (int mt = 0; mt < 4; ++mt) a[mt] = an[mt];
-  }
-}
 
 // torch.max's order: NaN beats everything, otherwise the larger value; equal values (or two NaN) -> the lower index
 __device__ __forceinline__ bool mlp_better(float v, int i, float bv, int bi) {
@@ -191,11 +140,11 @@ __global__ void __launch_bounds__(kMlpThreads, 2) mlp_kernel(const __grid_consta
           xs[r * kMlpStride + n] = v;
         }
         __syncthreads();
-        mlp_mma_block(acc, xs, Wp, KT, MT, k0 >> 3, kc8 >> 3, wm, n_base, lane);
+        mma_block_64x32<kMlpStride>(acc, xs, Wp, KT, MT, k0 >> 3, kc8 >> 3, wm, n_base, lane);
       }
     } else {
       const int KT = p.layer[l - 1].Cpad >> 3;
-      mlp_mma_block(acc, in, Wp, KT, MT, 0, KT, wm, n_base, lane);
+      mma_block_64x32<kMlpStride>(acc, in, Wp, KT, MT, 0, KT, wm, n_base, lane);
     }
     if (l == 0 && p.n_interp > 0) __syncthreads();             // the gathered tile is complete (and visible)
     float* out = (l & 1) ? bufB : bufA;
@@ -274,8 +223,8 @@ __global__ void mlp_pack_kernel(const float* __restrict__ W, int ld, int C_out, 
                                 MlpPackSeg seg, float* __restrict__ out) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= total) return;
-  const int i = e & 3, lane = (e >> 2) & 31, tile = e >> 7, kt = tile % KT, mt = tile / KT;
-  const int row = mt * 16 + (lane >> 2) + (i & 1) * 8, col = kt * 8 + (lane & 3) + (i >> 1) * 4;
+  int row, col;
+  a_frag_row_col(e, KT, row, col);
   float v = 0.f;
   if (row < C_out && col < K) {
     int s = 0;

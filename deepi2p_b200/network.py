@@ -19,6 +19,7 @@ touches neither CUDA nor the network.
 """
 import math
 import os
+import types
 
 import torch
 import torch.nn as nn
@@ -326,11 +327,22 @@ def fold_pointnet(pointnet, dtype=torch.float32):
     return out
 
 
+def fold_knn_fusion(module, dtype=torch.float32):
+    """The layers of a _KnnFusion as plain affine maps for inference: (before, after), each [(W [C_out,C_in], b
+    [C_out], relu)] folded as fold_pointnet does (eval-mode BatchNorm in float64, rounded once to `dtype`).  The first
+    after layer keeps its 2 C_b input columns, the per-node max first: what point_ops.knn_fusion takes."""
+    return (fold_pointnet(types.SimpleNamespace(layers=module.layers_before), dtype),
+            fold_pointnet(types.SimpleNamespace(layers=module.layers_after), dtype))
+
+
 class FusedInference:
     """Inference through KeypointDetector with its per-point layers fused (DESIGN.md 4.21): first_pointnet,
     second_pointnet and the decoder's two per-point interpolations + concatenation + per_point_pn + predict each run
     as one point_ops.pointwise_mlp call, so no [B,C,N] tensor wider than 64 channels is built.  Everything else (the
-    node-level layers, the kNN module, ResNet) is the model's own code.
+    node-level layers, ResNet, and with the default encoder="torch" the kNN module and final_pointnet) is the model's
+    own code.  encoder="fused" also runs the point encoder's kNN module as one point_ops.knn_fusion call and
+    final_pointnet + the max over the nodes as one point_ops.pointwise_mlp_max call (DESIGN.md 4.26), so no
+    [B,C,Mb,K] tensor and no [B,512,Mb] tensor is built.
 
     The fused layers compute in TF32 whatever torch's TF32 flags say, with BatchNorm folded into the weights, so the
     scores differ from model.forward's at rounding level and a prediction can differ where the top two scores nearly
@@ -341,25 +353,41 @@ class FusedInference:
                ("second", lambda m: m.pc_encoder.second_pointnet, ((32, 0, 0), (32, 0, 0))),
                ("head", lambda m: m.per_point_pn, None))
 
-    def __init__(self, model):
+    ENCODERS = ("torch", "fused")
+
+    def __init__(self, model, encoder="torch"):
         if not isinstance(model, KeypointDetector):
             raise TypeError("FusedInference wraps a network.KeypointDetector")
-        self.model = model
+        if encoder not in self.ENCODERS:
+            raise ValueError(f"encoder must be one of {self.ENCODERS}, got {encoder!r}")
+        self.model, self.encoder = model, encoder
         self._packed, self._stamp = {}, {}
+
+    def _cached(self, name, module, pack):
+        tensors = list(module.parameters()) + list(module.buffers())
+        stamp = tuple((t.data_ptr(), t._version) for t in tensors)
+        if self._stamp.get(name) != stamp:
+            self._packed[name] = pack()
+            self._stamp[name] = stamp
+        return self._packed[name]
 
     def _chain(self, name):
         model = self.model
+        enc = model.pc_encoder
+        if name == "knn":
+            C = enc.knnlayer.layers_before[0].conv.in_channels - 3
+            return self._cached(name, enc.knnlayer,
+                                lambda: point_ops.pack_knn_fusion(C, *fold_knn_fusion(enc.knnlayer)))
+        if name == "final":
+            pn = enc.final_pointnet
+            return self._cached(name, pn, lambda: point_ops.pack_pointwise_mlp_max(pn.layers[0].conv.in_channels,
+                                                                                     fold_pointnet(pn)))
         _, get, spec = next(c for c in self._CHAINS if c[0] == name)
         if spec is None:
             spec = ((128, model.node_a_num, model.k_interp_point_a), (512, model.node_b_num, model.k_interp_point_b),
                     (32, 0, 0), (64, 0, 0))
         pn = get(model)
-        tensors = list(pn.parameters()) + list(pn.buffers())
-        stamp = tuple((t.data_ptr(), t._version) for t in tensors)
-        if self._stamp.get(name) != stamp:
-            self._packed[name] = point_ops.pack_pointwise_mlp(spec, fold_pointnet(pn))
-            self._stamp[name] = stamp
-        return self._packed[name]
+        return self._cached(name, pn, lambda: point_ops.pack_pointwise_mlp(spec, fold_pointnet(pn)))
 
     def classify(self, pc, intensity, sn, node_a, node_b, img, return_scores=False):
         """(pc [B,3,N], intensity [B,1,N], sn [B,3,N], node_a [B,3,Ma], node_b [B,3,Mb], img [B,3,H,W]) float32 CUDA ->
@@ -390,9 +418,14 @@ class FusedInference:
         second_pn_out = point_ops.pointwise_mlp([first_pn_out, scattered], self._chain("second"))
         del scattered
         node_a_features = point_ops.cluster_max_pool(second_pn_out, min_idx, Ma)
-        node_b_features = enc.knnlayer(node_b, ca["cluster_mean"], node_a_features, model.k_ab)
-        final_pn_out = enc.final_pointnet(torch.cat((node_b, node_b_features), dim=1))
-        global_feature = torch.max(final_pn_out, dim=2, keepdim=True)[0]
+        if self.encoder == "fused":
+            node_b_features = point_ops.knn_fusion(node_b, ca["cluster_mean"], node_a_features, model.k_ab,
+                                                   self._chain("knn"))
+            global_feature = point_ops.pointwise_mlp_max([node_b, node_b_features], self._chain("final"))
+        else:
+            node_b_features = enc.knnlayer(node_b, ca["cluster_mean"], node_a_features, model.k_ab)
+            final_pn_out = enc.final_pointnet(torch.cat((node_b, node_b_features), dim=1))
+            global_feature = torch.max(final_pn_out, dim=2, keepdim=True)[0]
 
         s16, s32 = model.img_encoder.backbone(img)
         img_global = s32.mean(dim=(2, 3))
@@ -423,7 +456,7 @@ class FusedInference:
                                        return_scores=return_scores)
 
 
-HEADS = ("torch", "fused")
+HEADS = ("torch", "fused", "fused_encoder")
 
 
 def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chunk=DEFAULT_CHUNK, n_inits=60, seed=0,
@@ -441,7 +474,8 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
     head selects a numeric contract, not a tuning.  "torch" (the default) is model.forward and network.predict: the
     convolutions are cuDNN's and honour torch's TF32 flags.  "fused" is FusedInference.classify per chunk: the
     per-point layers run as fused TF32 tensor-core kernels whatever the flags say, so predictions can differ from
-    "torch" at points whose top two scores nearly tie.
+    "torch" at points whose top two scores nearly tie.  "fused_encoder" is FusedInference(model, encoder="fused")
+    per chunk: the point encoder's kNN module and final_pointnet + max run fused in TF32 too.
 
     Returns dict(P [S,4,4] f64, cost [S] f64, coarse_pred int8 [S,N], fine_pred int32 [S,N] or None, degenerate
     int32 [S]); a sample with no point predicted inside gets P = I, cost 1e4 and degenerate = 1."""
@@ -451,7 +485,8 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
         raise ValueError(f"chunk must be >= 1, got {chunk}")
     if head not in HEADS:
         raise ValueError(f"head must be one of {HEADS}, got {head!r}")
-    fused = FusedInference(model) if head == "fused" else None
+    fused = FusedInference(model, encoder="fused" if head == "fused_encoder" else "torch") if head != "torch" \
+        else None
     for t, name in ((intensity, "intensity"), (sn, "sn"), (node_a, "node_a"), (node_b, "node_b"), (img, "img")):
         if t.shape[0] != S:
             raise ValueError(f"{name} has {t.shape[0]} samples, pc has {S}")
@@ -465,7 +500,7 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
             for a in range(0, S, chunk):
                 b = min(a + chunk, S)
                 args = (pc[a:b], intensity[a:b], sn[a:b], node_a[a:b], node_b[a:b], img[a:b])
-                if head == "fused":
+                if fused is not None:
                     out = None
                     c, f = fused.classify(*args)
                 else:

@@ -743,3 +743,226 @@ def pointwise_mlp(sources, layers, output="activations", c_split=None, return_sc
     if output == "activations":
         return out
     return (pred_a, pred_b, out) if return_scores else (pred_a, pred_b)
+
+
+KNN_FUSION_MAX_WIDTH = 512
+KNN_FUSION_MAX_SIDE = 3
+_mlp_max_ws = {}
+
+
+def _chain_widths(layers, c_in, name, lo=1):
+    """[(C_out, relu)] of lo to 3 layers (W [C_out,C_in], b [C_out] or None, relu), widths in [1, 512]; ValueError
+    otherwise.  The first layer takes c_in rows."""
+    if not isinstance(layers, (list, tuple)) or not lo <= len(layers) <= KNN_FUSION_MAX_SIDE:
+        raise ValueError(f"{name}: need a list of {lo} to {KNN_FUSION_MAX_SIDE} layers")
+    meta = []
+    for i, layer in enumerate(layers):
+        if not isinstance(layer, (list, tuple)) or len(layer) != 3:
+            raise ValueError(f"{name}[{i}]: need (W, b, relu)")
+        W, b, relu = layer
+        if not isinstance(W, torch.Tensor) or W.dim() != 2 or W.shape[1] != c_in:
+            raise ValueError(f"{name}[{i}]: W must be [C_out, {c_in}]")
+        if not 1 <= W.shape[0] <= KNN_FUSION_MAX_WIDTH:
+            raise ValueError(f"{name}[{i}]: need 1 <= C_out <= {KNN_FUSION_MAX_WIDTH}, got {W.shape[0]}")
+        if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (W.shape[0],)):
+            raise ValueError(f"{name}[{i}]: b must be [{W.shape[0]}] or None")
+        c_in = W.shape[0]
+        meta.append((c_in, bool(relu)))
+    return meta
+
+
+class PackedChain:
+    """The layers of one knn_fusion or pointwise_mlp_max chain in the kernel's order on the device (weights rounded
+    to TF32 once), for c_in input rows: meta = [(C_out, relu)] over every layer, n_before of them before the per-node
+    max (all of them for pointwise_mlp_max).  pack_knn_fusion and pack_pointwise_mlp_max build it."""
+
+    def __init__(self, kind, c_in, meta, n_before, packed):
+        self.kind, self.c_in, self.meta, self.n_before, self.packed = kind, c_in, list(meta), n_before, packed
+
+
+def _pack_chain(kind, c_in, layers, meta, n_before):
+    dev = layers[0][0].device
+    keep = []
+    for W, b, _ in layers:
+        for t in (W, b):
+            if t is None:
+                continue
+            if t.requires_grad and torch.is_grad_enabled():
+                raise RuntimeError(f"{kind} has no backward: call it under torch.no_grad() or detach the layers")
+            if not t.is_cuda or t.device != dev or t.dtype != torch.float32:
+                raise RuntimeError("the layers must be float32 CUDA tensors on one device")
+        keep.append((W.detach().contiguous(), None if b is None else b.detach().contiguous()))
+    _, lay = _mlp_tables([], meta)
+    for i, (W, b) in enumerate(keep):
+        lay[i, 0], lay[i, 1] = W.data_ptr(), 0 if b is None else b.data_ptr()
+    lib = _native.load()
+    if kind == "knn_fusion":
+        args = (c_in, lay.ctypes.data, n_before, len(meta) - n_before)
+        need = lib.knn_fusion_packed_bytes(*args)
+    else:
+        args = (c_in, lay.ctypes.data, len(meta))
+        need = lib.pointwise_mlp_max_packed_bytes(*args)
+    if need == 0:
+        raise ValueError(f"{kind}: " + lib.dib_last_error().decode("utf-8", "replace"))
+    with torch.cuda.device(dev):
+        packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
+        stream = torch.cuda.current_stream().cuda_stream
+        if kind == "knn_fusion":
+            rc = lib.knn_fusion_pack_f32(*args, packed.data_ptr(), need, stream)
+        else:
+            rc = lib.pointwise_mlp_max_pack_f32(*args, packed.data_ptr(), need, stream)
+    _native.check(rc, kind + "_pack_f32")
+    del keep
+    return PackedChain(kind, c_in, meta, n_before, packed)
+
+
+def _knn_fusion_meta(C, before, after):
+    if not isinstance(C, int) or not 1 <= C <= KNN_FUSION_MAX_WIDTH - 3:
+        raise ValueError(f"knn_fusion: need 1 <= C <= {KNN_FUSION_MAX_WIDTH - 3} feature channels, got {C}")
+    mb = _chain_widths(before, 3 + C, "before")
+    ma = _chain_widths(after, 2 * mb[-1][0], "after")
+    return mb + ma, len(mb)
+
+
+def pack_knn_fusion(C, before, after):
+    """Pack the folded layers of a kNN fusion module for C feature channels (network.fold_knn_fusion's lists) once;
+    knn_fusion does this itself when given the raw layers."""
+    meta, n_before = _knn_fusion_meta(int(C), before, after)
+    return _pack_chain("knn_fusion", 3 + int(C), list(before) + list(after), meta, n_before)
+
+
+def knn_fusion(query, database, features, K, layers, return_idx=False):
+    """The node kNN module (GeneralKNNFusionModule.forward, layers_pc.py:793-818) in one kernel, for inference
+    (DESIGN.md 4.26): group the K nearest database nodes of each query as knn_group does, the "before" layers, the max
+    over the K neighbours, the "after" layers over the concatenation [max; x], the max over K again.  No [B,C,M,K]
+    tensor is built: the max half of the first after layer is projected once per node and added like a bias.
+
+    query [B,3,M], database [B,3,N], features [B,C,N] float32 CUDA; 1 <= K <= 32, K <= N <= 2048, 3 + C <= 512.
+    layers: (before, after), each a list of 1 to 3 (W [C_out,C_in], b [C_out] or None, relu) with every C_out in
+    [1, 512] (BatchNorm folded: network.fold_knn_fusion), the first after layer taking 2 C_b rows (max first), or a
+    PackedChain from pack_knn_fusion.  Returns out [B,C_out,M], and knn_group's knn_idx [B,M,K] int32 with
+    return_idx=True.
+
+    TF32 tensor-core products with float32 accumulation whatever torch's TF32 flags say: weights, the grouped values
+    and the activations between layers are rounded to TF32 (nearest, ties away from zero); bias, ReLU (NaN stays NaN)
+    and both maxes are float32, a NaN among a node's K columns giving NaN.  No backward: an input that requires grad
+    raises RuntimeError unless grad mode is off.  Shape and bound errors raise ValueError before anything is
+    launched."""
+    for t, name in ((query, "query"), (database, "database"), (features, "features")):
+        if not isinstance(t, torch.Tensor) or t.dim() != 3:
+            raise ValueError(f"{name} must be a 3-D tensor")
+    B, C, N = features.shape
+    M = query.shape[2]
+    if query.shape[:2] != (B, 3) or database.shape != (B, 3, N):
+        raise ValueError("query must be [B,3,M], database [B,3,N] and features [B,C,N]")
+    if isinstance(K, bool) or int(K) != K or not 1 <= K <= KNN_MAX_K:
+        raise ValueError(f"K: need 1 <= K <= {KNN_MAX_K}, got {K}")
+    K = int(K)
+    if not 1 <= N <= KNN_MAX_NODES or K > N:
+        raise ValueError(f"database: need K <= N <= {KNN_MAX_NODES}, got K = {K}, N = {N}")
+    if not 1 <= B <= MLP_MAX_BATCH or M < 1:
+        raise ValueError(f"need 1 <= B <= {MLP_MAX_BATCH} and M >= 1, got B = {B}, M = {M}")
+    if isinstance(layers, PackedChain):
+        if layers.kind != "knn_fusion" or layers.c_in != 3 + C:
+            raise ValueError(f"the layers were packed as {layers.kind} for {layers.c_in} input rows, need 3 + C = "
+                             f"{3 + C}")
+        packed = layers
+        meta, n_before = packed.meta, packed.n_before
+    else:
+        if not isinstance(layers, (list, tuple)) or len(layers) != 2:
+            raise ValueError("layers: need (before, after) or a PackedChain")
+        meta, n_before = _knn_fusion_meta(C, *layers)
+        packed = None
+    for t in (query, database, features):
+        if t.requires_grad and torch.is_grad_enabled():
+            raise RuntimeError("knn_fusion has no backward: call it under torch.no_grad() or detach the inputs")
+        if t.dtype != torch.float32:
+            raise RuntimeError("query, database and features must be float32")
+        if not t.is_cuda or t.device != features.device:
+            raise RuntimeError("query, database and features must be CUDA tensors on one device")
+    dev = features.device
+    query, database, features = query.contiguous(), database.contiguous(), features.contiguous()
+    if packed is None:
+        packed = pack_knn_fusion(C, *layers)
+    if packed.packed.device != dev:
+        raise RuntimeError(f"the layers must be on {dev}")
+    _, lay = _mlp_tables([], meta)
+    lib = _native.load()
+    with torch.cuda.device(dev):
+        idx = torch.empty((B, M, K), dtype=torch.int32, device=dev)
+        out = torch.empty((B, meta[-1][0], M), dtype=torch.float32, device=dev)
+        rc = lib.knn_fusion_f32(query.data_ptr(), database.data_ptr(), features.data_ptr(), B, C, M, N, K,
+                                lay.ctypes.data, n_before, len(meta) - n_before, packed.packed.data_ptr(),
+                                packed.packed.numel() * 4, idx.data_ptr(), out.data_ptr(),
+                                torch.cuda.current_stream().cuda_stream)
+    _native.check(rc, "knn_fusion_f32")
+    return (out, idx) if return_idx else out
+
+
+def pack_pointwise_mlp_max(c_in, layers):
+    """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] for c_in input rows once;
+    pointwise_mlp_max does this itself when given the raw layers."""
+    c_in = int(c_in)
+    if not 1 <= c_in <= KNN_FUSION_MAX_WIDTH:
+        raise ValueError(f"pointwise_mlp_max: need 1 <= input rows <= {KNN_FUSION_MAX_WIDTH}, got {c_in}")
+    return _pack_chain("pointwise_mlp_max", c_in, layers, _chain_widths(layers, c_in, "layers"), len(layers))
+
+
+def pointwise_mlp_max(sources, layers):
+    """A chain of one to three 1x1-convolution layers over the columns of each sample, then the max over all of them,
+    in one kernel and a fixed-order reduction, for inference (DESIGN.md 4.26): final_pointnet + torch.max(dim=2) of
+    the point encoder, with the input concatenation and the [B,C_out,N] activations never built.
+
+    sources: 1 to 4 dense float32 CUDA tensors [B,C,N] (a channel slice of a wider contiguous tensor is read in
+    place), at most 512 rows in all.  layers: [(W [C_out,C_in], b [C_out] or None, relu)], every C_out in [1, 512],
+    or a PackedChain from pack_pointwise_mlp_max.  Returns [B,C_out,1] float32.  pointwise_mlp's TF32 rule; the max
+    is float32 with torch.max's NaN rule.  No backward; shape and bound errors raise ValueError before any launch."""
+    if not isinstance(sources, (list, tuple)) or not all(isinstance(s, torch.Tensor) for s in sources):
+        raise ValueError("sources: need a list of dense [B,C,N] tensors")
+    spec, B, N = _mlp_source_shapes(sources)
+    c_in = sum(c for c, _, _ in spec)
+    if c_in > KNN_FUSION_MAX_WIDTH:
+        raise ValueError(f"the concatenated input has {c_in} rows, more than {KNN_FUSION_MAX_WIDTH}")
+    if isinstance(layers, PackedChain):
+        if layers.kind != "pointwise_mlp_max" or layers.c_in != c_in:
+            raise ValueError(f"the layers were packed as {layers.kind} for {layers.c_in} input rows, got {c_in}")
+        packed, meta = layers, layers.meta
+    else:
+        packed, meta = None, _chain_widths(layers, c_in, "layers")
+    dev = sources[0].device
+    for t in sources:
+        if t.requires_grad and torch.is_grad_enabled():
+            raise RuntimeError("pointwise_mlp_max has no backward: call it under torch.no_grad() or detach the inputs")
+        if not t.is_cuda or t.device != dev:
+            raise RuntimeError(f"pointwise_mlp_max: every source must be a CUDA tensor on {dev}")
+        if t.dtype != torch.float32:
+            raise RuntimeError("pointwise_mlp_max: every source must be float32")
+    src, lay = _mlp_tables(spec, meta)
+    keep = []
+    for i, s in enumerate(sources):
+        C = s.shape[1]
+        if (N > 1 and s.stride(2) != 1) or (C > 1 and s.stride(1) != N) or (B > 1 and s.stride(0) < C * N):
+            s = s.contiguous()
+        keep.append(s)
+        src[i, 0], src[i, 1] = s.data_ptr(), s.stride(0) if B > 1 else C * N
+    if packed is None:
+        packed = pack_pointwise_mlp_max(c_in, layers)
+    if packed.packed.device != dev:
+        raise RuntimeError(f"the layers must be on {dev}")
+    C_out = meta[-1][0]
+    lib = _native.load()
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream().cuda_stream
+        need = lib.pointwise_mlp_max_workspace_bytes(C_out, B, N)
+        key = (dev.index, stream)
+        ws = _mlp_max_ws.get(key)
+        if ws is None or ws.numel() < need:
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            _mlp_max_ws[key] = ws
+        out = torch.empty((B, C_out, 1), dtype=torch.float32, device=dev)
+        rc = lib.pointwise_mlp_max_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.packed.data_ptr(),
+                                       packed.packed.numel() * 4, B, N, out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                       stream)
+    _native.check(rc, "pointwise_mlp_max_f32")
+    del keep
+    return out

@@ -689,6 +689,43 @@ int pointwise_mlp_f32(const int64_t* sources, int n_sources, const int64_t* laye
                       void* workspace, size_t workspace_bytes, dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Fused inference of the point encoder's node kNN module (GeneralKNNFusionModule.forward, models/layers_pc.py:793-818)
+ * and of its global feature (final_pointnet + torch.max over the nodes, models/networks_pc.py:107-115; SURVEY.md 8f
+ * N21).  DESIGN.md 4.26 states the contract.  Inference only, BatchNorm folded into W and b by the caller; layers use
+ * pointwise_mlp's DIB_MLP_LAYER table, every C_out in [1, 512].  The products run on the tensor cores in TF32 with f32
+ * accumulation; weights (once, when packed), staged inputs and the activations fed to the next layer are rounded to
+ * TF32 (nearest, ties away from zero); bias, ReLU (NaN stays NaN) and every max are f32, a NaN in a group giving NaN.
+ * Deterministic: no atomics.  [dev] pointers; 0 <= B <= 65535.
+ *
+ * knn_fusion_*: layers holds n_before (1..3) then n_after (1..3) layers.  Layer 1 takes C_in = 3 + C rows (<= 512);
+ *   the first after layer takes 2 C_b rows, C_b the last before layer's width: columns [0, C_b) multiply the per-node
+ *   max and [C_b, 2 C_b) the columns themselves (torch.cat((max, x), dim=1)).
+ * knn_fusion_pack_f32 writes the layers in the kernel's order into packed ([dev] 16-byte aligned, >=
+ *   knn_fusion_packed_bytes).
+ * knn_fusion_f32: query [B][3][M], database [B][3][N], features [B][C][N] f32 contiguous; 1 <= N <= 2048, 1 <= K <=
+ *   min(32, N).  knn_idx [B][M][K] int32 receives knn_group_forward_f32's indices; out [B][C_out][M] f32 = the max
+ *   over the K neighbours of the after layers over the columns [database[idx] - query; features[idx]] extended by
+ *   the max over the K neighbours of the before layers.
+ * pointwise_mlp_max_*: a chain of 1..3 layers over the concatenation of 1..4 dense sources (pointwise_mlp's
+ *   DIB_MLP_SRC table with NODES = 0, C_in <= 512 rows in all), then the max over the N >= 1 columns of each sample:
+ *   out [B][C_out] f32.  workspace: [dev] 16-byte aligned, >= pointwise_mlp_max_workspace_bytes(C_out, B, N) (the
+ *   per-tile maxes, reduced in ascending tile order).
+ * ------------------------------------------------------------------------------------------ */
+size_t knn_fusion_packed_bytes(int C_in, const int64_t* layers, int n_before, int n_after);
+int knn_fusion_pack_f32(int C_in, const int64_t* layers, int n_before, int n_after, void* packed, size_t packed_bytes,
+                        dib_stream_t stream);
+int knn_fusion_f32(const float* query, const float* database, const float* features, int B, int C, int M, int N,
+                   int K, const int64_t* layers, int n_before, int n_after, const void* packed, size_t packed_bytes,
+                   int32_t* knn_idx, float* out, dib_stream_t stream);
+size_t pointwise_mlp_max_packed_bytes(int C_in, const int64_t* layers, int n_layers);
+int pointwise_mlp_max_pack_f32(int C_in, const int64_t* layers, int n_layers, void* packed, size_t packed_bytes,
+                               dib_stream_t stream);
+size_t pointwise_mlp_max_workspace_bytes(int C_out, int B, int N);
+int pointwise_mlp_max_f32(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers,
+                          const void* packed, size_t packed_bytes, int B, int N, float* out, void* workspace,
+                          size_t workspace_bytes, dib_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Batched PNG decoding (KITTI's official odometry colour frames).  DESIGN.md 4.23 states the contract: 8-bit
  * truecolour, not interlaced, decoded bit for bit as OpenCV 4.13's cv2.imdecode(..., IMREAD_COLOR)[:, :, ::-1]
  * (HWC uint8 RGB).  deepi2p_b200/png.py walks the chunks, checks IHDR / PLTE / IEND and the zlib header, and fills
