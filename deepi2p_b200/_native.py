@@ -44,6 +44,7 @@ EXPORTS = (
     "jpeg_encode_workspace_bytes", "jpeg_encode_entropy_u8", "jpeg_encode_stuff_u8",
     "knn_fusion_packed_bytes", "knn_fusion_pack_f32", "knn_fusion_f32", "pointwise_mlp_max_packed_bytes",
     "pointwise_mlp_max_pack_f32", "pointwise_mlp_max_workspace_bytes", "pointwise_mlp_max_f32",
+    "node_mlp_packed_bytes", "node_mlp_pack_f32", "node_mlp_workspace_bytes", "node_mlp_f32",
 )
 
 
@@ -270,6 +271,14 @@ def load():
     lib.pointwise_mlp_max_workspace_bytes.argtypes = [i32, i32, i32]
     lib.pointwise_mlp_max_f32.restype = i32
     lib.pointwise_mlp_max_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, vp, vp, sz, vp]
+    lib.node_mlp_packed_bytes.restype = sz
+    lib.node_mlp_packed_bytes.argtypes = [vp, i32, vp, i32]
+    lib.node_mlp_pack_f32.restype = i32
+    lib.node_mlp_pack_f32.argtypes = [vp, i32, vp, i32, vp, sz, vp]
+    lib.node_mlp_workspace_bytes.restype = sz
+    lib.node_mlp_workspace_bytes.argtypes = [vp, i32, vp, i32, i32]
+    lib.node_mlp_f32.restype = i32
+    lib.node_mlp_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, vp, vp, sz, vp]
     lib.png_decode_workspace_bytes.restype = sz
     lib.png_decode_workspace_bytes.argtypes = [vp, i32, vp, i32, sz]
     lib.png_decode_batch_u8.restype = i32

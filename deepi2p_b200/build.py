@@ -16,7 +16,7 @@ LIB = os.path.join(LIBDIR, "libdeepi2p_b200.so")
 SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "ball_query_xyz.cu", "cluster_assign.cu",
            "pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu", "classifier_loss.cu",
            "encoder_ops.cu", "fusion.cu", "jpeg.cu", "png.cu", "pointwise_mlp.cu", "oxford_build.cu", "oxford_images.cu",
-           "jpeg_encode.cu", "knn_fusion.cu"]
+           "jpeg_encode.cu", "knn_fusion.cu", "node_mlp.cu"]
 # Compiled on their own without FMA contraction: oracle_pnp/pnp_oracle.cpp, oracle_icp/icp_oracle.cpp and
 # oracle_prep/prep_oracle.cpp, oracle_assemble/, oracle_interp/, oracle_image/ and oracle.pose_diff_restated (metrics.cu)
 # restate their arithmetic bit for bit (oracle_oxford_build/ and oracle_oxford_images/ too); metrics.cu and

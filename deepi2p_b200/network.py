@@ -342,7 +342,10 @@ class FusedInference:
     node-level layers, ResNet, and with the default encoder="torch" the kNN module and final_pointnet) is the model's
     own code.  encoder="fused" also runs the point encoder's kNN module as one point_ops.knn_fusion call and
     final_pointnet + the max over the nodes as one point_ops.pointwise_mlp_max call (DESIGN.md 4.26), so no
-    [B,C,Mb,K] tensor and no [B,512,Mb] tensor is built.
+    [B,C,Mb,K] tensor and no [B,512,Mb] tensor is built.  decoder="fused" runs the decoder's four node-level
+    PointNets (node_b_attention_pn, node_b_pn, node_a_attention_pn, node_a_pn) as one point_ops.node_mlp call each
+    (DESIGN.md 4.27): the per-sample inputs (img_global, global_feature) are projected once per sample instead of
+    being expanded and concatenated.  attention_fusion and the ab interpolation stay the project's exact ops.
 
     The fused layers compute in TF32 whatever torch's TF32 flags say, with BatchNorm folded into the weights, so the
     scores differ from model.forward's at rounding level and a prediction can differ where the top two scores nearly
@@ -354,13 +357,22 @@ class FusedInference:
                ("head", lambda m: m.per_point_pn, None))
 
     ENCODERS = ("torch", "fused")
+    DECODERS = ("torch", "fused")
 
-    def __init__(self, model, encoder="torch"):
+    # node-level PointNets of the decoder: the (channels, per sample) of their input rows, in torch.cat's order
+    _NODE_CHAINS = {"att_b": (lambda m: m.node_b_attention_pn, ((256, False), (512, True))),
+                    "node_b": (lambda m: m.node_b_pn, ((256, False), (512, True), (512, False), (512, True))),
+                    "att_a": (lambda m: m.node_a_attention_pn, ((64, False), (512, True))),
+                    "node_a": (lambda m: m.node_a_pn, ((64, False), (512, False), (256, False)))}
+
+    def __init__(self, model, encoder="torch", decoder="torch"):
         if not isinstance(model, KeypointDetector):
             raise TypeError("FusedInference wraps a network.KeypointDetector")
         if encoder not in self.ENCODERS:
             raise ValueError(f"encoder must be one of {self.ENCODERS}, got {encoder!r}")
-        self.model, self.encoder = model, encoder
+        if decoder not in self.DECODERS:
+            raise ValueError(f"decoder must be one of {self.DECODERS}, got {decoder!r}")
+        self.model, self.encoder, self.decoder = model, encoder, decoder
         self._packed, self._stamp = {}, {}
 
     def _cached(self, name, module, pack):
@@ -382,6 +394,10 @@ class FusedInference:
             pn = enc.final_pointnet
             return self._cached(name, pn, lambda: point_ops.pack_pointwise_mlp_max(pn.layers[0].conv.in_channels,
                                                                                      fold_pointnet(pn)))
+        if name in self._NODE_CHAINS:
+            get, spec = self._NODE_CHAINS[name]
+            pn = get(model)
+            return self._cached(name, pn, lambda: point_ops.pack_node_mlp(spec, fold_pointnet(pn)))
         _, get, spec = next(c for c in self._CHAINS if c[0] == name)
         if spec is None:
             spec = ((128, model.node_a_num, model.k_interp_point_a), (512, model.node_b_num, model.k_interp_point_b),
@@ -435,18 +451,31 @@ class FusedInference:
         img_global_a = img_global.unsqueeze(2).expand(B, C_img, Ma)
         img_global_b = img_global.unsqueeze(2).expand(B, C_img, Mb)
 
-        att_b = model.node_b_attention_pn(torch.cat((node_b_features, img_global_b), dim=1))
-        weighted_s32 = point_ops.attention_fusion(s32, att_b)
-        up_node_b_features = model.node_b_pn(torch.cat((node_b_features, global_feature.expand(B, -1, Mb),
-                                                        weighted_s32, img_global_b), dim=1))
+        if self.decoder == "fused":
+            node = lambda name, sources: point_ops.node_mlp(sources, self._chain(name))
+            g = global_feature[:, :, 0]
+            att_b = node("att_b", [node_b_features, img_global])
+            weighted_s32 = point_ops.attention_fusion(s32, att_b)
+            up_node_b_features = node("node_b", [node_b_features, g, weighted_s32, img_global])
+        else:
+            att_b = model.node_b_attention_pn(torch.cat((node_b_features, img_global_b), dim=1))
+            weighted_s32 = point_ops.attention_fusion(s32, att_b)
+            up_node_b_features = model.node_b_pn(torch.cat((node_b_features, global_feature.expand(B, -1, Mb),
+                                                            weighted_s32, img_global_b), dim=1))
         pb_idx = point_ops.cluster_assign_forward(pc, node_b, k=model.k_interp_point_b,
                                                   want_centers=False)["min_k_idx"]
-        att_a = model.node_a_attention_pn(torch.cat((node_a_features, img_global_a), dim=1))
+        if self.decoder == "fused":
+            att_a = node("att_a", [node_a_features, img_global])
+        else:
+            att_a = model.node_a_attention_pn(torch.cat((node_a_features, img_global_a), dim=1))
         weighted_s16 = point_ops.attention_fusion(s16, att_a)
         ab_idx = point_ops.cluster_assign_forward(node_a, node_b, k=model.k_interp_ab,
                                                   want_centers=False)["min_k_idx"]
         ab = point_ops.upsample_by_interpolation(ab_idx, node_a, node_b, up_node_b_features)
-        up_node_a_features = model.node_a_pn(torch.cat((node_a_features, ab, weighted_s16), dim=1))
+        if self.decoder == "fused":
+            up_node_a_features = node("node_a", [node_a_features, ab, weighted_s16])
+        else:
+            up_node_a_features = model.node_a_pn(torch.cat((node_a_features, ab, weighted_s16), dim=1))
 
         # the decoder's per-point half in one call: rows (pa, pb, first_pn_out, second_pn_out) of per_point_pn's input
         wa, ia = point_ops.interpolation_weights(ca["min_k_idx"], pc, node_a)
@@ -456,7 +485,7 @@ class FusedInference:
                                        return_scores=return_scores)
 
 
-HEADS = ("torch", "fused", "fused_encoder")
+HEADS = ("torch", "fused", "fused_encoder", "fused_all")
 
 
 def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chunk=DEFAULT_CHUNK, n_inits=60, seed=0,
@@ -475,7 +504,9 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
     convolutions are cuDNN's and honour torch's TF32 flags.  "fused" is FusedInference.classify per chunk: the
     per-point layers run as fused TF32 tensor-core kernels whatever the flags say, so predictions can differ from
     "torch" at points whose top two scores nearly tie.  "fused_encoder" is FusedInference(model, encoder="fused")
-    per chunk: the point encoder's kNN module and final_pointnet + max run fused in TF32 too.
+    per chunk: the point encoder's kNN module and final_pointnet + max run fused in TF32 too.  "fused_all" is
+    FusedInference(model, encoder="fused", decoder="fused") per chunk: the decoder's node-level PointNets run fused in
+    TF32 as well, so only ResNet keeps separate convolution / BatchNorm / ReLU kernels.
 
     Returns dict(P [S,4,4] f64, cost [S] f64, coarse_pred int8 [S,N], fine_pred int32 [S,N] or None, degenerate
     int32 [S]); a sample with no point predicted inside gets P = I, cost 1e4 and degenerate = 1."""
@@ -485,8 +516,8 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
         raise ValueError(f"chunk must be >= 1, got {chunk}")
     if head not in HEADS:
         raise ValueError(f"head must be one of {HEADS}, got {head!r}")
-    fused = FusedInference(model, encoder="fused" if head == "fused_encoder" else "torch") if head != "torch" \
-        else None
+    fused = FusedInference(model, encoder="fused" if head in ("fused_encoder", "fused_all") else "torch",
+                           decoder="fused" if head == "fused_all" else "torch") if head != "torch" else None
     for t, name in ((intensity, "intensity"), (sn, "sn"), (node_a, "node_a"), (node_b, "node_b"), (img, "img")):
         if t.shape[0] != S:
             raise ValueError(f"{name} has {t.shape[0]} samples, pc has {S}")

@@ -966,3 +966,187 @@ def pointwise_mlp_max(sources, layers):
     _native.check(rc, "pointwise_mlp_max_f32")
     del keep
     return out
+
+
+NODE_MLP_MAX_WIDTH = 1024         # dense input rows and every layer
+NODE_MLP_MAX_DENSE = 4
+NODE_MLP_MAX_PER_SAMPLE = 65536   # per-sample input rows
+_node_mlp_ws = {}
+
+
+def _node_mlp_source_shapes(sources, M):
+    """[(C, bcast)] per source and (B, M), from shapes alone: a 3-D tensor [B,C,M] is dense, a 2-D tensor [B,C] is
+    the same for every column of its sample; ValueError on a mismatch or a bound."""
+    if not isinstance(sources, (list, tuple)) or not sources or not all(isinstance(s, torch.Tensor) for s in sources):
+        raise ValueError("sources: need a non-empty list of tensors [B,C,M] (dense) or [B,C] (per sample)")
+    spec, B = [], sources[0].shape[0]
+    for i, s in enumerate(sources):
+        if s.dim() not in (2, 3):
+            raise ValueError(f"sources[{i}]: need [B,C,M] (dense) or [B,C] (per sample), got {tuple(s.shape)}")
+        if s.shape[0] != B:
+            raise ValueError(f"sources[{i}] has {s.shape[0]} samples, sources[0] has {B}")
+        if s.shape[1] < 1:
+            raise ValueError(f"sources[{i}]: need at least one channel")
+        if s.dim() == 3:
+            if M is None:
+                M = s.shape[2]
+            elif s.shape[2] != M:
+                raise ValueError(f"sources[{i}] has {s.shape[2]} columns, expected {M}")
+        spec.append((int(s.shape[1]), s.dim() == 2))
+    if M is None:
+        raise ValueError("M: give the number of columns when every source is per sample")
+    _check_node_mlp_rows(spec)
+    if not 1 <= B <= MLP_MAX_BATCH or M < 1:
+        raise ValueError(f"need 1 <= B <= {MLP_MAX_BATCH} and M >= 1, got B = {B}, M = {M}")
+    return spec, B, int(M)
+
+
+def _check_node_mlp_rows(spec):
+    dense = [c for c, bc in spec if not bc]
+    if len(dense) > NODE_MLP_MAX_DENSE:
+        raise ValueError(f"sources: at most {NODE_MLP_MAX_DENSE} dense sources")
+    if sum(dense) > NODE_MLP_MAX_WIDTH:
+        raise ValueError(f"the dense sources have {sum(dense)} rows, more than {NODE_MLP_MAX_WIDTH}")
+    if sum(c for c, bc in spec if bc) > NODE_MLP_MAX_PER_SAMPLE:
+        raise ValueError(f"the per-sample sources have more than {NODE_MLP_MAX_PER_SAMPLE} rows")
+
+
+def _node_mlp_widths(layers, c_in):
+    """[(C_out, relu)] of 1 to 3 layers (W [C_out,C_in], b [C_out] or None, relu), widths in [1, 1024]."""
+    if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= MLP_MAX_LAYERS:
+        raise ValueError(f"layers: need a list of 1 to {MLP_MAX_LAYERS} layers")
+    meta = []
+    for i, layer in enumerate(layers):
+        if not isinstance(layer, (list, tuple)) or len(layer) != 3:
+            raise ValueError(f"layers[{i}]: need (W, b, relu)")
+        W, b, relu = layer
+        if not isinstance(W, torch.Tensor) or W.dim() != 2 or W.shape[1] != c_in:
+            raise ValueError(f"layers[{i}]: W must be [C_out, {c_in}]")
+        if not 1 <= W.shape[0] <= NODE_MLP_MAX_WIDTH:
+            raise ValueError(f"layers[{i}]: need 1 <= C_out <= {NODE_MLP_MAX_WIDTH}, got {W.shape[0]}")
+        if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (W.shape[0],)):
+            raise ValueError(f"layers[{i}]: b must be [{W.shape[0]}] or None")
+        c_in = W.shape[0]
+        meta.append((c_in, bool(relu)))
+    return meta
+
+
+def _node_mlp_tables(spec, meta):
+    import numpy as np
+    src = np.zeros((len(spec), _MLP_SRC), dtype=np.int64)
+    for i, (C, bcast) in enumerate(spec):
+        src[i, 2], src[i, 7] = C, int(bcast)
+    _, lay = _mlp_tables([], meta)
+    return src, lay
+
+
+class PackedNodeMLP:
+    """The layers of one node_mlp chain in the kernel's order on the device (weights rounded to TF32 once, the per-
+    sample sources' columns of W1 split off and transposed), for sources of the widths and kinds `spec` = [(C,
+    per_sample)].  pack_node_mlp builds it."""
+
+    def __init__(self, spec, meta, packed):
+        self.spec, self.meta, self.packed = list(spec), list(meta), packed
+
+
+def pack_node_mlp(spec, layers):
+    """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] (network.fold_pointnet's list) for
+    sources of the widths and kinds `spec` = [(C, per_sample)] in input-row order; node_mlp does this itself when given
+    the raw layers."""
+    spec = [(int(c), bool(bc)) for c, bc in spec]
+    if not spec or any(c < 1 for c, _ in spec):
+        raise ValueError("spec: need a non-empty list of (C >= 1, per_sample)")
+    _check_node_mlp_rows(spec)
+    meta = _node_mlp_widths(layers, sum(c for c, _ in spec))
+    dev = layers[0][0].device
+    keep = []
+    for W, b, _ in layers:
+        for t in (W, b):
+            if t is None:
+                continue
+            if t.requires_grad and torch.is_grad_enabled():
+                raise RuntimeError("node_mlp has no backward: call it under torch.no_grad() or detach the layers")
+            if not t.is_cuda or t.device != dev or t.dtype != torch.float32:
+                raise RuntimeError("the layers must be float32 CUDA tensors on one device")
+        keep.append((W.detach().contiguous(), None if b is None else b.detach().contiguous()))
+    src, lay = _node_mlp_tables(spec, meta)
+    for i, (W, b) in enumerate(keep):
+        lay[i, 0], lay[i, 1] = W.data_ptr(), 0 if b is None else b.data_ptr()
+    lib = _native.load()
+    need = lib.node_mlp_packed_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta))
+    if need == 0:
+        raise ValueError("node_mlp: " + lib.dib_last_error().decode("utf-8", "replace"))
+    with torch.cuda.device(dev):
+        packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
+        rc = lib.node_mlp_pack_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.data_ptr(), need,
+                                   torch.cuda.current_stream().cuda_stream)
+    _native.check(rc, "node_mlp_pack_f32")
+    del keep
+    return PackedNodeMLP(spec, meta, packed)
+
+
+def node_mlp(sources, layers, M=None):
+    """A chain of one to three 1x1-convolution layers y = act(W x + b) over the M columns (nodes) of each sample, in
+    one kernel, for inference (DESIGN.md 4.27): the decoder's node-level PointNets, with BatchNorm already folded into
+    W and b (network.fold_pointnet) and the input concatenation never built.
+
+    sources: in the order of layer 1's input rows, float32 CUDA tensors that are either dense [B,C,M] (at most 4 with
+    at most 1024 rows in all; a channel slice of a wider contiguous tensor is read in place) or per sample [B,C] (any
+    number, at most 65536 rows in all; a [B,C,1] tensor is passed as t[:, :, 0], with no copy).  M is needed only when every source is per sample.
+    layers: [(W [C_out,C_in], b [C_out] or None, relu)] with every C_out in [1, 1024], or a PackedNodeMLP.  Returns
+    the last layer [B,C_out,M] float32.
+
+    The dense rows' products run on the tensor cores in TF32 with float32 accumulation whatever torch's TF32 flags
+    say.  A per-sample source's block of W1 is applied once per sample and output row, as a float32 fma chain in
+    ascending input row, and added to every column before the bias.  Weights, source values and the activations
+    between layers are rounded to TF32 (nearest, ties away from zero); bias and ReLU (NaN stays NaN) are float32.  No
+    backward: an input that requires grad raises RuntimeError unless grad mode is off.  Shape and bound errors raise
+    ValueError before anything is launched."""
+    spec, B, M = _node_mlp_source_shapes(sources, M)
+    if isinstance(layers, PackedNodeMLP):
+        if layers.spec != spec:
+            raise ValueError(f"the layers were packed for sources {layers.spec}, got {spec}")
+        packed, meta = layers, layers.meta
+    else:
+        packed, meta = None, _node_mlp_widths(layers, sum(c for c, _ in spec))
+    dev = sources[0].device
+    for t in sources:
+        if t.requires_grad and torch.is_grad_enabled():
+            raise RuntimeError("node_mlp has no backward: call it under torch.no_grad() or detach the inputs")
+        if not t.is_cuda or t.device != dev:
+            raise RuntimeError(f"node_mlp: every source must be a CUDA tensor on {dev}")
+        if t.dtype != torch.float32:
+            raise RuntimeError("node_mlp: every source must be float32")
+    src, lay = _node_mlp_tables(spec, meta)
+    keep = []
+    for i, s in enumerate(sources):
+        C = s.shape[1]
+        if s.dim() == 3:
+            if (M > 1 and s.stride(2) != 1) or (C > 1 and s.stride(1) != M) or (B > 1 and s.stride(0) < C * M):
+                s = s.contiguous()
+        elif (C > 1 and s.stride(1) != 1) or (B > 1 and s.stride(0) < C):
+            s = s.contiguous()
+        keep.append(s)
+        src[i, 0], src[i, 1] = s.data_ptr(), s.stride(0) if B > 1 else C * (M if s.dim() == 3 else 1)
+    if packed is None:
+        packed = pack_node_mlp(spec, layers)
+    if packed.packed.device != dev:
+        raise RuntimeError(f"the layers must be on {dev}")
+    lib = _native.load()
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream().cuda_stream
+        need = lib.node_mlp_workspace_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), B)
+        ws = None
+        if need:
+            key = (dev.index, stream)
+            ws = _node_mlp_ws.get(key)
+            if ws is None or ws.numel() < need:
+                ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                _node_mlp_ws[key] = ws
+        out = torch.empty((B, meta[-1][0], M), dtype=torch.float32, device=dev)
+        rc = lib.node_mlp_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.packed.data_ptr(),
+                              packed.packed.numel() * 4, B, M, out.data_ptr(),
+                              ws.data_ptr() if ws is not None else None, ws.numel() if ws is not None else 0, stream)
+    _native.check(rc, "node_mlp_f32")
+    del keep
+    return out

@@ -674,6 +674,7 @@ int jpeg_decode_batch_u8(const uint8_t* data, size_t data_bytes, const int64_t* 
 #define DIB_MLP_SRC_W 4
 #define DIB_MLP_SRC_IDX 5
 #define DIB_MLP_SRC_K 6
+#define DIB_MLP_SRC_BCAST 7
 #define DIB_MLP_LAYER 4
 #define DIB_MLP_LAYER_W 0
 #define DIB_MLP_LAYER_B 1
@@ -724,6 +725,35 @@ size_t pointwise_mlp_max_workspace_bytes(int C_out, int B, int N);
 int pointwise_mlp_max_f32(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers,
                           const void* packed, size_t packed_bytes, int B, int N, float* out, void* workspace,
                           size_t workspace_bytes, dib_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Fused inference of the decoder's node-level PointNets (node_b_attention_pn, node_b_pn, node_a_attention_pn and
+ * node_a_pn of models/networks_united.py:147-189; SURVEY.md 8f N22).  DESIGN.md 4.27 states the contract.  A chain of
+ * 1..3 layers y = act(W x + b) over the M columns of each of B samples, inference only, BatchNorm folded into W and b
+ * by the caller; every C_out in [1, 1024].  Layer 1's input rows are the concatenation, in order, of the sources
+ * (pointwise_mlp's DIB_MLP_SRC table, NODES = 0), which is never written to memory:
+ *   dense source (BCAST = 0, at most 4 with at most 1024 rows in all): DATA f32, element (b, c, m) at b * BSTRIDE + c * M + m (BSTRIDE >=
+ *     CHANNELS * M, so a channel slice of a wider tensor passes the wider tensor's batch stride).
+ *   broadcast source (BCAST = 1, any number with at most 65536 rows in all): DATA f32 [B][C] (or [B][C][1]), element (b, c) at b * BSTRIDE + c
+ *     (BSTRIDE >= CHANNELS), the same for every column of sample b.
+ * The dense rows' block of W1 runs on the tensor cores in TF32 with f32 accumulation.  The broadcast rows' block is
+ * applied once per (sample, output row) as an f32 fma chain in ascending input row (TF32 weights times TF32 values,
+ * each product exact in f32) and added to every column of the sample before the bias.  Weights (once, when packed),
+ * source values and the activations fed to the next layer are rounded to TF32 (nearest, ties away from zero); bias and
+ * ReLU (NaN stays NaN) are f32.  Deterministic: no atomics.  [dev] pointers; 0 <= B <= 65535, M >= 0.
+ *
+ * node_mlp_pack_f32 writes the layers in the kernel's order into packed ([dev] 16-byte aligned, >=
+ *   node_mlp_packed_bytes); it depends on the sources' CHANNELS and BCAST only.
+ * node_mlp_f32: out [B][C_out][M] f32, the last layer.  workspace: [dev] 16-byte aligned, >= node_mlp_workspace_bytes
+ *   (the per-sample projections, [B][C1 rounded up to 16]; 0 bytes, and may be NULL, without broadcast sources).
+ * ------------------------------------------------------------------------------------------ */
+size_t node_mlp_packed_bytes(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers);
+int node_mlp_pack_f32(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, void* packed,
+                      size_t packed_bytes, dib_stream_t stream);
+size_t node_mlp_workspace_bytes(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, int B);
+int node_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, const void* packed,
+                 size_t packed_bytes, int B, int M, float* out, void* workspace, size_t workspace_bytes,
+                 dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Batched PNG decoding (KITTI's official odometry colour frames).  DESIGN.md 4.23 states the contract: 8-bit

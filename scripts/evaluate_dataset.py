@@ -4,7 +4,7 @@ frustum.pose_error_batch, with registration_result_analysis.py's summary line an
 P_pred_all_np.npy / P_gt_all_np.npy / cost_all_np.npy.
 
     python scripts/evaluate_dataset.py --dataset {kitti,oxford,nuscenes} --root R --checkpoint C
-        [--head torch|fused|fused_encoder] [--every k] [--batch B] [--seed S] [--inits I] [--version v1.0-trainval] [--out DIR]
+        [--head torch|fused|fused_encoder|fused_all] [--every k] [--batch B] [--seed S] [--inits I] [--version v1.0-trainval] [--out DIR]
 
 The checkpoint is what the reference's training saved (network.load_checkpoint).  Every k-th entry of the val list is
 taken (registration_lsq.py uses 30).  The per-sample draws (image pairing, Pr) come from numpy Generators seeded by
