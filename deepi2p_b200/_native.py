@@ -45,6 +45,7 @@ EXPORTS = (
     "knn_fusion_packed_bytes", "knn_fusion_pack_f32", "knn_fusion_f32", "pointwise_mlp_max_packed_bytes",
     "pointwise_mlp_max_pack_f32", "pointwise_mlp_max_workspace_bytes", "pointwise_mlp_max_f32",
     "node_mlp_packed_bytes", "node_mlp_pack_f32", "node_mlp_workspace_bytes", "node_mlp_f32",
+    "nuscenes_walk_count", "nuscenes_walk_scan_workspace_bytes", "nuscenes_walk_scan", "nuscenes_walk_fill",
 )
 
 
@@ -304,6 +305,14 @@ def load():
     lib.jpeg_encode_entropy_u8.argtypes = [vp, sz, vp, i32, vp, vp, vp, vp, sz, vp]
     lib.jpeg_encode_stuff_u8.restype = i32
     lib.jpeg_encode_stuff_u8.argtypes = [vp, i32, vp, vp, sz, vp, sz, vp]
+    lib.nuscenes_walk_count.restype = i32
+    lib.nuscenes_walk_count.argtypes = [vp, vp, vp, i64, vp, vp, i32, f64, vp, vp, vp]
+    lib.nuscenes_walk_scan_workspace_bytes.restype = sz
+    lib.nuscenes_walk_scan_workspace_bytes.argtypes = [i32]
+    lib.nuscenes_walk_scan.restype = i32
+    lib.nuscenes_walk_scan.argtypes = [vp, i32, vp, vp, sz, vp]
+    lib.nuscenes_walk_fill.restype = i32
+    lib.nuscenes_walk_fill.argtypes = [vp, vp, vp, i64, vp, vp, i32, f64, vp, vp, vp]
     _lib = lib
     return lib
 

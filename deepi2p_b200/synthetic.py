@@ -342,6 +342,128 @@ def write_nuscenes_dataroot(root, chains, seed=0, jpeg=None, version="v1.0-mini"
     return items
 
 
+NUSCENES_RAW_RATES = (("LIDAR_TOP", "lidar", 20.0),) + tuple((c, "camera", 12.0) for c in NUSCENES_CAMERAS) + (
+    ("RADAR_FRONT", "radar", 13.0),)
+NUSCENES_NIGHT_TOKEN = "e59a4d0cc6a84ed59f78fb21a45cdcb4"     # the first of make_datasets.py's test_night_scene_tokens
+NUSCENES_TIE_XY = (1000.0, 500.0)          # the tie scene's LIDAR_TOP position; its ties lie 10 m from it
+
+
+def _track(rng, times):
+    """Along-track distance at `times` for piecewise-constant speeds: stops (0 m/s, one segment in five), driving
+    (1-12 m/s) and reversing (-3 to -1 m/s), each 0.5-3 s long."""
+    edges, speeds = [0.0], []
+    while edges[-1] <= times[-1]:
+        edges.append(edges[-1] + float(rng.uniform(0.5, 3.0)))
+        u = rng.uniform()
+        speeds.append(0.0 if u < 0.2 else -float(rng.uniform(1.0, 3.0)) if u < 0.3 else float(rng.uniform(1.0, 12.0)))
+    edges, speeds = np.array(edges), np.array(speeds)
+    at_edge = np.concatenate([[0.0], np.cumsum(np.diff(edges) * speeds)])
+    k = np.searchsorted(edges, times, side="right") - 1
+    return at_edge[k] + speeds[k] * (times - edges[k])
+
+
+def write_nuscenes_raw(root, n_scenes=8, seed=0, version="v1.0-mini", seconds=(3.0, 8.0), special=True,
+                       all_night=False, jpeg=None, n_rings=4, n_azimuth=64, max_translation=10.0):
+    """A seeded raw devkit-layout root: <root>/<version>/{scene, sample, sample_data, sensor, calibrated_sensor,
+    ego_pose}.json.  LIDAR_TOP at 20 Hz, six cameras at 12 Hz and RADAR_FRONT at 13 Hz, each record with its own ego
+    pose; key frames at 2 Hz, the record of each channel nearest a sample's time.  Scenes last `seconds` (a range) and
+    drive at global positions 300-2000 m from the origin with stops and reversals.  With `special`, the first five
+    scenes are instead: a tie scene (identity rotations; camera translations whose t_lc is exactly (max_translation,
+    0, 0), (-max_translation, 0, 0) or (0, max_translation, 0), or one float32 ulp either side of it), a one-sweep
+    scene, a night scene, a day scene with a hard-coded night token and a scene whose camera chains end at the first
+    neighbour.  all_night marks every scene's description as night.  With jpeg (bytes), every LIDAR_TOP record gets a
+    make_nuscenes_sweep file and every camera record the JPEG, so the root feeds nuscenes.nuscenes_batch.  Returns
+    dict(tie_scene, tie_lanes: the (camera, chain position) of each planted exact tie)."""
+    import json
+    rng = np.random.default_rng(seed + 0x4E5D)
+    tabs = {k: [] for k in ("scene", "sample", "sample_data", "sensor", "calibrated_sensor", "ego_pose")}
+    for k, (ch, mod, _) in enumerate(NUSCENES_RAW_RATES):
+        tabs["sensor"].append(dict(token=f"sensor-{ch}", channel=ch, modality=mod))
+        cam = mod == "camera"
+        yaw = [0.0, 0.95, -0.95, math.pi, 1.9, -1.9][k - 1] if cam else 0.0
+        tabs["calibrated_sensor"].append(dict(
+            token=f"calib-{ch}", sensor_token=f"sensor-{ch}", translation=[1.7 if cam else 0.94, 0.1 * k, 1.5],
+            rotation=_quaternion(rng, yaw - math.pi / 2 if cam else -math.pi / 2),
+            camera_intrinsic=[[1266.4, 0.0, 816.3 + k], [0.0, 1266.4, 491.5], [0.0, 0.0, 1.0]] if cam else []))
+    f32 = lambda v: float(np.float32(v))
+    ulp = lambda v, d: float(np.nextafter(np.float32(v), np.float32(d)))
+    m = float(max_translation)
+    Lx, Ly = NUSCENES_TIE_XY
+    # tie scene, camera chain positions 2.. : (camera, position) -> (x, y) relative offsets from the lidar
+    ties = {("CAM_FRONT", 2): (Lx + m, Ly), ("CAM_FRONT_RIGHT", 2): (Lx - m, Ly), ("CAM_BACK", 2): (Lx, Ly + m),
+            ("CAM_BACK_LEFT", 3): (Lx + m, Ly)}
+    near = {("CAM_FRONT_LEFT", 2): (ulp(Lx + m, 0), Ly), ("CAM_FRONT_LEFT", 3): (ulp(Lx + m, 4096), Ly),
+            ("CAM_BACK_LEFT", 2): (Lx + m - 1.0, Ly), ("CAM_BACK_RIGHT", 2): (ulp(Lx + m, 4096), Ly)}
+    info = dict(tie_scene=None, tie_lanes=sorted(ties))
+    for c in range(n_scenes):
+        kind = ("tie", "one", "night", "token", "short")[c] if special and c < 5 else "drive"
+        T = dict(tie=1.2, one=0.04, short=0.1).get(kind, float(rng.uniform(*seconds)))
+        token = NUSCENES_NIGHT_TOKEN if kind == "token" else f"scene-{seed}-{c:04d}"
+        night = all_night or kind == "night"
+        desc = ["Night, rain, parked cars", "night driving"][c % 2] if night else ["Day, busy street", "Turn left"][c % 2]
+        if kind == "tie":
+            info["tie_scene"] = token
+        ns = max(1, int(math.ceil(T / 0.5 - 1e-9)))
+        s_tok = [f"sample-{seed}-{c}-{j}" for j in range(ns)]
+        for j in range(ns):
+            tabs["sample"].append(dict(token=s_tok[j], timestamp=int(1.5e15 + c * 1e8 + j * 5e5), scene_token=token,
+                                       prev=s_tok[j - 1] if j else "", next=s_tok[j + 1] if j + 1 < ns else ""))
+        tabs["scene"].append(dict(token=token, log_token=f"log-{c}", nbr_samples=ns, first_sample_token=s_tok[0],
+                                  last_sample_token=s_tok[-1], name=f"scene-{c:04d}", description=desc))
+        r0 = rng.uniform(300.0, 2000.0)
+        phi, heading = rng.uniform(-math.pi, math.pi, 2)
+        x0, y0 = r0 * math.cos(phi), r0 * math.sin(phi)
+        grid = np.arange(0.0, T + 1.0, 0.01)
+        s_grid = _track(rng, grid)
+        for k, (ch, mod, hz) in enumerate(NUSCENES_RAW_RATES):
+            off = 0.0 if k == 0 else 0.007 * k
+            times = off + np.arange(int(math.floor((T - off) * hz)) + 1) / hz if T > off else np.array([off])
+            n = len(times)
+            s = np.interp(times, grid, s_grid)
+            wob = 0.5 * np.sin(0.1 * s)
+            xs = x0 + s * math.cos(heading) - wob * math.sin(heading)
+            ys = y0 + s * math.sin(heading) + wob * math.cos(heading)
+            zs = 0.01 * np.sin(times)
+            keys = {int(np.argmin(np.abs(times - 0.5 * j))): j for j in range(ns)}
+            near_s = np.minimum(np.rint(times / 0.5).astype(int), ns - 1)
+            toks = [f"sd-{seed}-{c}-{ch}-{i}" for i in range(n)]
+            for i in range(n):
+                key = i in keys
+                if ch == "LIDAR_TOP":
+                    fn = f"{'samples' if key else 'sweeps'}/{ch}/s{c}_{i:04d}.pcd.bin"
+                else:
+                    fn = f"{'samples' if key else 'sweeps'}/{ch}/s{c}_{i:04d}.{'jpg' if mod == 'camera' else 'pcd'}"
+                if kind == "tie":
+                    rot = [1.0, 0.0, 0.0, 0.0]
+                    x, y = (Lx, Ly) if ch == "LIDAR_TOP" or mod != "camera" else ties.get(
+                        (ch, i), near.get((ch, i), (Lx + 0.25 * i, Ly + 0.5)))
+                    t = [f32(x), f32(y), 1.5]
+                else:
+                    rot = _quaternion(rng, heading + 0.001 * float(s[i]), tilt=0.005)
+                    t = [float(xs[i]), float(ys[i]), float(zs[i])]
+                ego_tok = f"ego-{seed}-{c}-{ch}-{i}"
+                tabs["ego_pose"].append(dict(token=ego_tok, timestamp=int(1.5e15 + c * 1e8 + times[i] * 1e6),
+                                             rotation=rot, translation=t))
+                tabs["sample_data"].append(dict(
+                    token=toks[i], sample_token=s_tok[keys[i]] if key else s_tok[near_s[i]], ego_pose_token=ego_tok,
+                    calibrated_sensor_token=f"calib-{ch}", timestamp=int(1.5e15 + c * 1e8 + times[i] * 1e6),
+                    fileformat=fn.rsplit(".", 1)[1], is_key_frame=key, height=900 if mod == "camera" else 0,
+                    width=1600 if mod == "camera" else 0, filename=fn,
+                    prev=toks[i - 1] if i else "", next=toks[i + 1] if i + 1 < n else ""))
+                if jpeg is not None and ch == "LIDAR_TOP":
+                    os.makedirs(os.path.join(root, os.path.dirname(fn)), exist_ok=True)
+                    make_nuscenes_sweep(seed * 65536 + c * 1024 + i, n_rings, n_azimuth).tofile(os.path.join(root, fn))
+                elif jpeg is not None and mod == "camera":
+                    os.makedirs(os.path.join(root, os.path.dirname(fn)), exist_ok=True)
+                    with open(os.path.join(root, fn), "wb") as f:
+                        f.write(jpeg)
+    os.makedirs(os.path.join(root, version), exist_ok=True)
+    for name, recs in tabs.items():
+        with open(os.path.join(root, version, name + ".json"), "w") as f:
+            json.dump(recs, f)
+    return info
+
+
 def write_icp_handoff(data_dir, monodepth_dir, seeds, shape="oxford"):
     """make_icp_frame frames as a hand-off directory (<id>_pc_label.npy / _K.npy / _P.npy, labels = the GT inside
     mask) plus the <monodepth_dir>/<id>_pc.npy depth clouds registration_icp.py:204 reads.  Returns the frames by id."""

@@ -877,6 +877,36 @@ int jpeg_encode_entropy_u8(const uint8_t* rgb, size_t rgb_bytes, const int64_t* 
 int jpeg_encode_stuff_u8(const int64_t* desc, int S, const int64_t* out_off, uint8_t* out, size_t out_bytes,
                          void* workspace, size_t workspace_bytes, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * nuScenes dataset list (data/nuscenes/make_datasets.py: search_nearby_cameras), the camera walks of E kept LIDAR_TOP
+ * sweeps per call.  DESIGN.md 4.28 states the contract; deepi2p_b200/nuscenes_build.py reads the tables, resumes
+ * the deferred walks with numpy and assembles the list.  All pointers [dev].
+ *
+ * Walk w = 2 (6 e + c) + d of W = 12 E: entry e, camera c, d = 0 along next, 1 along prev.  next, prev [n_sd] i32
+ *   sample_data links (-1: none), trans [n_sd][3] f32 the ego translation of each record, own [E][6] i32 the entry's
+ *   key-frame record of each camera, inv_rows [E][12] f64 rows 0-2 of inv(P_l), row-major.  From own, a walk steps to
+ *   the first neighbour without testing it, then tests each further record r: t = rows 0-2 of inv (trans[r], 1) and
+ *   N = |t| in fp64; r is appended while N < max_translation.  A step with |N - max_translation| within
+ *   4 gamma_4 (sum |inv_ij p_j| + N), or a non-finite N, ends the walk undecided (DIB_NSW_DEFERRED).
+ * nuscenes_walk_count: counts [W] i32 the records appended, status [W] i32 one of DIB_NSW_*.
+ * nuscenes_walk_scan: offsets [W + 1] i64, the exclusive scan of counts and the total; workspace >=
+ *   nuscenes_walk_scan_workspace_bytes(W), 8-byte aligned.
+ * nuscenes_walk_fill: the same walks; tokens [offsets[W]] i32 receives walk w's records at offsets[w].
+ * ------------------------------------------------------------------------------------------ */
+#define DIB_NSW_DONE 0        /* the chain ended or a record failed the radius test                          */
+#define DIB_NSW_DEFERRED 1    /* stopped undecided at step counts[w]; the host decides it with numpy          */
+#define DIB_NSW_BAD_LINK 2    /* own or a link outside [-1, n_sd)                                             */
+#define DIB_NSW_CYCLE 3       /* more than n_sd steps                                                         */
+int nuscenes_walk_count(const int32_t* next, const int32_t* prev, const float* trans, int64_t n_sd,
+                        const int32_t* own, const double* inv_rows, int E, double max_translation, int32_t* counts,
+                        int32_t* status, dib_stream_t stream);
+size_t nuscenes_walk_scan_workspace_bytes(int W);
+int nuscenes_walk_scan(const int32_t* counts, int W, int64_t* offsets, void* workspace, size_t workspace_bytes,
+                       dib_stream_t stream);
+int nuscenes_walk_fill(const int32_t* next, const int32_t* prev, const float* trans, int64_t n_sd,
+                       const int32_t* own, const double* inv_rows, int E, double max_translation,
+                       const int64_t* offsets, int32_t* tokens, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
