@@ -46,6 +46,7 @@ EXPORTS = (
     "pointwise_mlp_max_pack_f32", "pointwise_mlp_max_workspace_bytes", "pointwise_mlp_max_f32",
     "node_mlp_packed_bytes", "node_mlp_pack_f32", "node_mlp_workspace_bytes", "node_mlp_f32",
     "nuscenes_walk_count", "nuscenes_walk_scan_workspace_bytes", "nuscenes_walk_scan", "nuscenes_walk_fill",
+    "kitti_build_count_workspace_bytes", "kitti_build_count_f32", "kitti_build_scatter_f64", "kitti_build_finish_f32",
 )
 
 
@@ -313,6 +314,14 @@ def load():
     lib.nuscenes_walk_scan.argtypes = [vp, i32, vp, vp, sz, vp]
     lib.nuscenes_walk_fill.restype = i32
     lib.nuscenes_walk_fill.argtypes = [vp, vp, vp, i64, vp, vp, i32, f64, vp, vp, vp]
+    lib.kitti_build_count_workspace_bytes.restype = sz
+    lib.kitti_build_count_workspace_bytes.argtypes = [i32]
+    lib.kitti_build_count_f32.restype = i32
+    lib.kitti_build_count_f32.argtypes = [vp, i64, vp, vp, i32, vp, i32, vp, vp, vp, vp, vp, sz, vp]
+    lib.kitti_build_scatter_f64.restype = i32
+    lib.kitti_build_scatter_f64.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, vp]
+    lib.kitti_build_finish_f32.restype = i32
+    lib.kitti_build_finish_f32.argtypes = [vp, vp, vp, vp, i32, f64, i64, i64, vp, vp, vp]
     _lib = lib
     return lib
 

@@ -38,12 +38,18 @@ def pose_path(root, seq, i):
     return os.path.join(root, "poses", "%02d" % seq, "%06d.npz" % i)
 
 
-def record_dir(root, seq):
-    return os.path.join(root, "data_odometry_velodyne_NWU", "sequences", "%02d" % seq, RECORD_DIR)
+def _record_folder(root, seq, name):
+    return os.path.join(root, "data_odometry_velodyne_NWU", "sequences", "%02d" % seq, name)
 
 
-def record_path(root, seq, i):
-    return os.path.join(record_dir(root, seq), "%06d.npy" % i)
+def record_dir(root, seq, record_dir=RECORD_DIR):
+    """The sequence's folder of scan records named `record_dir`: the prepared scans (voxel0.1-SNr0.6) by default, or
+    e.g. the accumulated frames kitti_build writes (stride4-acc50-voxel0.4)."""
+    return _record_folder(root, seq, record_dir)
+
+
+def record_path(root, seq, i, record_dir=RECORD_DIR):
+    return os.path.join(_record_folder(root, seq, record_dir), "%06d.npy" % i)
 
 
 def image_dirs(root, seq, key):
@@ -164,11 +170,13 @@ def accumulation_walk(i, n, frame_num=ACCUMULATION_FRAME_NUM, skip=ACCUMULATION_
 
 class KittiDataset:
     """A KITTI root in the loader's layout: the entry list of `mode` (make_dataset), and the calibration and poses
-    (float32, as the loader reads them), read once and kept."""
+    (float32, as the loader reads them), read once and kept.  record_dir names the folder of scan records the batches
+    read (the loader's np_folder)."""
 
-    def __init__(self, root, mode, seqs=None):
+    def __init__(self, root, mode, seqs=None, record_dir=RECORD_DIR):
         self.root = root
         self.mode = mode
+        self.record_dir = record_dir
         self.entries = make_dataset(root, mode, seqs)
         self._calib, self._poses, self._inverses = {}, {}, {}
 
@@ -258,40 +266,42 @@ def plan_batch(dataset, items, mode, rng, translation_max=TRANSLATION_MAX, delta
     return out
 
 
-def scan_store(root, seqs, location="cuda", device=None):
+def scan_store(root, seqs, location="cuda", device=None, record_dir=RECORD_DIR):
     """A long-lived ScanStore of whole sequences (every record of each sequence's record folder, keyed (seq, frame)).
     Opt-in: KITTI sequences 0-8 take tens of GB (DESIGN.md 4.22); store_nbytes gives the size without loading."""
     recs, keys = [], []
     for seq in seqs:
-        for name, path in _record_files(root, seq):
+        for name, path in _record_files(root, seq, record_dir):
             recs.append(np.load(path, mmap_mode="r"))
             keys.append((int(seq), int(name[:6])))
     for (seq, i), r in zip(keys, recs):
         if r.ndim != 2 or r.shape[0] != 7:
-            raise ValueError(f"{record_path(root, seq, i)}: a KITTI scan record is [7, n] (got {r.shape})")
+            raise ValueError(f"{record_path(root, seq, i, record_dir)}: a KITTI scan record is [7, n] (got {r.shape})")
     return assemble.ScanStore(recs, location, keys=keys, device=device)
 
 
-def _record_files(root, seq):
-    d = _require(record_dir(root, seq), "scan record folder")
+def _record_files(root, seq, record_dir=RECORD_DIR):
+    d = _require(_record_folder(root, seq, record_dir), "scan record folder")
     names = sorted(f for f in os.listdir(d) if f.endswith(".npy"))
     if not names:
         raise ValueError(f"KITTI sequence {seq:02d} is empty: no scan record in {d}")
     return [(f, os.path.join(d, f)) for f in names]
 
 
-def store_nbytes(root, seqs):
+def store_nbytes(root, seqs, record_dir=RECORD_DIR):
     """The bytes a scan_store of `seqs` would take (28 per point: 7 float32 planes), from the .npy headers only."""
-    return sum(28 * int(np.load(p, mmap_mode="r").shape[1]) for seq in seqs for _, p in _record_files(root, seq))
+    return sum(28 * int(np.load(p, mmap_mode="r").shape[1]) for seq in seqs
+               for _, p in _record_files(root, seq, record_dir))
 
 
 def kitti_batch(root, items, mode, seed, rng=None, store=None, input_pt_num=assemble.INPUT_PT_NUM,
                 node_a_num=assemble.NODE_NUM, node_b_num=assemble.NODE_NUM, translation_max=TRANSLATION_MAX,
-                delta_ij_max=DELTA_IJ_MAX, device="cuda", stream=None):
+                delta_ij_max=DELTA_IJ_MAX, device="cuda", stream=None, record_dir=None):
     """KittiLoader.__getitem__ for S = len(items) entries of a KittiDataset (or of KittiDataset(root, mode) when root
     is a path).  j is drawn per item from rng (a numpy Generator or a seed), which then draws Pr and the image crop and
     jitter; seed keys the device's Philox draws.  The scan records come from `store` (a ScanStore keyed (seq, frame),
-    e.g. scan_store) or, without one, from a per-batch store of the batch's distinct records.  The image is frame j's.
+    e.g. scan_store) or, without one, from a per-batch store of the batch's distinct records, read from the folder
+    `record_dir` (None: the dataset's, by default voxel0.1-SNr0.6).  The image is frame j's.
     Returns (pc [S,3,N], intensity [S,1,N], sn [S,3,N], node_a [S,3,Ma], node_b [S,3,Mb], P [S,3,4],
     img [S,3,160,512] float32 on the device; K [S,3,3], t_ji [S,3] float32 on the host)."""
     ds = root if isinstance(root, KittiDataset) else KittiDataset(root, mode)
@@ -307,7 +317,8 @@ def kitti_batch(root, items, mode, seed, rng=None, store=None, input_pt_num=asse
         frames = assemble.store_frames(store, [store.index(k) for k in keys], fs, FT)
     else:
         uniq, ids = assemble.unique_records(keys)
-        recs = [read_record(record_path(ds.root, seq, i)) for seq, i in uniq]
+        folder = ds.record_dir if record_dir is None else record_dir
+        recs = [read_record(record_path(ds.root, seq, i, folder)) for seq, i in uniq]
         frames = assemble.batch_frames(recs, ids, fs, FT, device, stream)
     Pc = np.stack([p["Pc"] for p in plan])
     Pji = np.stack([p["Pji"] for p in plan])

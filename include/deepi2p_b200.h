@@ -907,6 +907,39 @@ int nuscenes_walk_fill(const int32_t* next, const int32_t* prev, const float* tr
                        const int32_t* own, const double* inv_rows, int E, double max_translation,
                        const int64_t* offsets, int32_t* tokens, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * KITTI accumulated-frame records (data/kitti/frame_accumulation.py accumulate_sequence), B output frames per call
+ * from a ragged [7][plane_stride] float32 scan store (assemble.ScanStore: xyz, intensity, normals).  DESIGN.md 4.29
+ * states the contract; deepi2p_b200/kitti_build.py plans the windows and the transforms and chains the calls with
+ * voxel_downsample_batch_f64 (C = 4: colour, normals) between scatter and finish.  All arithmetic is fp64 without
+ * FMA unless stated, each sum in the association stated; all pointers [dev] unless marked [host].
+ *
+ * Pair t of T is store points [offset[t], offset[t] + npts[t]) of every plane, moved into output pair_out[t] by
+ * P [T][16] (row-major 4x4).  Output o owns pairs [first[o], first[o + 1]) ([B + 1] i32), in window order.  box [host,
+ * 4] float32 (x_lo, x_hi, y_lo, y_hi): a point is dropped when x_lo < x < x_hi and y_lo < y < y_hi in float32.
+ * kitti_build_count_f32: pos [T] i64 = first output index of each pair, n_pts [B] i64 = the output's kept points,
+ *   omax [B] f32 = their largest intensity (-inf when none).  workspace >= kitti_build_count_workspace_bytes(T),
+ *   256-byte aligned.
+ * kitti_build_scatter_f64: the kept points in pair order, then point order: xyz_out [B][3][n_stride] =
+ *   ((P0 x + P1 y) + P2 z) + P3 per row, attr_out [B][4][n_stride] = (double)(intensity / omax) in float32, then
+ *   ((P0 nx + P1 ny) + P2 nz) + P3 per row (the translation included, as the reference moves its normals).  Entries
+ *   past n_pts are not written; n_stride % 16 == 0 and n_stride >= max n_pts.
+ * kitti_build_finish_f32: xyz [B][3][n_stride], attr [B][4][n_stride], m_pts [B] i32 <= m_stride (the voxel grid's
+ *   outputs): the voxels with sqrt(x x + y y) < radius, in order, as out [B][7][m_stride] f32 = (x, y, z,
+ *   attr0 * omax, attr1, attr2, attr3) each rounded once, zeros past count [B] i32.
+ * ------------------------------------------------------------------------------------------ */
+size_t kitti_build_count_workspace_bytes(int T);
+int kitti_build_count_f32(const float* planes, int64_t plane_stride, const int64_t* offset, const int32_t* npts,
+                          int T, const int32_t* first, int B, const float* box, int64_t* pos, int64_t* n_pts,
+                          float* omax, void* workspace, size_t workspace_bytes, dib_stream_t stream);
+int kitti_build_scatter_f64(const float* planes, int64_t plane_stride, const int64_t* offset, const int32_t* npts,
+                            const int32_t* pair_out, const double* P, int T, int B, const float* box,
+                            const int64_t* pos, const float* omax, int64_t n_stride, double* xyz_out,
+                            double* attr_out, dib_stream_t stream);
+int kitti_build_finish_f32(const double* xyz, const double* attr, const int32_t* m_pts, const float* omax, int B,
+                           double radius, int64_t n_stride, int64_t m_stride, float* out, int32_t* count,
+                           dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
