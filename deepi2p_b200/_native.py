@@ -47,6 +47,7 @@ EXPORTS = (
     "node_mlp_packed_bytes", "node_mlp_pack_f32", "node_mlp_workspace_bytes", "node_mlp_f32",
     "nuscenes_walk_count", "nuscenes_walk_scan_workspace_bytes", "nuscenes_walk_scan", "nuscenes_walk_fill",
     "kitti_build_count_workspace_bytes", "kitti_build_count_f32", "kitti_build_scatter_f64", "kitti_build_finish_f32",
+    "resnet_conv_packed_bytes", "resnet_conv_pack_f32", "resnet_conv_f32", "resnet_maxpool_f32", "resnet_mean_f32",
 )
 
 
@@ -281,6 +282,17 @@ def load():
     lib.node_mlp_workspace_bytes.argtypes = [vp, i32, vp, i32, i32]
     lib.node_mlp_f32.restype = i32
     lib.node_mlp_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, vp, vp, sz, vp]
+    lib.resnet_conv_packed_bytes.restype = sz
+    lib.resnet_conv_packed_bytes.argtypes = [i32, i32]
+    lib.resnet_conv_pack_f32.restype = i32
+    lib.resnet_conv_pack_f32.argtypes = [vp, i32, i32, vp, sz, vp]
+    lib.resnet_conv_f32.restype = i32
+    lib.resnet_conv_f32.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, sz, vp, vp,
+                                    i32, i32, vp, vp, vp]
+    lib.resnet_maxpool_f32.restype = i32
+    lib.resnet_maxpool_f32.argtypes = [vp, i32, i32, i32, i32, vp, vp]
+    lib.resnet_mean_f32.restype = i32
+    lib.resnet_mean_f32.argtypes = [vp, i32, i32, vp, vp]
     lib.png_decode_workspace_bytes.restype = sz
     lib.png_decode_workspace_bytes.argtypes = [vp, i32, vp, i32, sz]
     lib.png_decode_batch_u8.restype = i32

@@ -24,7 +24,7 @@ import types
 import torch
 import torch.nn as nn
 
-from . import classifier, frustum, point_ops
+from . import classifier, frustum, point_ops, resnet
 
 # the image sizes of the shipped option sets (kitti/options.py, oxford/options.py, nuscenes_t/options.py); all three
 # use fine_scale 32, 20480 points, 128 / 128 nodes, k_ab 16, k = 3, BatchNorm and ReLU
@@ -335,6 +335,32 @@ def fold_knn_fusion(module, dtype=torch.float32):
             fold_pointnet(types.SimpleNamespace(layers=module.layers_after), dtype))
 
 
+def _fold_conv_bn(conv, norm, dtype):
+    W = conv.weight.detach().double()
+    scale = norm.weight.detach().double() / torch.sqrt(norm.running_var.detach().double() + norm.eps)
+    W = W * scale.reshape(-1, 1, 1, 1)
+    b = norm.bias.detach().double() - norm.running_mean.detach().double() * scale
+    return W.permute(0, 2, 3, 1).to(dtype).contiguous(), b.to(dtype).contiguous()
+
+
+def fold_resnet34(backbone, dtype=torch.float32):
+    """Every convolution of a _ResNet34 with its eval-mode BatchNorm folded in float64 (fold_pointnet's formula: W' =
+    W * gamma / sqrt(var + eps) per output channel, b' = beta - mean * gamma / sqrt(var + eps); the convolutions have no
+    bias), then rounded once to `dtype`.  Returns a dict in forward order, keyed by torchvision's module names: "conv1"
+    (the stem), "layer{s}.{j}.conv1", "layer{s}.{j}.conv2" and, for the first block of layers 2-4,
+    "layer{s}.0.downsample" (the 1x1 stride-2 convolution with its own BatchNorm), each (W [C_out, kh, kw, C_in], b
+    [C_out]): the layout resnet.pack_resnet34 reads.  fc is not used and not folded.  The tensors are new (detached)
+    and live on the backbone's device."""
+    out = {"conv1": _fold_conv_bn(backbone.conv1, backbone.bn1, dtype)}
+    for s in range(1, 5):
+        for j, block in enumerate(getattr(backbone, f"layer{s}")):
+            out[f"layer{s}.{j}.conv1"] = _fold_conv_bn(block.conv1, block.bn1, dtype)
+            out[f"layer{s}.{j}.conv2"] = _fold_conv_bn(block.conv2, block.bn2, dtype)
+            if block.downsample is not None:
+                out[f"layer{s}.{j}.downsample"] = _fold_conv_bn(block.downsample[0], block.downsample[1], dtype)
+    return out
+
+
 class FusedInference:
     """Inference through KeypointDetector with its per-point layers fused (DESIGN.md 4.21): first_pointnet,
     second_pointnet and the decoder's two per-point interpolations + concatenation + per_point_pn + predict each run
@@ -346,6 +372,9 @@ class FusedInference:
     PointNets (node_b_attention_pn, node_b_pn, node_a_attention_pn, node_a_pn) as one point_ops.node_mlp call each
     (DESIGN.md 4.27): the per-sample inputs (img_global, global_feature) are projected once per sample instead of
     being expanded and concatenated.  attention_fusion and the ab interpolation stay the project's exact ops.
+    image="fused" runs the ResNet-34 image encoder as resnet.resnet34_features (DESIGN.md 4.30): each convolution
+    with its BatchNorm folded in, bias, residual and ReLU in one implicit-GEMM kernel over NHWC activations, the
+    stride-16 / stride-32 maps written channel-major and img_global a float64 mean rounded once.
 
     The fused layers compute in TF32 whatever torch's TF32 flags say, with BatchNorm folded into the weights, so the
     scores differ from model.forward's at rounding level and a prediction can differ where the top two scores nearly
@@ -358,6 +387,7 @@ class FusedInference:
 
     ENCODERS = ("torch", "fused")
     DECODERS = ("torch", "fused")
+    IMAGES = ("torch", "fused")
 
     # node-level PointNets of the decoder: the (channels, per sample) of their input rows, in torch.cat's order
     _NODE_CHAINS = {"att_b": (lambda m: m.node_b_attention_pn, ((256, False), (512, True))),
@@ -365,14 +395,16 @@ class FusedInference:
                     "att_a": (lambda m: m.node_a_attention_pn, ((64, False), (512, True))),
                     "node_a": (lambda m: m.node_a_pn, ((64, False), (512, False), (256, False)))}
 
-    def __init__(self, model, encoder="torch", decoder="torch"):
+    def __init__(self, model, encoder="torch", decoder="torch", image="torch"):
         if not isinstance(model, KeypointDetector):
             raise TypeError("FusedInference wraps a network.KeypointDetector")
         if encoder not in self.ENCODERS:
             raise ValueError(f"encoder must be one of {self.ENCODERS}, got {encoder!r}")
         if decoder not in self.DECODERS:
             raise ValueError(f"decoder must be one of {self.DECODERS}, got {decoder!r}")
-        self.model, self.encoder, self.decoder = model, encoder, decoder
+        if image not in self.IMAGES:
+            raise ValueError(f"image must be one of {self.IMAGES}, got {image!r}")
+        self.model, self.encoder, self.decoder, self.image = model, encoder, decoder, image
         self._packed, self._stamp = {}, {}
 
     def _cached(self, name, module, pack):
@@ -394,6 +426,9 @@ class FusedInference:
             pn = enc.final_pointnet
             return self._cached(name, pn, lambda: point_ops.pack_pointwise_mlp_max(pn.layers[0].conv.in_channels,
                                                                                      fold_pointnet(pn)))
+        if name == "resnet":
+            bb = model.img_encoder.backbone
+            return self._cached(name, bb, lambda: resnet.pack_resnet34(fold_resnet34(bb)))
         if name in self._NODE_CHAINS:
             get, spec = self._NODE_CHAINS[name]
             pn = get(model)
@@ -443,11 +478,15 @@ class FusedInference:
             final_pn_out = enc.final_pointnet(torch.cat((node_b, node_b_features), dim=1))
             global_feature = torch.max(final_pn_out, dim=2, keepdim=True)[0]
 
-        s16, s32 = model.img_encoder.backbone(img)
-        img_global = s32.mean(dim=(2, 3))
-        C_img = img_global.shape[1]
-        s16 = s16.reshape(B, s16.shape[1], -1).contiguous()
-        s32 = s32.reshape(B, C_img, -1).contiguous()
+        if self.image == "fused":
+            s16, s32, img_global = resnet.resnet34_features(img.contiguous(), self._chain("resnet"))
+            C_img = img_global.shape[1]
+        else:
+            s16, s32 = model.img_encoder.backbone(img)
+            img_global = s32.mean(dim=(2, 3))
+            C_img = img_global.shape[1]
+            s16 = s16.reshape(B, s16.shape[1], -1).contiguous()
+            s32 = s32.reshape(B, C_img, -1).contiguous()
         img_global_a = img_global.unsqueeze(2).expand(B, C_img, Ma)
         img_global_b = img_global.unsqueeze(2).expand(B, C_img, Mb)
 
@@ -485,7 +524,7 @@ class FusedInference:
                                        return_scores=return_scores)
 
 
-HEADS = ("torch", "fused", "fused_encoder", "fused_all")
+HEADS = ("torch", "fused", "fused_encoder", "fused_all", "fused_image")
 
 
 def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chunk=DEFAULT_CHUNK, n_inits=60, seed=0,
@@ -506,7 +545,9 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
     "torch" at points whose top two scores nearly tie.  "fused_encoder" is FusedInference(model, encoder="fused")
     per chunk: the point encoder's kNN module and final_pointnet + max run fused in TF32 too.  "fused_all" is
     FusedInference(model, encoder="fused", decoder="fused") per chunk: the decoder's node-level PointNets run fused in
-    TF32 as well, so only ResNet keeps separate convolution / BatchNorm / ReLU kernels.
+    TF32 as well, so only ResNet keeps separate convolution / BatchNorm / ReLU kernels.  "fused_image" is
+    FusedInference(model, encoder="fused", decoder="fused", image="fused") per chunk: ResNet-34 runs as fused TF32
+    implicit-GEMM convolutions too, so no separate convolution, BatchNorm or ReLU kernel is left.
 
     Returns dict(P [S,4,4] f64, cost [S] f64, coarse_pred int8 [S,N], fine_pred int32 [S,N] or None, degenerate
     int32 [S]); a sample with no point predicted inside gets P = I, cost 1e4 and degenerate = 1."""
@@ -516,8 +557,9 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
         raise ValueError(f"chunk must be >= 1, got {chunk}")
     if head not in HEADS:
         raise ValueError(f"head must be one of {HEADS}, got {head!r}")
-    fused = FusedInference(model, encoder="fused" if head in ("fused_encoder", "fused_all") else "torch",
-                           decoder="fused" if head == "fused_all" else "torch") if head != "torch" else None
+    fused = FusedInference(model, encoder="fused" if head in ("fused_encoder", "fused_all", "fused_image") else "torch",
+                           decoder="fused" if head in ("fused_all", "fused_image") else "torch",
+                           image="fused" if head == "fused_image" else "torch") if head != "torch" else None
     for t, name in ((intensity, "intensity"), (sn, "sn"), (node_a, "node_a"), (node_b, "node_b"), (img, "img")):
         if t.shape[0] != S:
             raise ValueError(f"{name} has {t.shape[0]} samples, pc has {S}")

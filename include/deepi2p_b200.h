@@ -756,6 +756,38 @@ int node_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, i
                  dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Fused inference of the classifier's ResNet-34 image encoder (models/resnet.py; SURVEY.md 8f N25).  DESIGN.md 4.30
+ * states the contract.  One convolution with its eval-mode BatchNorm folded into the weights and bias by the caller,
+ * as an implicit GEMM on the TF32 tensor cores: M = B * H_out * W_out output pixels, N = C_out, K = kernel^2 * C_in
+ * (+ C2 with a shortcut).  H_out = (H + 2 pad - kernel) / stride + 1, the same for W.
+ *   x: NHWC [B][H][W][C_in] f32 (nchw = 0, C_in % 32 == 0, 16-byte aligned) or NCHW [B][C_in][H][W] f32 (nchw = 1, any
+ *     C_in: the stem reads the assembled image directly).
+ *   shortcut (or NULL): NHWC [B][H2][W2][C2] f32, C2 % 32 == 0, read as a 1x1 convolution of stride stride2 and no
+ *     padding whose K columns follow the main ones (a block's downsample fused into its second convolution; needs
+ *     kernel^2 * C_in % 32 == 0 and (H2 - 1) / stride2 + 1 == H_out, the same for W).
+ *   packed: resnet_conv_pack_f32's image of W [C_out][kernel][kernel][C_in] (with a shortcut, each row followed by
+ *     the shortcut's C2 weights: K = kernel^2 C_in + C2).  bias [C_out] f32.  residual (or NULL): NHWC [M][C_out] f32.
+ *   out = relu?((sum_k x_k W_k + bias) + residual) with operands rounded to TF32 (nearest, ties away from zero; the
+ *     weights when packed), f32 accumulation, and ReLU keeping NaN.  Written to out_nhwc [M][C_out] and/or out_cm
+ *     [B][C_out][H_out * W_out] (either may be NULL, not both); out_nhwc and residual 8-byte aligned.
+ * C_out % 8 == 0.  Deterministic: no atomics.  [dev] pointers; 1 <= B <= 65535.
+ *
+ * resnet_conv_pack_f32: w [C_out][K] f32 -> packed ([dev] 16-byte aligned, >= resnet_conv_packed_bytes(C_out, K)
+ *   bytes): each row rounded to TF32 and zero-padded to a multiple of 32.
+ * resnet_maxpool_f32: the 3x3 stride-2 pad-1 max-pool of NHWC x [B][H][W][C] into out [B][(H-1)/2+1][(W-1)/2+1][C];
+ *   a NaN in a window gives NaN (torch.nn.MaxPool2d's rule).
+ * resnet_mean_f32: out[r] = mean of x[r][0..P) for r < rows, a float64 sum in a fixed order rounded once.
+ * ------------------------------------------------------------------------------------------ */
+size_t resnet_conv_packed_bytes(int C_out, int K);
+int resnet_conv_pack_f32(const float* w, int C_out, int K, void* packed, size_t packed_bytes, dib_stream_t stream);
+int resnet_conv_f32(const float* x, int nchw, int B, int H, int W, int C_in, int kernel, int stride, int pad,
+                    const float* shortcut, int H2, int W2, int C2, int stride2, const void* packed,
+                    size_t packed_bytes, const float* bias, const float* residual, int relu, int C_out,
+                    float* out_nhwc, float* out_cm, dib_stream_t stream);
+int resnet_maxpool_f32(const float* x, int B, int H, int W, int C, float* out, dib_stream_t stream);
+int resnet_mean_f32(const float* x, int rows, int P, float* out, dib_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Batched PNG decoding (KITTI's official odometry colour frames).  DESIGN.md 4.23 states the contract: 8-bit
  * truecolour, not interlaced, decoded bit for bit as OpenCV 4.13's cv2.imdecode(..., IMREAD_COLOR)[:, :, ::-1]
  * (HWC uint8 RGB).  deepi2p_b200/png.py walks the chunks, checks IHDR / PLTE / IEND and the zlib header, and fills
