@@ -48,6 +48,7 @@ EXPORTS = (
     "nuscenes_walk_count", "nuscenes_walk_scan_workspace_bytes", "nuscenes_walk_scan", "nuscenes_walk_fill",
     "kitti_build_count_workspace_bytes", "kitti_build_count_f32", "kitti_build_scatter_f64", "kitti_build_finish_f32",
     "resnet_conv_packed_bytes", "resnet_conv_pack_f32", "resnet_conv_f32", "resnet_maxpool_f32", "resnet_mean_f32",
+    "monodepth_resize_f32", "monodepth_cloud_workspace_bytes", "monodepth_cloud_f32",
 )
 
 
@@ -293,6 +294,14 @@ def load():
     lib.resnet_maxpool_f32.argtypes = [vp, i32, i32, i32, i32, vp, vp]
     lib.resnet_mean_f32.restype = i32
     lib.resnet_mean_f32.argtypes = [vp, i32, i32, vp, vp]
+    lib.monodepth_resize_f32.restype = i32
+    lib.monodepth_resize_f32.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, i32, _c.c_float, _c.c_float,
+                                         vp, sz, vp, vp]
+    lib.monodepth_cloud_workspace_bytes.restype = sz
+    lib.monodepth_cloud_workspace_bytes.argtypes = [i32, i32, i32]
+    lib.monodepth_cloud_f32.restype = i32
+    lib.monodepth_cloud_f32.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, sz,
+                                        vp]
     lib.png_decode_workspace_bytes.restype = sz
     lib.png_decode_workspace_bytes.argtypes = [vp, i32, vp, i32, sz]
     lib.png_decode_batch_u8.restype = i32

@@ -16,13 +16,14 @@ LIB = os.path.join(LIBDIR, "libdeepi2p_b200.so")
 SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "ball_query_xyz.cu", "cluster_assign.cu",
            "pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu", "classifier_loss.cu",
            "encoder_ops.cu", "fusion.cu", "jpeg.cu", "png.cu", "pointwise_mlp.cu", "oxford_build.cu", "oxford_images.cu",
-           "jpeg_encode.cu", "knn_fusion.cu", "node_mlp.cu", "nuscenes_build.cu", "kitti_build.cu", "resnet.cu"]
+           "jpeg_encode.cu", "knn_fusion.cu", "node_mlp.cu", "nuscenes_build.cu", "kitti_build.cu", "resnet.cu", "monodepth.cu"]
 # Compiled on their own without FMA contraction: oracle_pnp/pnp_oracle.cpp, oracle_icp/icp_oracle.cpp and
 # oracle_prep/prep_oracle.cpp, oracle_assemble/, oracle_interp/, oracle_image/ and oracle.pose_diff_restated (metrics.cu)
 # restate their arithmetic bit for bit (oracle_oxford_build/, oracle_oxford_images/ and oracle_kitti_build/ too); metrics.cu and
-# classifier_loss.cu share the label rule of project.cuh.
+# classifier_loss.cu share the label rule of project.cuh.  monodepth.cu writes out the contractions of torch's bilinear
+# kernel with __fmaf_rn and keeps the back-projection to plain products and sums (DESIGN.md 4.31).
 NOFMA_SOURCES = ["pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu", "metrics.cu",
-                 "classifier_loss.cu", "oxford_build.cu", "oxford_images.cu", "kitti_build.cu"]
+                 "classifier_loss.cu", "oxford_build.cu", "oxford_images.cu", "kitti_build.cu", "monodepth.cu"]
 HEADERS = ["common.cuh", "morton_index.cuh", "sym3_eig.cuh", "project.cuh", "nearest_k.cuh", "tf32_mma.cuh", os.path.join("..", "..", "include", "deepi2p_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -181,11 +181,15 @@ def get_p_diff(P_pred, P_gt):
 
 def register_directory_icp(data_dir, monodepth_dir, H, W, n_inits=60, seed=0, max_corr_dist=1.0, max_iteration=30,
                            enu2cam=False, batch=64, names=None, device="cuda", out_dir=None, t_thresh=2.0,
-                           r_thresh=5.0):
+                           r_thresh=5.0, *, depth_model=None, image_dir=None):
     """The __main__ of evaluation/icp/registration_icp.py:165-245 as one function: every frame of a legacy directory
     and its <monodepth_dir>/<id>_pc.npy depth cloud, scale-calibrated with the ground truth (icp.calibrate_scale),
     through icp.icp_register_batch (the GPU path, random_inits(S, n_inits, seed + first frame of the batch)), errors
-    by get_p_diff, and the P_pred_all_np / P_gt_all_np / cost_all_np files (cost = fitness, :241-243)."""
+    by get_p_diff, and the P_pred_all_np / P_gt_all_np / cost_all_np files (cost = fitness, :241-243).
+
+    With depth_model (a monodepth.DepthNet, monodepth.load_monodepth), the depth clouds are made on the device from
+    <image_dir>/<id>_img.png instead (save_depth_map.py's input; image_dir defaults to the sibling visualization/ of
+    data_dir, the reference's layout) by icp.register_images, and monodepth_dir is not read."""
     import torch
     from . import icp
 
@@ -194,7 +198,24 @@ def register_directory_icp(data_dir, monodepth_dir, H, W, n_inits=60, seed=0, ma
     P_pred = np.zeros((len(names), 4, 4))
     P_gt = np.zeros((len(names), 4, 4))
     cost = np.zeros((len(names),))
+    if depth_model is not None:
+        from . import imageprep
+        if image_dir is None:
+            image_dir = os.path.join(os.path.dirname(os.path.normpath(data_dir)), "visualization")
     for a in range(0, len(names), batch):
+        if depth_model is not None:
+            part = names[a:a + batch]
+            recs = [load_record(data_dir, name, enu2cam=enu2cam) for name in part]
+            src, n = icp.pack_clouds([r[0] for r in recs], device)
+            K_raw = np.stack([np.load(os.path.join(data_dir, name + "_K.npy")) for name in part])
+            images = imageprep.read_png_batch([os.path.join(image_dir, name + "_img.png") for name in part], device)
+            P_gt[a:a + len(part)] = np.stack([r[3] for r in recs])
+            init = torch.from_numpy(icp.random_inits(len(part), n_inits, seed + a)).to(src.device)
+            out = icp.register_images(src, n, images, K_raw, P_gt[a:a + len(part)], init, depth_model,
+                                      max_corr_dist=max_corr_dist, max_iteration=max_iteration)
+            P_pred[a:a + batch] = out["P"].cpu().numpy()
+            cost[a:a + batch] = out["fitness"].cpu().numpy()
+            continue
         srcs, tgts = [], []
         for s, name in enumerate(names[a:a + batch]):
             pc, _, K, P = load_record(data_dir, name, enu2cam=enu2cam)

@@ -139,6 +139,30 @@ def calibrate_scale(pc, P_gt, K, H, W, depth_pc):
     return float(np.mean(z[mask]) / np.mean(np.asarray(depth_pc, dtype=np.float64)[2, :]))
 
 
+def register_images(src, n_pts, images, K, P_gt, init, model, K_inv=None, stream=None, **kw):
+    """registration_icp.py from images: the depth clouds of pack_images' frames (monodepth.depth_clouds with `model`,
+    one image size per call), their ground-truth scale calibration and the float32 target are made on the device and
+    handed to icp_register_batch with the LiDAR clouds src [S,3,Ns] f32 / n_pts [S] int32 or None and init
+    [S,I,4,4] f64.  K [S,3,3] in its stored dtype (the intrinsics of the images, also used for the inside test in
+    float64), P_gt [S,4,4] float64; K_inv defaults to monodepth.k_inverse(K).  Other keywords go to
+    icp_register_batch.  Returns its dict with "scale" [S] f64 added."""
+    from . import monodepth
+    K = np.asarray(K)
+    if K_inv is None:
+        K_inv = monodepth.k_inverse(K)
+    d = monodepth.depth_clouds(model, images, K_inv, src=src, n_pts=n_pts, P_gt=P_gt,
+                               K=np.asarray(K, np.float64).reshape(-1, 9), cloud64=False, stream=stream)
+    tgt = d["tgt"]
+    M = tgt.shape[2]
+    Ms = round_up(max(M, 1), 16)
+    if Ms != M:
+        tgt = torch.nn.functional.pad(tgt, (0, Ms - M)).contiguous()
+    m = torch.full((tgt.shape[0],), M, dtype=torch.int32, device=tgt.device)
+    out = icp_register_batch(src, n_pts, tgt, m, init, stream=stream, **kw)
+    out["scale"] = d["scale"]
+    return out
+
+
 def icp_random_init(pc_np, pc_monodepth_np, num_iterations, is_plot, seed=0):
     """Drop-in body of icp_random_init (registration_icp.py:115-139): numpy in, (P 4x4 ndarray, fitness float) out.
     Both clouds are rounded to float32; the inits are random_inits(1, num_iterations, seed)."""

@@ -972,6 +972,36 @@ int kitti_build_finish_f32(const double* xyz, const double* attr, const int32_t*
                            double radius, int64_t n_stride, int64_t m_stride, float* out, int32_t* count,
                            dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Monodepth depth clouds for the ICP baseline (evaluation/icp/save_depth_map.py; SURVEY.md 8f N26).  DESIGN.md 4.31
+ * states the contract.
+ *
+ * monodepth_resize_f32: Pillow's Image.resize((out_w, out_h), LANCZOS) of S uint8 HWC RGB frames of one size h x w,
+ *   then ToTensor and the encoder's normalisation: out [S][3][out_h][out_w] f32 = (v / 255 - sub) * mul, v the
+ *   resized uint8 value ((x - 0.45) / 0.225 as torch computes it on the device: sub = 0.45f, mul = 1.0f / 0.225f).
+ *   data: [dev] frame s at data + offsets[s] ([dev] int64 [S]; NULL: s * h * w * 3).  tab_x ([dev] int32
+ *   [out_w][2 + kx]: first input column, tap count, kx fixed-point coefficients in 2^-22 units) must be given exactly
+ *   when w != out_w, tab_y ([out_h][2 + ky], rows) exactly when h != out_h; the horizontal pass runs first.  With both
+ *   passes tmp [dev] holds the uint8 intermediate (>= S * h * out_w * 3 bytes).  1 <= S <= 65535.
+ *
+ * monodepth_cloud_f32: for disp [dev] [S][h][w] f32 (the decoder's ("disp", 0)), depth = 1 / bilinear(disp) at
+ *   H x W (torch's CUDA upsample_bilinear2d with align_corners=False, bit for bit, then torch.reciprocal), and the
+ *   point y W + x of the cloud is K_inv[s] (d x, d y, d) in fp64 (K_inv [dev] [S][9] row-major).  Outputs (any may be
+ *   NULL, not all): depth [S][H*W] f32; out64 [S][3][H*W] f64, unscaled; scale [S] f64 = mean camera z of the
+ *   LiDAR points inside the image under P_gt (src [S][3][Ns] f32, n_pts [S] i32 or NULL, P_gt [S][16] f64, K [S][9]
+ *   f64, the project_inside rule at H x W) over the mean z of the cloud, both fp64 sums in a fixed order (NaN
+ *   without an inside point); out32 [S][3][H*W] f32 = float32(p scale[s]) (needs scale).  The scale needs
+ *   workspace >= monodepth_cloud_workspace_bytes(S, H, W).  All pointers [dev].  Deterministic: no atomics.
+ * ------------------------------------------------------------------------------------------ */
+int monodepth_resize_f32(const uint8_t* data, const int64_t* offsets, int S, int h, int w, int out_h, int out_w,
+                         const int32_t* tab_x, int kx, const int32_t* tab_y, int ky, float sub, float mul,
+                         uint8_t* tmp, size_t tmp_bytes, float* out, dib_stream_t stream);
+size_t monodepth_cloud_workspace_bytes(int S, int H, int W);
+int monodepth_cloud_f32(const float* disp, int S, int h, int w, int H, int W, const double* K_inv, float* depth,
+                        double* out64, const float* src, const int32_t* n_pts, int Ns, const double* P_gt,
+                        const double* K, double* scale, float* out32, void* workspace, size_t workspace_bytes,
+                        dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,11 +6,14 @@ Replaces `python evaluation/registration_lsq.py` + `registration_result_analysis
 visualize_and_save_data.py:174-186, and, with --method pnp, `python evaluation/registration_pnp.py`
 (registration_pnp.py:151-259: grid classification + PnP-RANSAC, cost = outlier ratio) and, with --method icp,
 `python evaluation/icp/registration_icp.py` (registration_icp.py:165-245: monodepth cloud + multi-start ICP,
-cost = fitness; the depth clouds <id>_pc.npy come from --monodepth).  Examples:
+cost = fitness; the depth clouds <id>_pc.npy come from --monodepth, or are made on the GPU from the
+<id>_img.png frames of the sibling visualization/ directory by the monodepth2 checkpoint in --depth-model, as
+save_depth_map.py would).  Examples:
 
     python scripts/register_dir.py /data/kitti/save/run/data --H 160 --W 512 --out /data/kitti/save/run
     python scripts/register_dir.py /data/kitti/save/run/data --H 160 --W 512 --method pnp --fine-scale 0.03125
     python scripts/register_dir.py /data/oxford/run/data --H 384 --W 640 --method icp --monodepth /data/oxford/run/monodepth
+    python scripts/register_dir.py run/data --H 384 --W 640 --method icp --depth-model models/mono+stereo_640x192
 """
 import argparse
 import json
@@ -32,7 +35,12 @@ def main():
                          "pnp: grid classification + PnP-RANSAC (registration_pnp.py); "
                          "icp: monodepth cloud + multi-start ICP (icp/registration_icp.py)")
     ap.add_argument("--monodepth", default=None,
-                    help="icp only (required): directory of the <id>_pc.npy depth clouds (save_depth_map.py)")
+                    help="icp only (this or --depth-model): directory of the <id>_pc.npy depth clouds "
+                         "(save_depth_map.py)")
+    ap.add_argument("--depth-model", default=None,
+                    help="icp only (this or --monodepth): monodepth2 checkpoint directory (encoder.pth, "
+                         "depth.pth); the depth clouds are made on the GPU from the <id>_img.png frames in "
+                         "visualization/ beside data_dir")
     ap.add_argument("--labels", default="coarse_prediction", choices=sorted(handoff.LABEL_ROWS),
                     help="lsq only: the in/out-of-frustum row the solver reads")
     ap.add_argument("--fine-scale", type=float, default=1 / 32.0,
@@ -49,15 +57,23 @@ def main():
 
     if args.method == "lsq" and args.labels.startswith("fine_"):
         ap.error("--labels %s holds grid cell indices, not in/out-of-frustum labels; use --method pnp" % args.labels)
-    if args.method == "icp" and args.monodepth is None:
-        ap.error("--method icp needs --monodepth DIR (the <id>_pc.npy depth clouds)")
+    if args.method == "icp" and args.monodepth is None and args.depth_model is None:
+        ap.error("--method icp needs --monodepth DIR (the <id>_pc.npy depth clouds) or --depth-model DIR")
+    if args.method == "icp" and args.monodepth is not None and args.depth_model is not None:
+        ap.error("--monodepth and --depth-model are alternatives; give one")
     if args.method != "icp" and args.monodepth is not None:
         ap.error("--monodepth is only used by --method icp")
+    if args.method != "icp" and args.depth_model is not None:
+        ap.error("--depth-model is only used by --method icp")
     names = handoff.list_records(args.data_dir)[::args.every]
     if args.method == "icp":
+        model = None
+        if args.depth_model is not None:
+            from deepi2p_b200 import monodepth
+            model = monodepth.load_monodepth(args.depth_model)
         res = handoff.register_directory_icp(args.data_dir, args.monodepth, args.H, args.W, n_inits=args.inits,
                                              seed=args.seed, enu2cam=args.enu2cam, batch=args.batch,
-                                             names=names, out_dir=args.out)
+                                             names=names, out_dir=args.out, depth_model=model)
     elif args.method == "pnp":
         res = handoff.register_directory_pnp(args.data_dir, args.H, args.W, fine_scale=args.fine_scale,
                                              iterations=args.iterations, seed=args.seed, enu2cam=args.enu2cam,
