@@ -60,6 +60,21 @@ def ball_query_forward(node_to_point_dist, radius, K):
 _xyz_ws = {}
 
 
+def _stream_workspace(cache, dev, stream, need, floor):
+    """One cached scratch per (device, stream): launches on one stream run in order, so they can share it; launches on
+    different streams may overlap.  While the current stream is being captured into a CUDA graph the scratch is a new
+    allocation from the graph's private pool and is not cached: a graph-pool buffer is never handed to a later eager
+    call, and a cached eager buffer is never resized under a graph that captured its address."""
+    if torch.cuda.is_current_stream_capturing():
+        return torch.empty(max(need, floor), dtype=torch.uint8, device=dev)
+    key = (dev.index, stream)
+    ws = cache.get(key)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(max(need, floor), dtype=torch.uint8, device=dev)
+        cache[key] = ws
+    return ws
+
+
 def ball_query_xyz_forward(points, nodes, radius, K):
     """Grid-hash radius search from coordinates: points [B,3,N], nodes [B,3,M] float32 CUDA -> int32 [B,M,K]
     with the ball_query contract (first K indices in ascending n within radius; none -> 0; fewer -> cyclic).
@@ -77,12 +92,8 @@ def ball_query_xyz_forward(points, nodes, radius, K):
     K = int(K)
     dev = points.device
     with torch.cuda.device(dev):
-        need = lib.ball_query_xyz_workspace_bytes(B, N)
-        key = (dev.index, torch.cuda.current_stream().cuda_stream)     # one scratch per stream: launches may overlap
-        ws = _xyz_ws.get(key)
-        if ws is None or ws.numel() < need:
-            ws = torch.empty(max(need, 1 << 20), dtype=torch.uint8, device=dev)
-            _xyz_ws[key] = ws
+        ws = _stream_workspace(_xyz_ws, dev, torch.cuda.current_stream().cuda_stream,
+                               lib.ball_query_xyz_workspace_bytes(B, N), 1 << 20)
         out = torch.empty((B, M, K), dtype=torch.int32, device=dev)
         rc = lib.ball_query_xyz_forward(points.data_ptr(), nodes.data_ptr(), float(radius), out.data_ptr(), B, M, N, K,
                                         ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
@@ -110,12 +121,8 @@ def cluster_assign_forward(pc, node, k=1, want_centers=True):
     k = int(k)
     dev = pc.device
     with torch.cuda.device(dev):
-        need = lib.cluster_assign_workspace_bytes(B, M)
-        key = (dev.index, torch.cuda.current_stream().cuda_stream)
-        ws = _ca_ws.get(key)
-        if ws is None or ws.numel() < need:
-            ws = torch.empty(max(need, 1 << 16), dtype=torch.uint8, device=dev)
-            _ca_ws[key] = ws
+        ws = _stream_workspace(_ca_ws, dev, torch.cuda.current_stream().cuda_stream,
+                               lib.cluster_assign_workspace_bytes(B, M), 1 << 16)
         topk = torch.empty((B, N, k), dtype=torch.int32, device=dev)
         min_idx = torch.empty((B, N), dtype=torch.int32, device=dev)
         count = torch.empty((B, M), dtype=torch.int32, device=dev)
@@ -140,12 +147,7 @@ _backward_ws = {}
 def _backward_workspace(dev, stream, need):
     """The fp64 slice partials of the interpolation's and the encoder ops' backwards: one scratch per stream (launches
     on one stream run in order, so they can share it; launches on different streams may overlap)."""
-    key = (dev.index, stream)
-    ws = _backward_ws.get(key)
-    if ws is None or ws.numel() < need:
-        ws = torch.empty(max(need, 1 << 16), dtype=torch.uint8, device=dev)
-        _backward_ws[key] = ws
-    return ws
+    return _stream_workspace(_backward_ws, dev, stream, need, 1 << 16)
 
 
 def _check_interp_args(topk_idx, query, node, features):
