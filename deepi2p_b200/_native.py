@@ -1,62 +1,87 @@
-"""ctypes binding of the C ABI declared in include/deepi2p_b200.h.
+"""ctypes binding of the C ABI declared in include/deepi2p_b200.h, and the host helpers every wrapper around it shares.
 
-There is no CPU fallback: if the library is missing or a call fails, this raises.
+The signatures are read from the header itself when the library is loaded, so the header is the only place an entry
+point is declared.  There is no CPU fallback: if the library is missing or a call fails, this raises.
 """
 import ctypes
 import os
+import re
+
+import torch
 
 from . import build as _build
 
 _c = ctypes
 _lib = None
 
-EXPORTS = (
-    "dib_abi_version", "dib_last_error", "dib_device_sm_count", "dib_profile_solve_events", "dib_evaluate_sliced", "frustum_solve_slice_after", "frustum_solve_slice_rounds",
-    "frustum_solve_workspace_bytes", "frustum_solve_batch_f32", "frustum_solve_batch_f64", "frustum_solve_traced_f32",
-    "frustum_register_workspace_bytes", "frustum_register_batch_f32",
-    "frustum_evaluate_workspace_bytes",
-    "frustum_evaluate_f32", "frustum_evaluate_f64", "frustum_residuals_f32", "frustum_residuals_f64",
-    "frustum_poly_roots_f64", "frustum_interp_step_f64", "frustum_lm_next_step_f64",
-    "frustum_prepare_workspace_bytes", "frustum_prepare_batch_f32", "frustum_sort_batch_f32",
-    "frustum_inside_mask_f32", "pose_error_batch",
-    "index_max_forward", "ball_query_forward", "ball_query_xyz_workspace_bytes", "ball_query_xyz_forward",
-    "cluster_assign_workspace_bytes", "cluster_assign_forward",
-    "pnp_ransac_workspace_bytes", "pnp_ransac_batch_f32", "epnp_batch_f64",
-    "icp_workspace_bytes", "icp_register_batch_f32", "icp_register_batch_counted_f32", "icp_build_index_f32",
-    "voxel_downsample_workspace_bytes", "voxel_downsample_batch_f32", "voxel_downsample_batch_f64",
-    "estimate_normals_workspace_bytes",
-    "estimate_normals_batch_f32", "nearest_batch_f32", "sym3_eig_batch_f64",
-    "assemble_accumulate_workspace_bytes", "assemble_accumulate_f32",
-    "assemble_accumulate_gather_workspace_bytes", "assemble_accumulate_gather_f32",
-    "assemble_accumulate_f64_workspace_bytes", "assemble_accumulate_f64", "assemble_resample_workspace_bytes",
-    "assemble_resample_f32", "assemble_candidates_workspace_bytes", "assemble_candidates_f32", "fps_batch_f32",
-    "fps_batch_f64", "interp_weights_f32", "interp_forward_f32", "interp_backward_workspace_bytes",
-    "interp_backward_f32", "image_assemble_workspace_bytes", "image_assemble_f32", "image_assemble_u8",
-    "classifier_loss_workspace_bytes", "classifier_loss_forward_f32", "classifier_loss_backward_f32",
-    "cluster_pool_forward_f32", "cluster_pool_backward_workspace_bytes", "cluster_pool_backward_f32",
-    "knn_group_forward_f32", "knn_group_backward_workspace_bytes", "knn_group_backward_f32",
-    "attn_fusion_forward_f32", "attn_fusion_backward_f32", "jpeg_decode_workspace_bytes", "jpeg_decode_batch_u8",
-    "pointwise_mlp_packed_bytes", "pointwise_mlp_pack_f32", "pointwise_mlp_workspace_bytes", "pointwise_mlp_f32",
-    "png_decode_workspace_bytes", "png_decode_batch_u8",
-    "oxford_build_plan_f64", "oxford_build_count_workspace_bytes", "oxford_build_count_f64",
-    "oxford_build_scatter_f64", "oxford_build_pack_f32",
-    "oxford_debayer_workspace_bytes", "oxford_debayer_undistort_u8",
-    "jpeg_encode_workspace_bytes", "jpeg_encode_entropy_u8", "jpeg_encode_stuff_u8",
-    "knn_fusion_packed_bytes", "knn_fusion_pack_f32", "knn_fusion_f32", "pointwise_mlp_max_packed_bytes",
-    "pointwise_mlp_max_pack_f32", "pointwise_mlp_max_workspace_bytes", "pointwise_mlp_max_f32",
-    "node_mlp_packed_bytes", "node_mlp_pack_f32", "node_mlp_workspace_bytes", "node_mlp_f32",
-    "nuscenes_walk_count", "nuscenes_walk_scan_workspace_bytes", "nuscenes_walk_scan", "nuscenes_walk_fill",
-    "kitti_build_count_workspace_bytes", "kitti_build_count_f32", "kitti_build_scatter_f64", "kitti_build_finish_f32",
-    "resnet_conv_packed_bytes", "resnet_conv_pack_f32", "resnet_conv_f32", "resnet_maxpool_f32", "resnet_mean_f32",
-    "monodepth_resize_f32", "monodepth_cloud_workspace_bytes", "monodepth_cloud_f32",
-)
+EXPECTED_ABI = 4        # dib_abi_version() of the library include/deepi2p_b200.h declares
 
-
-EXPECTED_ABI = 4        # dib_abi_version() the argtypes below were written for
+_SCALARS = {"int": _c.c_int, "int32_t": _c.c_int, "int64_t": _c.c_int64, "uint64_t": _c.c_uint64,
+            "size_t": _c.c_size_t, "float": _c.c_float, "double": _c.c_double, "dib_stream_t": _c.c_void_p}
 
 
 class NativeError(RuntimeError):
     pass
+
+
+def parse_header(text):
+    """{name: (restype, argtypes)} of every prototype in the C header `text`: plain C with block comments, #-lines,
+    typedefs and extern "C" guards.  Pointers bind as c_void_p, a `const char*` return as c_char_p and a `void` return
+    as None; any type outside those and _SCALARS raises NativeError, so no argument is bound with a guessed width."""
+    text = re.sub(r"/\*.*?\*/|^\s*#[^\n]*|extern\s*\"C\"\s*\{|\}", " ", text, flags=re.S | re.M)
+    sigs = {}
+    for decl in text.split(";"):
+        decl = " ".join(re.sub(r"\s*\*", "* ", decl).split())
+        if not decl or decl.startswith("typedef "):
+            continue
+        m = re.fullmatch(r"(.+) (\w+) ?\((.*)\)", decl)
+        if m is None:
+            raise NativeError(f"cannot read the declaration {decl!r}")
+        ret, name, args = m.groups()
+
+        def ctype(spec):
+            if spec.endswith("*"):
+                return _c.c_void_p
+            t = _SCALARS.get(spec.removeprefix("const "))
+            if t is None:
+                raise NativeError(f"{name}: no ctypes binding for the type {spec!r} in {decl!r}")
+            return t
+        restype = None if ret == "void" else _c.c_char_p if ret == "const char*" else ctype(ret)
+        argtypes = [] if args in ("", "void") else [ctype(a.strip().rpartition(" ")[0]) for a in args.split(",")]
+        sigs[name] = (restype, argtypes)
+    return sigs
+
+
+def _require_cuda():
+    if not torch.cuda.is_available():
+        raise NativeError("deepi2p_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
+
+
+def _stream_ptr(stream=None):
+    s = stream if stream is not None else torch.cuda.current_stream()
+    return s.cuda_stream
+
+
+def _ptr(t):
+    return 0 if t is None else t.data_ptr()
+
+
+def _workspace(cache, need, device, stream=None, floor=1 << 20):
+    """Scratch buffer of at least max(need, floor) bytes for launches on `stream` (None: the current stream), cached in
+    the caller's pool `cache` per (device index, stream pointer): launches on one stream run in order, so they can
+    share it; launches on different streams may overlap.  It is allocated while `stream` is current, so the allocator
+    ties it to the stream that uses it.  While that stream is being captured into a CUDA graph the buffer is a new
+    allocation from the graph's private pool and is not cached: a graph-pool buffer is never handed to a later eager
+    call, and a cached eager buffer is never resized under a graph that captured its address."""
+    with torch.cuda.stream(stream):
+        if torch.cuda.is_current_stream_capturing():
+            return torch.empty(max(need, floor), dtype=torch.uint8, device=device)
+        key = (device.index if device.index is not None else torch.cuda.current_device(), _stream_ptr(stream))
+        ws = cache.get(key)
+        if ws is None or ws.numel() < need:
+            ws = torch.empty(max(need, floor), dtype=torch.uint8, device=device)
+            cache[key] = ws
+    return ws
 
 
 def lib_path():
@@ -86,263 +111,15 @@ def load():
             warnings.warn(f"deepi2p_b200: {path} is older than its sources and the rebuild failed ({e}); "
                           "loading the stale library (its ABI version is checked)")
     lib = ctypes.CDLL(path)
-    vp, i32, f64, sz = _c.c_void_p, _c.c_int, _c.c_double, _c.c_size_t
-    lib.dib_abi_version.restype = i32
+    sigs = parse_header(open(_build.HEADER).read())
+    lib.dib_abi_version.restype, lib.dib_abi_version.argtypes = sigs["dib_abi_version"]
     abi = lib.dib_abi_version()
     if abi != EXPECTED_ABI:
         raise NativeError(f"{path} has ABI version {abi}, this binding was written for {EXPECTED_ABI}: "
                           "rebuild with `python -m deepi2p_b200.build --force`")
-    lib.dib_last_error.restype = _c.c_char_p
-    lib.dib_device_sm_count.restype = i32
-    lib.dib_evaluate_sliced.restype = None
-    lib.dib_evaluate_sliced.argtypes = [i32]
-    lib.frustum_solve_slice_after.restype = i32
-    lib.frustum_solve_slice_after.argtypes = [i32, i32, i32, i32]
-    lib.frustum_solve_slice_rounds.restype = i32
-    lib.frustum_solve_slice_rounds.argtypes = [i32, i32, i32, i32]
-    lib.dib_profile_solve_events.restype = None
-    lib.dib_profile_solve_events.argtypes = [vp, vp]
-    lib.frustum_solve_workspace_bytes.restype = sz
-    lib.frustum_solve_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.frustum_evaluate_workspace_bytes.restype = sz
-    lib.frustum_evaluate_workspace_bytes.argtypes = [i32, i32]
-    solve_args = [vp, vp, vp, i32, vp, vp, vp, vp, f64, f64, i32, i32, i32, i32,
-                  vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    for name in ("frustum_solve_batch_f32", "frustum_solve_batch_f64"):
-        getattr(lib, name).restype = i32
-        getattr(lib, name).argtypes = solve_args
-    lib.frustum_solve_traced_f32.restype = i32
-    lib.frustum_solve_traced_f32.argtypes = solve_args[:20] + [vp, i32] + solve_args[20:]
-    lib.frustum_register_workspace_bytes.restype = sz
-    lib.frustum_register_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.frustum_register_batch_f32.restype = i32
-    lib.frustum_register_batch_f32.argtypes = [vp, vp, i32, i32, i32, i32, _c.c_uint64, f64, f64, vp, vp, vp, f64, f64,
-                                               i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    eval_args = [vp, vp, vp, i32, vp, vp, f64, f64, i32, i32, vp, vp, vp, vp, sz, vp]
-    for name in ("frustum_evaluate_f32", "frustum_evaluate_f64"):
-        getattr(lib, name).restype = i32
-        getattr(lib, name).argtypes = eval_args
-    res_args = [vp, vp, i32, i32, vp, vp, f64, f64, i32, vp, vp, vp]
-    for name in ("frustum_residuals_f32", "frustum_residuals_f64"):
-        getattr(lib, name).restype = i32
-        getattr(lib, name).argtypes = res_args
-    lib.frustum_poly_roots_f64.restype = i32
-    lib.frustum_poly_roots_f64.argtypes = [vp, vp, i32, vp, vp]
-    lib.frustum_interp_step_f64.restype = i32
-    lib.frustum_interp_step_f64.argtypes = [vp, vp, i32, vp, vp]
-    lib.frustum_lm_next_step_f64.restype = i32
-    lib.frustum_lm_next_step_f64.argtypes = [i32, i32, vp, vp, vp, vp, vp]
-    lib.frustum_prepare_workspace_bytes.restype = sz
-    lib.frustum_prepare_workspace_bytes.argtypes = [i32, i32]
-    lib.frustum_prepare_batch_f32.restype = i32
-    lib.frustum_prepare_batch_f32.argtypes = [vp, vp, i32, i32, i32, i32, _c.c_uint64, f64, f64, i32,
-                                              vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    lib.frustum_sort_batch_f32.restype = i32
-    lib.frustum_sort_batch_f32.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp]
-    lib.frustum_inside_mask_f32.restype = i32
-    lib.frustum_inside_mask_f32.argtypes = [vp, vp, i32, vp, vp, f64, f64, i32, vp, vp]
-    lib.pose_error_batch.restype = i32
-    lib.pose_error_batch.argtypes = [vp, vp, i32, f64, f64, vp, vp, vp, vp]
-    lib.index_max_forward.restype = i32
-    lib.index_max_forward.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp]
-    lib.ball_query_xyz_workspace_bytes.restype = sz
-    lib.ball_query_xyz_workspace_bytes.argtypes = [i32, i32]
-    lib.ball_query_xyz_forward.restype = i32
-    lib.ball_query_xyz_forward.argtypes = [vp, vp, _c.c_float, vp, i32, i32, i32, i32, vp, sz, vp]
-    lib.cluster_assign_workspace_bytes.restype = sz
-    lib.cluster_assign_workspace_bytes.argtypes = [i32, i32]
-    lib.cluster_assign_forward.restype = i32
-    lib.cluster_assign_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    lib.ball_query_forward.restype = i32
-    lib.ball_query_forward.argtypes = [vp, _c.c_float, vp, i32, i32, i32, i32, vp]
-    lib.pnp_ransac_workspace_bytes.restype = sz
-    lib.pnp_ransac_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.pnp_ransac_batch_f32.restype = i32
-    lib.pnp_ransac_batch_f32.argtypes = [vp, vp, vp, vp, i32, i32, vp, f64, f64, f64, i32, f64, f64, _c.c_uint64,
-                                         vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    lib.epnp_batch_f64.restype = i32
-    lib.epnp_batch_f64.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp]
-    lib.icp_workspace_bytes.restype = sz
-    lib.icp_workspace_bytes.argtypes = [i32, i32, i32, i32]
-    lib.icp_register_batch_f32.restype = i32
-    lib.icp_register_batch_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, i32, f64, i32, f64, f64, i32,
-                                           vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    lib.icp_register_batch_counted_f32.restype = i32
-    lib.icp_register_batch_counted_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, i32, f64, i32, f64, f64, i32,
-                                                   vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    lib.icp_build_index_f32.restype = i32
-    lib.icp_build_index_f32.argtypes = [vp, vp, i32, i32, vp, sz, vp]
-    lib.voxel_downsample_workspace_bytes.restype = sz
-    lib.voxel_downsample_workspace_bytes.argtypes = [i32, i32, i32]
-    for name in ("voxel_downsample_batch_f32", "voxel_downsample_batch_f64"):
-        getattr(lib, name).restype = i32
-        getattr(lib, name).argtypes = [vp, vp, i32, i32, vp, i32, f64, vp, vp, vp, vp, sz, vp]
-    lib.estimate_normals_workspace_bytes.restype = sz
-    lib.estimate_normals_workspace_bytes.argtypes = [i32, i32]
-    lib.estimate_normals_batch_f32.restype = i32
-    lib.estimate_normals_batch_f32.argtypes = [vp, vp, i32, i32, f64, i32, vp, vp, vp, vp, sz, vp]
-    lib.nearest_batch_f32.restype = i32
-    lib.nearest_batch_f32.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp, vp, sz, vp]
-    lib.sym3_eig_batch_f64.restype = i32
-    lib.sym3_eig_batch_f64.argtypes = [vp, i32, vp, vp, vp]
-    lib.assemble_accumulate_workspace_bytes.restype = sz
-    lib.assemble_accumulate_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.assemble_accumulate_f32.restype = i32
-    lib.assemble_accumulate_f32.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp, vp, i32, vp, vp, sz,
-                                            vp]
-    lib.assemble_accumulate_gather_workspace_bytes.restype = sz
-    lib.assemble_accumulate_gather_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.assemble_accumulate_gather_f32.restype = i32
-    lib.assemble_accumulate_gather_f32.argtypes = [vp, vp, vp, _c.c_int64, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp,
-                                                   vp, i32, vp, vp, sz, vp]
-    lib.assemble_accumulate_f64_workspace_bytes.restype = sz
-    lib.assemble_accumulate_f64_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.assemble_accumulate_f64.restype = i32
-    lib.assemble_accumulate_f64.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, f64, vp, vp, vp, i32, vp, vp, sz, vp]
-    lib.assemble_resample_workspace_bytes.restype = sz
-    lib.assemble_resample_workspace_bytes.argtypes = [i32, i32]
-    lib.assemble_resample_f32.restype = i32
-    lib.assemble_resample_f32.argtypes = [vp, vp, vp, vp, i32, i32, i32, _c.c_uint64, vp, f64, f64, i32, vp, vp, vp,
-                                          vp, vp, sz, vp]
-    lib.assemble_candidates_workspace_bytes.restype = sz
-    lib.assemble_candidates_workspace_bytes.argtypes = [i32, i32]
-    lib.assemble_candidates_f32.restype = i32
-    lib.assemble_candidates_f32.argtypes = [vp, i32, i32, _c.c_uint64, i32, i32, vp, vp, vp, sz, vp]
-    for name in ("fps_batch_f32", "fps_batch_f64"):
-        getattr(lib, name).restype = i32
-        getattr(lib, name).argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp]
-    lib.interp_weights_f32.restype = i32
-    lib.interp_weights_f32.argtypes = [vp, i32, vp, vp, i32, i32, i32, i32, vp, vp, vp]
-    lib.interp_forward_f32.restype = i32
-    lib.interp_forward_f32.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp]
-    lib.interp_backward_workspace_bytes.restype = sz
-    lib.interp_backward_workspace_bytes.argtypes = [i32, i32, i32, i32]
-    lib.interp_backward_f32.restype = i32
-    lib.interp_backward_f32.argtypes = [vp, _c.c_int64, vp, vp, i32, i32, i32, i32, i32, vp, vp, sz, vp]
-    lib.image_assemble_workspace_bytes.restype = sz
-    lib.image_assemble_workspace_bytes.argtypes = [i32, i32, i32]
-    for name in ("image_assemble_f32", "image_assemble_u8"):
-        getattr(lib, name).restype = i32
-        getattr(lib, name).argtypes = [vp, sz, vp, vp, vp, i32, i32, i32, vp, vp, sz, vp]
-    lib.classifier_loss_workspace_bytes.restype = sz
-    lib.classifier_loss_workspace_bytes.argtypes = [i32, i32]
-    lib.classifier_loss_forward_f32.restype = i32
-    lib.classifier_loss_forward_f32.argtypes = [vp, _c.c_int64, vp, _c.c_int64, i32, vp, vp, vp, i32, i32, f64, f64,
-                                                f64, i32, i32, f64, f64, i32, f64, vp, vp, vp, vp, vp, vp, vp, vp, vp,
-                                                vp, vp, vp, vp, vp, sz, vp]
-    lib.classifier_loss_backward_f32.restype = i32
-    lib.classifier_loss_backward_f32.argtypes = [vp, _c.c_int64, vp, _c.c_int64, i32, i32, i32, vp, vp, vp, vp, vp, vp,
-                                                 vp, f64, f64, i32, f64, vp, vp, vp]
-    lib.cluster_pool_forward_f32.restype = i32
-    lib.cluster_pool_forward_f32.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp]
-    lib.cluster_pool_backward_workspace_bytes.restype = sz
-    lib.cluster_pool_backward_workspace_bytes.argtypes = [i32, i32, i32, i32]
-    lib.cluster_pool_backward_f32.restype = i32
-    lib.cluster_pool_backward_f32.argtypes = [vp, vp, _c.c_int64, vp, vp, vp, i32, i32, i32, i32, vp, vp, sz, vp]
-    lib.knn_group_forward_f32.restype = i32
-    lib.knn_group_forward_f32.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
-    lib.knn_group_backward_workspace_bytes.restype = sz
-    lib.knn_group_backward_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
-    lib.knn_group_backward_f32.restype = i32
-    lib.knn_group_backward_f32.argtypes = [vp, _c.c_int64, vp, i32, i32, i32, i32, i32, vp, vp, sz, vp]
-    lib.attn_fusion_forward_f32.restype = i32
-    lib.attn_fusion_forward_f32.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp]
-    lib.attn_fusion_backward_f32.restype = i32
-    lib.attn_fusion_backward_f32.argtypes = [vp, _c.c_int64, vp, vp, i32, i32, i32, i32, vp, vp, vp]
-    lib.jpeg_decode_workspace_bytes.restype = sz
-    lib.jpeg_decode_workspace_bytes.argtypes = [vp, i32, sz, i32]
-    lib.jpeg_decode_batch_u8.restype = i32
-    lib.jpeg_decode_batch_u8.argtypes = [vp, sz, vp, vp, vp, i32, i32, vp, sz, vp, vp, sz, vp]
-    lib.pointwise_mlp_packed_bytes.restype = sz
-    lib.pointwise_mlp_packed_bytes.argtypes = [vp, i32, vp, i32]
-    lib.pointwise_mlp_pack_f32.restype = i32
-    lib.pointwise_mlp_pack_f32.argtypes = [vp, i32, vp, i32, vp, sz, vp]
-    lib.pointwise_mlp_workspace_bytes.restype = sz
-    lib.pointwise_mlp_workspace_bytes.argtypes = [vp, i32, vp, i32, i32]
-    lib.pointwise_mlp_f32.restype = i32
-    lib.pointwise_mlp_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, i32, vp, vp, vp, vp, sz, vp]
-    lib.knn_fusion_packed_bytes.restype = sz
-    lib.knn_fusion_packed_bytes.argtypes = [i32, vp, i32, i32]
-    lib.knn_fusion_pack_f32.restype = i32
-    lib.knn_fusion_pack_f32.argtypes = [i32, vp, i32, i32, vp, sz, vp]
-    lib.knn_fusion_f32.restype = i32
-    lib.knn_fusion_f32.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, sz, vp, vp, vp]
-    lib.pointwise_mlp_max_packed_bytes.restype = sz
-    lib.pointwise_mlp_max_packed_bytes.argtypes = [i32, vp, i32]
-    lib.pointwise_mlp_max_pack_f32.restype = i32
-    lib.pointwise_mlp_max_pack_f32.argtypes = [i32, vp, i32, vp, sz, vp]
-    lib.pointwise_mlp_max_workspace_bytes.restype = sz
-    lib.pointwise_mlp_max_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.pointwise_mlp_max_f32.restype = i32
-    lib.pointwise_mlp_max_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, vp, vp, sz, vp]
-    lib.node_mlp_packed_bytes.restype = sz
-    lib.node_mlp_packed_bytes.argtypes = [vp, i32, vp, i32]
-    lib.node_mlp_pack_f32.restype = i32
-    lib.node_mlp_pack_f32.argtypes = [vp, i32, vp, i32, vp, sz, vp]
-    lib.node_mlp_workspace_bytes.restype = sz
-    lib.node_mlp_workspace_bytes.argtypes = [vp, i32, vp, i32, i32]
-    lib.node_mlp_f32.restype = i32
-    lib.node_mlp_f32.argtypes = [vp, i32, vp, i32, vp, sz, i32, i32, vp, vp, sz, vp]
-    lib.resnet_conv_packed_bytes.restype = sz
-    lib.resnet_conv_packed_bytes.argtypes = [i32, i32]
-    lib.resnet_conv_pack_f32.restype = i32
-    lib.resnet_conv_pack_f32.argtypes = [vp, i32, i32, vp, sz, vp]
-    lib.resnet_conv_f32.restype = i32
-    lib.resnet_conv_f32.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, sz, vp, vp,
-                                    i32, i32, vp, vp, vp]
-    lib.resnet_maxpool_f32.restype = i32
-    lib.resnet_maxpool_f32.argtypes = [vp, i32, i32, i32, i32, vp, vp]
-    lib.resnet_mean_f32.restype = i32
-    lib.resnet_mean_f32.argtypes = [vp, i32, i32, vp, vp]
-    lib.monodepth_resize_f32.restype = i32
-    lib.monodepth_resize_f32.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, i32, _c.c_float, _c.c_float,
-                                         vp, sz, vp, vp]
-    lib.monodepth_cloud_workspace_bytes.restype = sz
-    lib.monodepth_cloud_workspace_bytes.argtypes = [i32, i32, i32]
-    lib.monodepth_cloud_f32.restype = i32
-    lib.monodepth_cloud_f32.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, sz,
-                                        vp]
-    lib.png_decode_workspace_bytes.restype = sz
-    lib.png_decode_workspace_bytes.argtypes = [vp, i32, vp, i32, sz]
-    lib.png_decode_batch_u8.restype = i32
-    lib.png_decode_batch_u8.argtypes = [vp, sz, vp, i32, vp, i32, vp, sz, vp, vp, sz, vp]
-    i64 = _c.c_int64
-    lib.oxford_build_plan_f64.restype = i32
-    lib.oxford_build_plan_f64.argtypes = [vp, vp, i64, vp, vp, i32, vp, f64, i32, vp, vp, vp, vp, vp]
-    lib.oxford_build_count_workspace_bytes.restype = sz
-    lib.oxford_build_count_workspace_bytes.argtypes = [i32, i32]
-    lib.oxford_build_count_f64.restype = i32
-    lib.oxford_build_count_f64.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, f64, vp, vp, vp, vp, sz, vp]
-    lib.oxford_build_scatter_f64.restype = i32
-    lib.oxford_build_scatter_f64.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f64, i32, vp, vp, vp]
-    lib.oxford_build_pack_f32.restype = i32
-    lib.oxford_build_pack_f32.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, vp, vp]
-    lib.oxford_debayer_workspace_bytes.restype = sz
-    lib.oxford_debayer_workspace_bytes.argtypes = [i32]
-    lib.oxford_debayer_undistort_u8.restype = i32
-    lib.oxford_debayer_undistort_u8.argtypes = [vp, sz, vp, i64, vp, i32, vp, sz, vp, sz, vp]
-    lib.jpeg_encode_workspace_bytes.restype = sz
-    lib.jpeg_encode_workspace_bytes.argtypes = [vp, i32]
-    lib.jpeg_encode_entropy_u8.restype = i32
-    lib.jpeg_encode_entropy_u8.argtypes = [vp, sz, vp, i32, vp, vp, vp, vp, sz, vp]
-    lib.jpeg_encode_stuff_u8.restype = i32
-    lib.jpeg_encode_stuff_u8.argtypes = [vp, i32, vp, vp, sz, vp, sz, vp]
-    lib.nuscenes_walk_count.restype = i32
-    lib.nuscenes_walk_count.argtypes = [vp, vp, vp, i64, vp, vp, i32, f64, vp, vp, vp]
-    lib.nuscenes_walk_scan_workspace_bytes.restype = sz
-    lib.nuscenes_walk_scan_workspace_bytes.argtypes = [i32]
-    lib.nuscenes_walk_scan.restype = i32
-    lib.nuscenes_walk_scan.argtypes = [vp, i32, vp, vp, sz, vp]
-    lib.nuscenes_walk_fill.restype = i32
-    lib.nuscenes_walk_fill.argtypes = [vp, vp, vp, i64, vp, vp, i32, f64, vp, vp, vp]
-    lib.kitti_build_count_workspace_bytes.restype = sz
-    lib.kitti_build_count_workspace_bytes.argtypes = [i32]
-    lib.kitti_build_count_f32.restype = i32
-    lib.kitti_build_count_f32.argtypes = [vp, i64, vp, vp, i32, vp, i32, vp, vp, vp, vp, vp, sz, vp]
-    lib.kitti_build_scatter_f64.restype = i32
-    lib.kitti_build_scatter_f64.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, vp]
-    lib.kitti_build_finish_f32.restype = i32
-    lib.kitti_build_finish_f32.argtypes = [vp, vp, vp, vp, i32, f64, i64, i64, vp, vp, vp]
+    for name, (restype, argtypes) in sigs.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 

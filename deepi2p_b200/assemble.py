@@ -15,7 +15,8 @@ import numpy as np
 import torch
 
 from . import _native
-from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace, round_up
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _ws_cache, round_up
 from .icp import _check
 from . import pointprep
 
@@ -204,12 +205,12 @@ def accumulate(xyz, intensity, sn, n_pts, frame_sample, frame_T, range_max=None,
         cnt = torch.zeros((S,), dtype=torch.int32, device=dev)
         sp = _stream_ptr(stream)
         if f64:
-            ws = _workspace(lib.assemble_accumulate_f64_workspace_bytes(T, n, S), dev, sp)
+            ws = _workspace(_ws_cache, lib.assemble_accumulate_f64_workspace_bytes(T, n, S), dev, stream)
             rc = lib.assemble_accumulate_f64(_ptr(xyz), _ptr(intensity), _ptr(n_d), n, T, _ptr(fs_d), _ptr(FT_d), S, r,
                                              None if box is None else box.ctypes.data_as(_native._c.c_void_p),
                                              _ptr(out_x), _ptr(out_i), A, _ptr(cnt), _ptr(ws), ws.numel(), sp)
         else:
-            ws = _workspace(lib.assemble_accumulate_workspace_bytes(T, n, S), dev, sp)
+            ws = _workspace(_ws_cache, lib.assemble_accumulate_workspace_bytes(T, n, S), dev, stream)
             rc = lib.assemble_accumulate_f32(_ptr(xyz), _ptr(intensity), _ptr(sn), _ptr(n_d), n, T, _ptr(fs_d),
                                              _ptr(FT_d), S, r, _ptr(out_x), _ptr(out_i), _ptr(out_n), A, _ptr(cnt),
                                              _ptr(ws), ws.numel(), sp)
@@ -399,7 +400,7 @@ def accumulate_gather(frames, range_max=None, stream=None):
         out_n = torch.zeros((S, 3, A), dtype=torch.float32, device=dev) if st.has_sn else None
         cnt = torch.zeros((S,), dtype=torch.int32, device=dev)
         sp = _stream_ptr(stream)
-        ws = _workspace(lib.assemble_accumulate_gather_workspace_bytes(T, n_max, S), dev, sp)
+        ws = _workspace(_ws_cache, lib.assemble_accumulate_gather_workspace_bytes(T, n_max, S), dev, stream)
         px, pi, pn = st.plane_ptrs()
         rc = lib.assemble_accumulate_gather_f32(px, pi, pn or None, st.data.stride(0), _ptr(off_d), _ptr(n_d), n_max,
                                                 T, _ptr(fs_d), _ptr(FT_d), S, r, _ptr(out_x), _ptr(out_i),
@@ -473,7 +474,7 @@ def resample(xyz, intensity, sn, n_pts, N, seed, M=None, jitter=(), sigma=SIGMA,
                    sn=torch.empty((S, 3, N), dtype=torch.float32, device=dev),
                    src=torch.empty((S, N), dtype=torch.int32, device=dev))
         sp = _stream_ptr(stream)
-        ws = _workspace(lib.assemble_resample_workspace_bytes(S, A), dev, sp)
+        ws = _workspace(_ws_cache, lib.assemble_resample_workspace_bytes(S, A), dev, stream)
         rc = lib.assemble_resample_f32(_ptr(xyz), _ptr(intensity), _ptr(sn), _ptr(n_pts), A, S, N,
                                        int(seed) & (2**64 - 1), _ptr(M_d), float(sigma), float(clip), mask,
                                        _ptr(res["pc"]), _ptr(res["intensity"]), _ptr(res["sn"]), _ptr(res["src"]),
@@ -498,7 +499,7 @@ def candidates(pc, m, seed, node_set, stream=None):
         idx = torch.empty((S, m), dtype=torch.int32, device=dev)
         xyz = torch.empty((S, 3, m), dtype=torch.float32, device=dev)
         sp = _stream_ptr(stream)
-        ws = _workspace(lib.assemble_candidates_workspace_bytes(S, N), dev, sp)
+        ws = _workspace(_ws_cache, lib.assemble_candidates_workspace_bytes(S, N), dev, stream)
         rc = lib.assemble_candidates_f32(_ptr(pc), N, S, int(seed) & (2**64 - 1), int(node_set), int(m), _ptr(idx),
                                          _ptr(xyz), _ptr(ws), ws.numel(), sp)
     _native.check(rc, "assemble_candidates")

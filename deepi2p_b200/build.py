@@ -4,6 +4,7 @@
 
 nvcc cross-compiles without a GPU.  The .so is git-ignored but travels with the working tree.
 """
+import glob
 import os
 import shutil
 import subprocess
@@ -13,10 +14,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdeepi2p_b200.so")
-SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "ball_query_xyz.cu", "cluster_assign.cu",
-           "pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu", "classifier_loss.cu",
-           "encoder_ops.cu", "fusion.cu", "jpeg.cu", "png.cu", "pointwise_mlp.cu", "oxford_build.cu", "oxford_images.cu",
-           "jpeg_encode.cu", "knn_fusion.cu", "node_mlp.cu", "nuscenes_build.cu", "kitti_build.cu", "resnet.cu", "monodepth.cu"]
+HEADER = os.path.join(os.path.dirname(HERE), "include", "deepi2p_b200.h")
+# Every .cu of csrc/ is a translation unit of the library (named by file, as NOFMA_SOURCES names them); every header
+# of csrc/ and the public header are dependencies.
+SOURCES = sorted(os.path.basename(p) for p in glob.glob(os.path.join(CSRC, "*.cu")))
+HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [HEADER]
 # Compiled on their own without FMA contraction: oracle_pnp/pnp_oracle.cpp, oracle_icp/icp_oracle.cpp and
 # oracle_prep/prep_oracle.cpp, oracle_assemble/, oracle_interp/, oracle_image/ and oracle.pose_diff_restated (metrics.cu)
 # restate their arithmetic bit for bit (oracle_oxford_build/, oracle_oxford_images/ and oracle_kitti_build/ too); metrics.cu and
@@ -24,7 +26,7 @@ SOURCES = ["frustum_solver.cu", "prepare.cu", "point_ops.cu", "metrics.cu", "bal
 # kernel with __fmaf_rn and keeps the back-projection to plain products and sums (DESIGN.md 4.31).
 NOFMA_SOURCES = ["pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu", "metrics.cu",
                  "classifier_loss.cu", "oxford_build.cu", "oxford_images.cu", "kitti_build.cu", "monodepth.cu"]
-HEADERS = ["common.cuh", "morton_index.cuh", "sym3_eig.cuh", "project.cuh", "nearest_k.cuh", "tf32_mma.cuh", os.path.join("..", "..", "include", "deepi2p_b200.h")]
+assert set(NOFMA_SOURCES) <= set(SOURCES), set(NOFMA_SOURCES) - set(SOURCES)
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -48,7 +50,7 @@ def is_stale():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS] + [os.path.abspath(__file__)]
+    deps = [os.path.join(CSRC, s) for s in SOURCES] + HEADERS + [os.path.abspath(__file__)]
     return any(os.path.exists(d) and os.path.getmtime(d) > t for d in deps)
 
 
@@ -83,7 +85,7 @@ def build(force=False, verbose=False, extra=(), out=None):
     if not force and not is_stale():
         return LIB
     os.makedirs(LIBDIR, exist_ok=True)
-    srcs = [os.path.join(CSRC, s) for s in SOURCES if s not in NOFMA_SOURCES and os.path.exists(os.path.join(CSRC, s))]
+    srcs = [os.path.join(CSRC, s) for s in SOURCES if s not in NOFMA_SOURCES]
     srcs += _nofma_objects(LIBDIR, extra, verbose)
     env_extra = os.environ.get("DIB_NVCC_EXTRA", "").split()
     cmd = [nvcc_path(), *NVCC_FLAGS, *extra, *env_extra, "-o", LIB + ".tmp", *srcs]

@@ -12,6 +12,7 @@ import numbers
 import torch
 
 from . import _native
+from ._native import _ptr, _stream_ptr
 
 
 def fine_grid(H, W, fine_scale):
@@ -87,10 +88,6 @@ def _scores_view(t):
     return t, (t.stride(0) if B > 1 else 0)
 
 
-def _ptr(t):
-    return t.data_ptr() if t is not None else None
-
-
 class _ClassifierLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, coarse_scores, fine_scores, pc, P12, K9, cfg, extras):
@@ -120,7 +117,7 @@ class _ClassifierLoss(torch.autograd.Function):
                 coarse_labels.data_ptr(), _ptr(fine_labels), coarse_pred.data_ptr(), _ptr(fine_pred), _ptr(lse),
                 loss.data_ptr(), coarse_loss.data_ptr(), fine_loss.data_ptr(), accuracy.data_ptr(),
                 n_inside.data_ptr(), coarse_correct.data_ptr(), _ptr(fine_correct), n_inside_total.data_ptr(),
-                ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
+                ws.data_ptr(), ws.numel(), _stream_ptr())
         _native.check(rc, "classifier_loss_forward_f32")
         extras.update(coarse_labels=coarse_labels, fine_labels=fine_labels, coarse_predictions=coarse_pred,
                       fine_predictions=fine_pred, n_inside=n_inside, coarse_accuracy=accuracy[0],
@@ -148,8 +145,7 @@ class _ClassifierLoss(torch.autograd.Function):
             rc = lib.classifier_loss_backward_f32(
                 coarse.data_ptr(), cbs, _ptr(fine), fbs, L, B, N, coarse_labels.data_ptr(), _ptr(fine_labels),
                 _ptr(lse), n_inside_total.data_ptr(), g_loss.data_ptr(), g_coarse.data_ptr(), g_fine.data_ptr(),
-                float(coarse_alpha), float(focal_alpha), gamma, float(eps), _ptr(gc), _ptr(gf),
-                torch.cuda.current_stream().cuda_stream)
+                float(coarse_alpha), float(focal_alpha), gamma, float(eps), _ptr(gc), _ptr(gf), _stream_ptr())
         _native.check(rc, "classifier_loss_backward_f32")
         return gc, gf, None, None, None, None, None
 

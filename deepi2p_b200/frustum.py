@@ -16,6 +16,7 @@ import numpy as np
 import torch
 
 from . import _native
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
 
 DEFAULT_T_LB = (-5.0, -0.1, -10.0)      # registration_lsq.py:340
 DEFAULT_T_UB = (5.0, 0.1, 10.0)
@@ -23,20 +24,6 @@ RY_SIGMA = 10.0 * math.pi / 180.0       # registration_lsq.py:339
 T_AMPLITUDE = 10.0                      # registration_lsq.py:337
 TERMINATION = ("gradient_tolerance", "parameter_tolerance", "function_tolerance", "max_iterations",
                "min_trust_region_radius", "invalid_steps", "infeasible_start")
-
-
-def _require_cuda():
-    if not torch.cuda.is_available():
-        raise _native.NativeError("deepi2p_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
-
-
-def _stream_ptr(stream=None):
-    s = stream if stream is not None else torch.cuda.current_stream()
-    return s.cuda_stream
-
-
-def _ptr(t):
-    return 0 if t is None else t.data_ptr()
 
 
 def round_up(n, m):
@@ -108,18 +95,7 @@ def _check_cloud(xyz, label=None, n_pts=None, what="xyz", dtypes=(torch.float32,
     return S, Ns
 
 
-_ws_cache = {}
-
-
-def _workspace(nbytes, device, stream_ptr=0):
-    """Scratch buffer of the solver, cached per (device, stream): launches on different streams may overlap, so
-    they must not share a workspace; launches on one stream are ordered and can."""
-    key = (device.index if device.index is not None else torch.cuda.current_device(), int(stream_ptr))
-    buf = _ws_cache.get(key)
-    if buf is None or buf.numel() < nbytes:
-        buf = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8, device=device)
-        _ws_cache[key] = buf
-    return buf
+_ws_cache = {}      # scratch of the solver, shared with the other wrappers that launch on its streams (1 MiB floor)
 
 
 def last_solve_timeline(device=None, stream=None, register_shape=None):
@@ -205,7 +181,7 @@ def solve_batch(xyz, label, n_pts, K, init, H, W, t_lb=DEFAULT_T_LB, t_ub=DEFAUL
                 stats = torch.empty((S, I, 4), dtype=torch.int32, device=dev)
         wsb = lib.frustum_solve_workspace_bytes(S, I, Ns)
         sp = _stream_ptr(stream)
-        ws = _workspace(wsb, dev, sp)
+        ws = _workspace(_ws_cache, wsb, dev, stream)
         trace = None
         if trace_cap > 0:
             if xyz.dtype != torch.float32:
@@ -248,7 +224,7 @@ def evaluate_batch(xyz, label, n_pts, K, x, H, W, is_2d=True, stream=None, slice
         grad = torch.empty((S, 6), dtype=torch.float64, device=dev)
         JtJ = torch.empty((S, 36), dtype=torch.float64, device=dev)
         sp = _stream_ptr(stream)
-        ws = _workspace(lib.frustum_evaluate_workspace_bytes(S, Ns), dev, sp)
+        ws = _workspace(_ws_cache, lib.frustum_evaluate_workspace_bytes(S, Ns), dev, stream)
         fn = lib.frustum_evaluate_f32 if xyz.dtype == torch.float32 else lib.frustum_evaluate_f64
         rc = fn(_ptr(xyz), _ptr(label), _ptr(n_pts), Ns, _ptr(K9), _ptr(x), float(H), float(W), 1 if is_2d else 0, S,
                 _ptr(cost), _ptr(grad), _ptr(JtJ), _ptr(ws), ws.numel(), sp)
@@ -384,7 +360,7 @@ def register_batch(xyz_in, pred, n_in, K, H, W, n_inits=60, seed=0, t_lb=DEFAULT
                            costs=torch.empty((S, I), dtype=torch.float64, device=dev),
                            stats=torch.empty((S, I, 4), dtype=torch.int32, device=dev))
         sp = _stream_ptr(stream)
-        ws = _workspace(lib.frustum_register_workspace_bytes(S, I, n_in), dev, sp)
+        ws = _workspace(_ws_cache, lib.frustum_register_workspace_bytes(S, I, n_in), dev, stream)
         rc = lib.frustum_register_batch_f32(
             _ptr(xyz_in), _ptr(pred), n_in, Ns_in, S, I, int(seed), float(RY_SIGMA), float(T_AMPLITUDE), _ptr(K9),
             lb.ctypes.data, ub.ctypes.data, float(H), float(W), int(max_iter), 1 if is_2d else 0, _ptr(res["P"]),

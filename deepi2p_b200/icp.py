@@ -14,7 +14,8 @@ import numpy as np
 import torch
 
 from . import _native, synthetic
-from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace, round_up
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _ws_cache, round_up
 
 MAX_CORR_DIST = 1.0            # registration_icp.py:148
 MAX_ITERATION = 30             # Open3D ICPConvergenceCriteria defaults
@@ -83,7 +84,7 @@ def icp_register_batch(src, n_pts, tgt, m_pts, init, max_corr_dist=MAX_CORR_DIST
         else:
             res = {k: torch.empty(shp, dtype=dt, device=dev) for k, (shp, dt) in shapes.items()}
         sp = _stream_ptr(stream)
-        ws = _workspace(max(lib.icp_workspace_bytes(S, max(I, 1), Ns, max(Ms, 16)), 1), dev, sp)
+        ws = _workspace(_ws_cache, max(lib.icp_workspace_bytes(S, max(I, 1), Ns, max(Ms, 16)), 1), dev, stream)
         args = (_ptr(src), _ptr(n_pts), Ns, _ptr(tgt), _ptr(m_pts), Ms, S, _ptr(init), I, float(max_corr_dist),
                 int(max_iteration), float(relative_fitness), float(relative_rmse), int(bool(force_2d)), _ptr(res["P"]),
                 _ptr(res["fitness"]), _ptr(res["best"]), _ptr(res.get("T")), _ptr(res.get("fitness_all")),
@@ -188,7 +189,7 @@ def build_index(tgt, m_pts=None, stream=None):
         _check(m_pts, "m_pts", torch.int32, (S,), tgt.device)
     with torch.cuda.device(tgt.device):
         sp = _stream_ptr(stream)
-        ws = _workspace(max(lib.icp_workspace_bytes(S, 1, 16, max(Ms, 16)), 1), tgt.device, sp)
+        ws = _workspace(_ws_cache, max(lib.icp_workspace_bytes(S, 1, 16, max(Ms, 16)), 1), tgt.device, stream)
         rc = lib.icp_build_index_f32(_ptr(tgt), _ptr(m_pts), Ms, S, _ptr(ws), ws.numel(), sp)
     _native.check(rc, "icp_build_index")
 

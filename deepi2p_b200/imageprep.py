@@ -22,7 +22,8 @@ from . import jpeg as _jpeg
 from . import jpeg_encode as _jpege
 from . import png as _png
 from .assemble import MODES
-from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _ws_cache
 
 _JPEGE_DESC = 8                   # include/deepi2p_b200.h DIB_JPEGE_DESC
 IMAGE_PARAMS = 16                 # include/deepi2p_b200.h DIB_IMAGE_PARAMS and the DIB_IMG_* slots below
@@ -114,7 +115,7 @@ def decode_jpeg_batch(blobs, device="cuda", stream=None, *, _window_bits=None):
             nws = lib.jpeg_decode_workspace_bytes(desc.ctypes.data, S, pk["data"].size, wb)
             if nws == 0:
                 raise _native.NativeError("jpeg_decode_workspace_bytes rejected the batch")
-            ws = _workspace(nws, dev, sp)
+            ws = _workspace(_ws_cache, nws, dev, stream)
             rc = lib.jpeg_decode_batch_u8(_ptr(data), pk["data"].size, desc.ctypes.data, _ptr(huff), _ptr(quant), S, wb,
                                           _ptr(out), out.numel(), _ptr(status), _ptr(ws), ws.numel(), sp)
             _native.check(rc, "jpeg_decode")
@@ -185,7 +186,7 @@ def _decode_png(blobs, device, stream, grey):
             nws = lib.png_decode_workspace_bytes(desc.ctypes.data, S, chunks.ctypes.data, len(chunks), data.numel())
             if nws == 0:
                 raise _native.NativeError("png_decode_workspace_bytes rejected the batch")
-            ws = _workspace(nws, dev, sp)
+            ws = _workspace(_ws_cache, nws, dev, stream)
             rc = lib.png_decode_batch_u8(_ptr(data), data.numel(), desc.ctypes.data, S, chunks.ctypes.data,
                                          len(chunks), _ptr(out), out.numel(), _ptr(status), _ptr(ws), ws.numel(), sp)
             _native.check(rc, "png_decode")
@@ -245,7 +246,7 @@ def encode_jpeg_batch(images, quality=95, stream=None):
         nws = lib.jpeg_encode_workspace_bytes(desc.ctypes.data, S)
         if nws == 0:
             raise _native.NativeError("jpeg_encode_workspace_bytes rejected the batch")
-        ws = _workspace(nws, dev, sp)
+        ws = _workspace(_ws_cache, nws, dev, stream)
         counts = torch.empty((S, 2), dtype=torch.int64, device=dev)
         rc = lib.jpeg_encode_entropy_u8(_ptr(data), data.numel(), desc.ctypes.data, S, quant.ctypes.data,
                                         huff.ctypes.data, _ptr(counts), _ptr(ws), ws.numel(), sp)
@@ -407,7 +408,7 @@ def assemble_images(images, K, mode="train", params=None, rng=None, flip=None, o
         img = torch.empty((S, 3, H, W), dtype=out_dtype, device=dev)
         if S:
             sp = _stream_ptr(stream)
-            ws = _workspace(lib.image_assemble_workspace_bytes(S, H, W), dev, sp)
+            ws = _workspace(_ws_cache, lib.image_assemble_workspace_bytes(S, H, W), dev, stream)
             fn = lib.image_assemble_f32 if out_dtype == torch.float32 else lib.image_assemble_u8
             rc = fn(_ptr(data), data.numel(), offsets.ctypes.data, P.ctypes.data, factors.ctypes.data, S, H, W,
                     _ptr(img), _ptr(ws), ws.numel(), sp)

@@ -19,7 +19,8 @@ import numpy as np
 import torch
 
 from . import _native, assemble, kitti, pointprep
-from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace, round_up
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _ws_cache, round_up
 
 # frame_accumulation.py main(): the parameters the published records were written with
 FRAME_STRIDE_DIST = 4
@@ -159,7 +160,7 @@ def build_frames(store, ids, first, P, voxel_size=VOXEL_SIZE, accumulate_radius=
         pos = torch.zeros((max(T, 1),), dtype=torch.int64, device=dev)
         n_pts = torch.zeros((B,), dtype=torch.int64, device=dev)
         imax = torch.zeros((B,), dtype=torch.float32, device=dev)
-        ws = _workspace(max(lib.kitti_build_count_workspace_bytes(T), 1), dev, sp)
+        ws = _workspace(_ws_cache, max(lib.kitti_build_count_workspace_bytes(T), 1), dev, stream)
         rc = lib.kitti_build_count_f32(planes, ps, _ptr(off_d), _ptr(n_d), T, _ptr(first_d), B,
                                        b.ctypes.data_as(_native._c.c_void_p), _ptr(pos), _ptr(n_pts), _ptr(imax),
                                        _ptr(ws), ws.numel(), sp)

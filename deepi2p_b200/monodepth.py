@@ -28,7 +28,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _native
-from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _ws_cache
 from .network import _BasicBlock
 
 PRECISION_BITS = 22                      # Pillow's Resample.c, 8 bits per channel
@@ -214,7 +215,7 @@ def resize_normalise(images, feed_height, feed_width, stream=None):
         out = torch.empty((S, 3, feed_height, feed_width), dtype=torch.float32, device=dev)
         tmp = None
         if tx is not None and ty is not None:
-            tmp = _workspace(S * h * feed_width * 3, dev, sp)
+            tmp = _workspace(_ws_cache, S * h * feed_width * 3, dev, stream)
         rc = lib.monodepth_resize_f32(_ptr(data), _ptr(off), S, h, w, feed_height, feed_width, _ptr(tx),
                                       0 if tx is None else tx.shape[1] - 2, _ptr(ty),
                                       0 if ty is None else ty.shape[1] - 2, float(FEED_SUB), float(FEED_MUL),
@@ -286,7 +287,7 @@ def depth_clouds(model, images, K_inv, *, src=None, n_pts=None, P_gt=None, K=Non
             K_d = _dev_f64(K, (S, 9), dev, "K")
             res["scale"] = torch.empty((S,), dtype=torch.float64, device=dev)
             res["tgt"] = torch.empty((S, 3, H * W), dtype=torch.float32, device=dev)
-            ws = _workspace(lib.monodepth_cloud_workspace_bytes(S, H, W), dev, sp)
+            ws = _workspace(_ws_cache, lib.monodepth_cloud_workspace_bytes(S, H, W), dev, stream)
         if not res:
             raise ValueError("no output requested")
         rc = lib.monodepth_cloud_f32(_ptr(disp), S, disp.shape[2], disp.shape[3], H, W, _ptr(ki),

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _native
-from .frustum import _ptr, _require_cuda
+from ._native import _ptr, _require_cuda
 from .nuscenes import CAMERAS, P_from_record
 
 LIDAR = "LIDAR_TOP"

@@ -18,7 +18,8 @@ import numpy as np
 import torch
 
 from . import _native, oxford, pointprep
-from .frustum import _ptr, _require_cuda, _stream_ptr, round_up
+from ._native import _ptr, _require_cuda, _stream_ptr
+from .frustum import round_up
 
 LMS_HZ = 50                                 # build_dataset.py:285, the LMS-front scan rate the velocity rule assumes
 PARAMS = dict(pc_sample_distance=2.0, min_vehicle_velocity=0.2, accumulation_distance=100.0, ignore_first_n_second=20,

@@ -15,7 +15,8 @@ import numpy as np
 import torch
 
 from . import _native
-from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _ws_cache
 from .imageprep import decode_grey_png_batch, encode_jpeg_batch
 
 LUT_FILE = "stereo_narrow_left_distortion_lut.bin"    # <sdk>/models/, the stereo centre camera's undistortion LUT
@@ -99,7 +100,7 @@ def debayer_undistort_batch(grey, lut, pattern=PATTERN, stream=None):
             desc[:, 0], desc[:, 1], desc[:, 2], desc[:, 3], desc[:, 4] = offsets, out_off, shapes[:, 0], \
                 shapes[:, 1], lut_off
             sp = _stream_ptr(stream)
-            ws = _workspace(lib.oxford_debayer_workspace_bytes(S), dev, sp)
+            ws = _workspace(_ws_cache, lib.oxford_debayer_workspace_bytes(S), dev, stream)
             rc = lib.oxford_debayer_undistort_u8(_ptr(data), data.numel(), _ptr(table), table.shape[0],
                                                  desc.ctypes.data, S, _ptr(out), out.numel(), _ptr(ws), ws.numel(),
                                                  sp)

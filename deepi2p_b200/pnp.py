@@ -9,7 +9,8 @@ import numpy as np
 import torch
 
 from . import _native
-from .frustum import _as_K, _ptr, _require_cuda, _stream_ptr, _workspace, round_up
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _as_K, _ws_cache, round_up
 
 SOLVEPNP_EPNP = 1          # the value of cv2.SOLVEPNP_EPNP, the only method implemented
 
@@ -69,7 +70,7 @@ def pnp_ransac_batch(xyz, coarse_pred, fine_pred, n_pts, K, H, W, scale=1 / 32.0
                     res["hyp_pose"].zero_()
                     res["hyp_inliers"].zero_()
         sp = _stream_ptr(stream)
-        ws = _workspace(max(lib.pnp_ransac_workspace_bytes(S, Ns, max(iterations, 1)), 1), dev, sp)
+        ws = _workspace(_ws_cache, max(lib.pnp_ransac_workspace_bytes(S, Ns, max(iterations, 1)), 1), dev, stream)
         rc = lib.pnp_ransac_batch_f32(
             _ptr(xyz), _ptr(coarse_pred), _ptr(fine_pred), _ptr(n_pts), Ns, S, _ptr(K9), float(H), float(W),
             float(scale), iterations, float(reproj_err), float(confidence), int(seed) & 0xFFFFFFFFFFFFFFFF,

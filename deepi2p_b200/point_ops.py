@@ -9,6 +9,7 @@ stream (SURVEY.md 8b).
 import torch
 
 from . import _native
+from ._native import _stream_ptr, _workspace
 
 
 def _check_input(t, name, dtype):
@@ -34,8 +35,7 @@ def index_max_forward(data, index, K):
     K = int(K)
     with torch.cuda.device(data.device):
         out = torch.empty((B, C, K), dtype=torch.int32, device=data.device)
-        rc = lib.index_max_forward(data.data_ptr(), index.data_ptr(), out.data_ptr(), B, C, N, K,
-                                   torch.cuda.current_stream().cuda_stream)
+        rc = lib.index_max_forward(data.data_ptr(), index.data_ptr(), out.data_ptr(), B, C, N, K, _stream_ptr())
     _native.check(rc, "index_max_forward")
     return out
 
@@ -52,27 +52,12 @@ def ball_query_forward(node_to_point_dist, radius, K):
     with torch.cuda.device(node_to_point_dist.device):
         out = torch.empty((B, M, K), dtype=torch.int32, device=node_to_point_dist.device)
         rc = lib.ball_query_forward(node_to_point_dist.data_ptr(), float(radius), out.data_ptr(), B, M, N, K,
-                                    torch.cuda.current_stream().cuda_stream)
+                                    _stream_ptr())
     _native.check(rc, "ball_query_forward")
     return out
 
 
 _xyz_ws = {}
-
-
-def _stream_workspace(cache, dev, stream, need, floor):
-    """One cached scratch per (device, stream): launches on one stream run in order, so they can share it; launches on
-    different streams may overlap.  While the current stream is being captured into a CUDA graph the scratch is a new
-    allocation from the graph's private pool and is not cached: a graph-pool buffer is never handed to a later eager
-    call, and a cached eager buffer is never resized under a graph that captured its address."""
-    if torch.cuda.is_current_stream_capturing():
-        return torch.empty(max(need, floor), dtype=torch.uint8, device=dev)
-    key = (dev.index, stream)
-    ws = cache.get(key)
-    if ws is None or ws.numel() < need:
-        ws = torch.empty(max(need, floor), dtype=torch.uint8, device=dev)
-        cache[key] = ws
-    return ws
 
 
 def ball_query_xyz_forward(points, nodes, radius, K):
@@ -92,11 +77,10 @@ def ball_query_xyz_forward(points, nodes, radius, K):
     K = int(K)
     dev = points.device
     with torch.cuda.device(dev):
-        ws = _stream_workspace(_xyz_ws, dev, torch.cuda.current_stream().cuda_stream,
-                               lib.ball_query_xyz_workspace_bytes(B, N), 1 << 20)
+        ws = _workspace(_xyz_ws, lib.ball_query_xyz_workspace_bytes(B, N), dev)
         out = torch.empty((B, M, K), dtype=torch.int32, device=dev)
         rc = lib.ball_query_xyz_forward(points.data_ptr(), nodes.data_ptr(), float(radius), out.data_ptr(), B, M, N, K,
-                                        ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
+                                        ws.data_ptr(), ws.numel(), _stream_ptr())
     _native.check(rc, "ball_query_xyz_forward")
     return out
 
@@ -121,8 +105,7 @@ def cluster_assign_forward(pc, node, k=1, want_centers=True):
     k = int(k)
     dev = pc.device
     with torch.cuda.device(dev):
-        ws = _stream_workspace(_ca_ws, dev, torch.cuda.current_stream().cuda_stream,
-                               lib.cluster_assign_workspace_bytes(B, M), 1 << 16)
+        ws = _workspace(_ca_ws, lib.cluster_assign_workspace_bytes(B, M), dev, floor=1 << 16)
         topk = torch.empty((B, N, k), dtype=torch.int32, device=dev)
         min_idx = torch.empty((B, N), dtype=torch.int32, device=dev)
         count = torch.empty((B, M), dtype=torch.int32, device=dev)
@@ -132,8 +115,7 @@ def cluster_assign_forward(pc, node, k=1, want_centers=True):
         rc = lib.cluster_assign_forward(pc.data_ptr(), node.data_ptr(), B, N, M, k, topk.data_ptr(), min_idx.data_ptr(),
                                         count.data_ptr(), mean.data_ptr(),
                                         centers.data_ptr() if want_centers else 0,
-                                        dec.data_ptr() if want_centers else 0, ws.data_ptr(), ws.numel(),
-                                        torch.cuda.current_stream().cuda_stream)
+                                        dec.data_ptr() if want_centers else 0, ws.data_ptr(), ws.numel(), _stream_ptr())
     _native.check(rc, "cluster_assign_forward")
     return dict(min_k_idx=topk, min_idx=min_idx, count=count, cluster_mean=mean, pc_centers=centers,
                 pc_decentered=dec)
@@ -144,10 +126,10 @@ INTERP_MAX_NODES = 2048
 _backward_ws = {}
 
 
-def _backward_workspace(dev, stream, need):
-    """The fp64 slice partials of the interpolation's and the encoder ops' backwards: one scratch per stream (launches
-    on one stream run in order, so they can share it; launches on different streams may overlap)."""
-    return _stream_workspace(_backward_ws, dev, stream, need, 1 << 16)
+def _backward_workspace(dev, need):
+    """The fp64 slice partials of the interpolation's and the encoder ops' backwards, for a launch on the current
+    stream."""
+    return _workspace(_backward_ws, need, dev, floor=1 << 16)
 
 
 def _check_interp_args(topk_idx, query, node, features):
@@ -194,7 +176,7 @@ class _Interpolation(torch.autograd.Function):
             idx = torch.empty((B, Nq, k), dtype=torch.int32, device=dev)
             out = torch.empty((B, C, Nq), dtype=torch.float32, device=dev)
             if out.numel():
-                stream = torch.cuda.current_stream().cuda_stream
+                stream = _stream_ptr()
                 rc = lib.interp_weights_f32(topk_idx.data_ptr(), topk_idx.element_size(), query.data_ptr(),
                                             node.data_ptr(), B, Nq, M, k, w.data_ptr(), idx.data_ptr(), stream)
                 _native.check(rc, "interp_weights_f32")
@@ -221,8 +203,8 @@ class _Interpolation(torch.autograd.Function):
         with torch.cuda.device(dev):
             gF = torch.empty((B, C, M), dtype=torch.float32, device=dev)
             if gF.numel():
-                stream = torch.cuda.current_stream().cuda_stream
-                ws = _backward_workspace(dev, stream, lib.interp_backward_workspace_bytes(B, C, Nq, M))
+                stream = _stream_ptr()
+                ws = _backward_workspace(dev, lib.interp_backward_workspace_bytes(B, C, Nq, M))
                 bstride = grad_out.stride(0) if B > 1 else 0
                 rc = lib.interp_backward_f32(grad_out.data_ptr(), bstride, w.data_ptr(), idx.data_ptr(), B, C, Nq, M,
                                              k, gF.data_ptr(), ws.data_ptr(), ws.numel(), stream)
@@ -293,7 +275,7 @@ class _ClusterMaxPool(torch.autograd.Function):
                 rc = lib.cluster_pool_forward_f32(features.data_ptr(), min_idx.data_ptr(), B, C, N, M, sel.data_ptr(),
                                                   mask.data_ptr(), pooled.data_ptr(),
                                                   scattered.data_ptr() if broadcast and scattered.numel() else None,
-                                                  torch.cuda.current_stream().cuda_stream)
+                                                  _stream_ptr())
                 _native.check(rc, "cluster_pool_forward_f32")
         ctx.set_materialize_grads(False)           # a missing pooled or scattered gradient stays None
         ctx.save_for_backward(min_idx, sel, mask)
@@ -319,10 +301,10 @@ class _ClusterMaxPool(torch.autograd.Function):
         with torch.cuda.device(dev):
             gF = torch.empty((B, C, N), dtype=torch.float32, device=dev)
             if gF.numel():
-                stream = torch.cuda.current_stream().cuda_stream
+                stream = _stream_ptr()
                 ws, ws_bytes = None, 0
                 if grad_scattered is not None:
-                    ws = _backward_workspace(dev, stream, lib.cluster_pool_backward_workspace_bytes(B, C, N, M))
+                    ws = _backward_workspace(dev, lib.cluster_pool_backward_workspace_bytes(B, C, N, M))
                     ws_bytes = ws.numel()
                 gs_ptr = grad_scattered.data_ptr() if grad_scattered is not None else None
                 bstride = grad_scattered.stride(0) if grad_scattered is not None and B > 1 else 0
@@ -384,8 +366,7 @@ class _KnnGroup(torch.autograd.Function):
             grouped = torch.empty((B, 3 + C, M, K), dtype=torch.float32, device=dev)
             if idx.numel():
                 rc = lib.knn_group_forward_f32(query.data_ptr(), database.data_ptr(), features.data_ptr(), B, C, M, N,
-                                               K, idx.data_ptr(), grouped.data_ptr(),
-                                               torch.cuda.current_stream().cuda_stream)
+                                               K, idx.data_ptr(), grouped.data_ptr(), _stream_ptr())
                 _native.check(rc, "knn_group_forward_f32")
         ctx.mark_non_differentiable(idx)
         ctx.set_materialize_grads(False)
@@ -412,8 +393,8 @@ class _KnnGroup(torch.autograd.Function):
         with torch.cuda.device(dev):
             gF = torch.empty((B, C, N), dtype=torch.float32, device=dev)
             if gF.numel():
-                stream = torch.cuda.current_stream().cuda_stream
-                ws = _backward_workspace(dev, stream, lib.knn_group_backward_workspace_bytes(B, C, M, N, K))
+                stream = _stream_ptr()
+                ws = _backward_workspace(dev, lib.knn_group_backward_workspace_bytes(B, C, M, N, K))
                 bstride = grad_grouped.stride(0) if B > 1 else 0
                 rc = lib.knn_group_backward_f32(grad_grouped.data_ptr() if M else None, bstride, idx.data_ptr(), B, C,
                                                 M, N, K, gF.data_ptr(), ws.data_ptr(), ws.numel(), stream)
@@ -471,7 +452,7 @@ class _AttentionFusion(torch.autograd.Function):
         with torch.cuda.device(dev):
             out = torch.empty((B, C, M), dtype=torch.float32, device=dev)
             rc = lib.attn_fusion_forward_f32(img_features.data_ptr(), attention.data_ptr(), B, C, P, M, out.data_ptr(),
-                                             torch.cuda.current_stream().cuda_stream)
+                                             _stream_ptr())
         _native.check(rc, "attn_fusion_forward_f32")
         ctx.set_materialize_grads(False)           # a missing output gradient stays None
         ctx.save_for_backward(img_features, attention)
@@ -497,7 +478,7 @@ class _AttentionFusion(torch.autograd.Function):
             bstride = grad_out.stride(0) if B > 1 else 0
             rc = lib.attn_fusion_backward_f32(grad_out.data_ptr(), bstride, F.data_ptr(), A.data_ptr(), B, C, P, M,
                                               gF.data_ptr() if need_F else None, gA.data_ptr() if need_A else None,
-                                              torch.cuda.current_stream().cuda_stream)
+                                              _stream_ptr())
         _native.check(rc, "attn_fusion_backward_f32")
         return gF, gA
 
@@ -530,7 +511,7 @@ def interpolation_weights(topk_idx, query, node):
         if w.numel():
             rc = lib.interp_weights_f32(topk_idx.data_ptr(), topk_idx.element_size(), query.data_ptr(),
                                         node.data_ptr(), B, Nq, node.shape[2], k, w.data_ptr(), idx.data_ptr(),
-                                        torch.cuda.current_stream().cuda_stream)
+                                        _stream_ptr())
             _native.check(rc, "interp_weights_f32")
     return w, idx
 
@@ -644,7 +625,7 @@ def pack_pointwise_mlp(spec, layers):
     with torch.cuda.device(dev):
         packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
         rc = lib.pointwise_mlp_pack_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.data_ptr(), need,
-                                        torch.cuda.current_stream().cuda_stream)
+                                        _stream_ptr())
     _native.check(rc, "pointwise_mlp_pack_f32")
     return PackedPointwiseMLP(spec, meta, packed)
 
@@ -720,15 +701,9 @@ def pointwise_mlp(sources, layers, output="activations", c_split=None, return_sc
         raise RuntimeError(f"the layers must be on {dev}")
     lib = _native.load()
     with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream().cuda_stream
+        stream = _stream_ptr()
         need = lib.pointwise_mlp_workspace_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), B)
-        ws = None
-        if need:
-            key = (dev.index, stream)
-            ws = _mlp_ws.get(key)
-            if ws is None or ws.numel() < need:
-                ws = torch.empty(need, dtype=torch.uint8, device=dev)
-                _mlp_ws[key] = ws
+        ws = _workspace(_mlp_ws, need, dev, floor=0) if need else None
         want_out = output == "activations" or return_scores
         out = torch.empty((B, C_out, N), dtype=torch.float32, device=dev) if want_out else None
         pred_a = torch.empty((B, N), dtype=torch.int8, device=dev) if output == "argmax" else None
@@ -808,7 +783,7 @@ def _pack_chain(kind, c_in, layers, meta, n_before):
         raise ValueError(f"{kind}: " + lib.dib_last_error().decode("utf-8", "replace"))
     with torch.cuda.device(dev):
         packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
-        stream = torch.cuda.current_stream().cuda_stream
+        stream = _stream_ptr()
         if kind == "knn_fusion":
             rc = lib.knn_fusion_pack_f32(*args, packed.data_ptr(), need, stream)
         else:
@@ -895,8 +870,7 @@ def knn_fusion(query, database, features, K, layers, return_idx=False):
         out = torch.empty((B, meta[-1][0], M), dtype=torch.float32, device=dev)
         rc = lib.knn_fusion_f32(query.data_ptr(), database.data_ptr(), features.data_ptr(), B, C, M, N, K,
                                 lay.ctypes.data, n_before, len(meta) - n_before, packed.packed.data_ptr(),
-                                packed.packed.numel() * 4, idx.data_ptr(), out.data_ptr(),
-                                torch.cuda.current_stream().cuda_stream)
+                                packed.packed.numel() * 4, idx.data_ptr(), out.data_ptr(), _stream_ptr())
     _native.check(rc, "knn_fusion_f32")
     return (out, idx) if return_idx else out
 
@@ -954,13 +928,9 @@ def pointwise_mlp_max(sources, layers):
     C_out = meta[-1][0]
     lib = _native.load()
     with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream().cuda_stream
+        stream = _stream_ptr()
         need = lib.pointwise_mlp_max_workspace_bytes(C_out, B, N)
-        key = (dev.index, stream)
-        ws = _mlp_max_ws.get(key)
-        if ws is None or ws.numel() < need:
-            ws = torch.empty(need, dtype=torch.uint8, device=dev)
-            _mlp_max_ws[key] = ws
+        ws = _workspace(_mlp_max_ws, need, dev, floor=0)
         out = torch.empty((B, C_out, 1), dtype=torch.float32, device=dev)
         rc = lib.pointwise_mlp_max_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.packed.data_ptr(),
                                        packed.packed.numel() * 4, B, N, out.data_ptr(), ws.data_ptr(), ws.numel(),
@@ -1081,7 +1051,7 @@ def pack_node_mlp(spec, layers):
     with torch.cuda.device(dev):
         packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
         rc = lib.node_mlp_pack_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.data_ptr(), need,
-                                   torch.cuda.current_stream().cuda_stream)
+                                   _stream_ptr())
     _native.check(rc, "node_mlp_pack_f32")
     del keep
     return PackedNodeMLP(spec, meta, packed)
@@ -1136,15 +1106,9 @@ def node_mlp(sources, layers, M=None):
         raise RuntimeError(f"the layers must be on {dev}")
     lib = _native.load()
     with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream().cuda_stream
+        stream = _stream_ptr()
         need = lib.node_mlp_workspace_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), B)
-        ws = None
-        if need:
-            key = (dev.index, stream)
-            ws = _node_mlp_ws.get(key)
-            if ws is None or ws.numel() < need:
-                ws = torch.empty(need, dtype=torch.uint8, device=dev)
-                _node_mlp_ws[key] = ws
+        ws = _workspace(_node_mlp_ws, need, dev, floor=0) if need else None
         out = torch.empty((B, meta[-1][0], M), dtype=torch.float32, device=dev)
         rc = lib.node_mlp_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.packed.data_ptr(),
                               packed.packed.numel() * 4, B, M, out.data_ptr(),

@@ -12,7 +12,8 @@ import numpy as np
 import torch
 
 from . import _native
-from .frustum import _ptr, _require_cuda, _stream_ptr, _workspace
+from ._native import _ptr, _require_cuda, _stream_ptr, _workspace
+from .frustum import _ws_cache
 from .icp import _check, pack_clouds
 
 VOXEL_SIZE = 0.1              # kitti_pc_bin_to_npy_with_downsample_sn.py: downsample_voxel_size, sn_radius, sn_max_nn
@@ -78,7 +79,7 @@ def voxel_downsample(xyz, n_pts, voxel_size, attr=None, stream=None):
         if C:
             res["attr"] = torch.zeros((S, C, N), dtype=torch.float64, device=dev)
         sp = _stream_ptr(stream)
-        ws = _workspace(max(lib.voxel_downsample_workspace_bytes(S, N, C), 1), dev, sp)
+        ws = _workspace(_ws_cache, max(lib.voxel_downsample_workspace_bytes(S, N, C), 1), dev, stream)
         fn = lib.voxel_downsample_batch_f32 if xyz.dtype == torch.float32 else lib.voxel_downsample_batch_f64
         rc = fn(_ptr(xyz), _ptr(n_pts), N, S, _ptr(attr), C, voxel_size, _ptr(res["xyz"]), _ptr(res.get("attr")),
                 _ptr(res["m_pts"]), _ptr(ws), ws.numel(), sp)
@@ -103,7 +104,7 @@ def estimate_normals(xyz, m_pts, radius=SN_RADIUS, max_nn=SN_MAX_NN, orient=(0.0
         nrm = torch.zeros((S, 3, M), dtype=torch.float64, device=dev)
         cnt = torch.zeros((S, M), dtype=torch.int32, device=dev) if counts else None
         sp = _stream_ptr(stream)
-        ws = _workspace(max(lib.estimate_normals_workspace_bytes(S, M), 1), dev, sp)
+        ws = _workspace(_ws_cache, max(lib.estimate_normals_workspace_bytes(S, M), 1), dev, stream)
         rc = lib.estimate_normals_batch_f32(_ptr(xyz), _ptr(m_pts), M, S, radius, int(max_nn),
                                             o.ctypes.data_as(_native._c.c_void_p), _ptr(nrm), _ptr(cnt), _ptr(ws),
                                             ws.numel(), sp)
@@ -133,7 +134,7 @@ def nearest(q, q_pts, xyz, m_pts, stream=None):
     with torch.cuda.device(dev), torch.cuda.stream(stream):
         idx = torch.full((S, Q), -1, dtype=torch.int32, device=dev)
         sp = _stream_ptr(stream)
-        ws = _workspace(max(lib.estimate_normals_workspace_bytes(S, M), 1), dev, sp)
+        ws = _workspace(_ws_cache, max(lib.estimate_normals_workspace_bytes(S, M), 1), dev, stream)
         rc = lib.nearest_batch_f32(_ptr(q), _ptr(q_pts), Q, _ptr(xyz), _ptr(m_pts), M, S, _ptr(idx), _ptr(ws),
                                    ws.numel(), sp)
     _native.check(rc, "nearest")

@@ -17,6 +17,7 @@ per-layer bound.
 import torch
 
 from . import _native
+from ._native import _ptr, _stream_ptr
 
 STAGES = ((64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2))     # (channels, blocks, first stride) of layers 1-4
 MIN_IMAGE = 32                                                     # the smallest H and W resnet34_features takes
@@ -90,8 +91,7 @@ def pack_conv(W, b, shortcut=None):
     need = lib.resnet_conv_packed_bytes(C_out, K)
     with torch.cuda.device(W.device):
         packed = torch.empty(need // 4, dtype=torch.float32, device=W.device)
-        rc = lib.resnet_conv_pack_f32(w.data_ptr(), C_out, K, packed.data_ptr(), need,
-                                      torch.cuda.current_stream().cuda_stream)
+        rc = lib.resnet_conv_pack_f32(w.data_ptr(), C_out, K, packed.data_ptr(), need, _stream_ptr())
     _native.check(rc, "resnet_conv_pack_f32")
     return PackedConv(packed, bias.contiguous(), int(k), int(C_in), int(C_out), c_short)
 
@@ -176,12 +176,10 @@ def conv2d_fused(x, layer, stride, residual=None, relu=True, shortcut=None, shor
     out = torch.empty((B, Ho, Wo, C_out), dtype=torch.float32, device=dev) if nhwc else None
     cm = torch.empty((B, C_out, Ho * Wo), dtype=torch.float32, device=dev) if channel_major else None
     lib = _native.load()
-    ptr = lambda t: 0 if t is None else t.data_ptr()
     with torch.cuda.device(dev):
-        rc = lib.resnet_conv_f32(x.data_ptr(), int(nchw_input), B, H, W, C, k, stride, pad, ptr(shortcut), H2, W2, C2,
+        rc = lib.resnet_conv_f32(x.data_ptr(), int(nchw_input), B, H, W, C, k, stride, pad, _ptr(shortcut), H2, W2, C2,
                                  shortcut_stride, layer.packed.data_ptr(), layer.packed.numel() * 4, layer.bias.data_ptr(),
-                                 ptr(residual), int(bool(relu)), C_out, ptr(out), ptr(cm),
-                                 torch.cuda.current_stream().cuda_stream)
+                                 _ptr(residual), int(bool(relu)), C_out, _ptr(out), _ptr(cm), _stream_ptr())
     _native.check(rc, "resnet_conv_f32")
     return (out, cm) if channel_major else out
 
@@ -198,7 +196,7 @@ def max_pool_3x3s2(x):
         return out
     lib = _native.load()
     with torch.cuda.device(x.device):
-        rc = lib.resnet_maxpool_f32(x.data_ptr(), B, H, W, C, out.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        rc = lib.resnet_maxpool_f32(x.data_ptr(), B, H, W, C, out.data_ptr(), _stream_ptr())
     _native.check(rc, "resnet_maxpool_f32")
     return out
 
@@ -219,8 +217,7 @@ def channel_mean(x):
         return out
     lib = _native.load()
     with torch.cuda.device(x.device):
-        rc = lib.resnet_mean_f32(x.data_ptr(), x.shape[0] * x.shape[1], x.shape[2], out.data_ptr(),
-                                 torch.cuda.current_stream().cuda_stream)
+        rc = lib.resnet_mean_f32(x.data_ptr(), x.shape[0] * x.shape[1], x.shape[2], out.data_ptr(), _stream_ptr())
     _native.check(rc, "resnet_mean_f32")
     return out
 

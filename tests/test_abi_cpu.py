@@ -21,7 +21,7 @@ def declared_symbols():
     return names
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_header_prototype():
     from deepi2p_b200 import build, _native
     lib = build.build()
     handle = ctypes.CDLL(lib)
@@ -30,12 +30,46 @@ def test_library_exports_every_declared_symbol():
             "frustum_prepare_batch_f32", "frustum_evaluate_f32", "frustum_residuals_f32"} <= decl
     for name in decl:
         assert hasattr(handle, name), name
-    assert set(_native.EXPORTS) <= decl | {"dib_last_error"}
+    assert set(_native.parse_header(open(build.HEADER).read())) == decl
     handle.dib_abi_version.restype = ctypes.c_int
     assert handle.dib_abi_version() == 4
     handle.frustum_solve_workspace_bytes.restype = ctypes.c_size_t
     handle.frustum_solve_workspace_bytes.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int]
     assert handle.frustum_solve_workspace_bytes(4096, 60, 20480) >= 4096 * 60 * (6 * 8 + 8 + 16)
+
+
+def test_every_prototype_is_bound_with_the_header_types():
+    """load() binds each prototype of the header with the types parse_header reads from it (compared by identity: an
+    int64_t or uint64_t argument bound as c_int would be truncated without an error)."""
+    from deepi2p_b200 import build, _native
+    c = ctypes
+    sigs = _native.parse_header(open(build.HEADER).read())
+    lib = _native.load()
+    assert len(sigs) >= 121
+    for name, (restype, argtypes) in sigs.items():
+        fn = getattr(lib, name)
+        assert fn.restype is restype, name
+        assert len(fn.argtypes) == len(argtypes) and all(a is b for a, b in zip(fn.argtypes, argtypes)), name
+    assert len(sigs["frustum_solve_batch_f32"][1]) == 23
+    loss = sigs["classifier_loss_forward_f32"][1]
+    assert loss[1] is c.c_int64 and loss[3] is c.c_int64
+    assert sigs["assemble_resample_f32"][1][7] is c.c_uint64
+    assert sigs["ball_query_xyz_forward"][1][2] is c.c_float
+    assert sigs["dib_last_error"] == (c.c_char_p, [])
+    assert sigs["dib_profile_solve_events"] == (None, [c.c_void_p, c.c_void_p])
+    sizes = [n for n in sigs if n.endswith("_workspace_bytes")]
+    assert sizes and all(sigs[n][0] is c.c_size_t for n in sizes)
+
+
+def test_header_parser_rejects_unknown_types():
+    from deepi2p_b200 import _native
+    c = ctypes
+    assert _native.parse_header("/* x; */\n#define A 1\ntypedef void* dib_stream_t;\n"
+                                "int f(const int64_t* p,\n      uint64_t seed, dib_stream_t s);") == \
+        {"f": (c.c_int, [c.c_void_p, c.c_uint64, c.c_void_p])}
+    for bad in ("unsigned int f(int a);", "int f(long n);", "long f(void);"):
+        with pytest.raises(_native.NativeError, match="f"):
+            _native.parse_header(bad)
 
 
 def test_argument_validation_without_gpu():

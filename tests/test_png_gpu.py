@@ -176,11 +176,11 @@ def test_feeds_assemble_images(cuda):
     assert torch.equal(a["img"], b["img"]) and np.array_equal(a["K64"], b["K64"])
 
 
-def test_unpadded_data_through_the_c_abi(cuda):
+def test_unpadded_data_decodes_through_the_c_abi(cuda):
     """The C ABI needs only 16-byte-aligned starts: an image whose IDAT data ends inside the buffer's last partial
     16-byte vector, with no padding after it, decodes (its Adler-32 trailer is in that vector)."""
     from deepi2p_b200 import _native, png
-    from deepi2p_b200.frustum import _workspace
+    from deepi2p_b200._native import _workspace
     lib = _native.load()
     for case in (GOOD[0], next(c for c in GOOD if c["name"] == "zlib_idat_1byte")):
         pk = png.pack_batch([case["blob"]])
@@ -192,7 +192,7 @@ def test_unpadded_data_through_the_c_abi(cuda):
         status = torch.empty((1, 4), dtype=torch.int32, device="cuda")
         sp = torch.cuda.current_stream().cuda_stream
         nws = lib.png_decode_workspace_bytes(desc.ctypes.data, 1, chunks.ctypes.data, len(chunks), n)
-        ws = _workspace(nws, torch.device("cuda"), sp)
+        ws = _workspace({}, nws, torch.device("cuda"))
         rc = lib.png_decode_batch_u8(data.data_ptr(), n, desc.ctypes.data, 1, chunks.ctypes.data, len(chunks),
                                      out.data_ptr(), out.numel(), status.data_ptr(), ws.data_ptr(), ws.numel(), sp)
         assert rc == 0
