@@ -21,11 +21,13 @@ SOURCES = sorted(os.path.basename(p) for p in glob.glob(os.path.join(CSRC, "*.cu
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [HEADER]
 # Compiled on their own without FMA contraction: oracle_pnp/pnp_oracle.cpp, oracle_icp/icp_oracle.cpp and
 # oracle_prep/prep_oracle.cpp, oracle_assemble/, oracle_interp/, oracle_image/ and oracle.pose_diff_restated (metrics.cu)
-# restate their arithmetic bit for bit (oracle_oxford_build/, oracle_oxford_images/ and oracle_kitti_build/ too); metrics.cu and
+# restate their arithmetic bit for bit (oracle_oxford_build/, oracle_oxford_images/, oracle_kitti_build/ and
+# oracle_kitti_depth/ too); metrics.cu and
 # classifier_loss.cu share the label rule of project.cuh.  monodepth.cu writes out the contractions of torch's bilinear
 # kernel with __fmaf_rn and keeps the back-projection to plain products and sums (DESIGN.md 4.31).
 NOFMA_SOURCES = ["pnp_ransac.cu", "icp.cu", "pointprep.cu", "assemble.cu", "interp.cu", "imageprep.cu", "metrics.cu",
-                 "classifier_loss.cu", "oxford_build.cu", "oxford_images.cu", "kitti_build.cu", "monodepth.cu"]
+                 "classifier_loss.cu", "oxford_build.cu", "oxford_images.cu", "kitti_build.cu", "monodepth.cu",
+                 "kitti_depth.cu"]
 assert set(NOFMA_SOURCES) <= set(SOURCES), set(NOFMA_SOURCES) - set(SOURCES)
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

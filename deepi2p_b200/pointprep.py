@@ -158,12 +158,13 @@ def sym3_eig_batch(C):
     return lam.cpu().numpy(), E.cpu().numpy().reshape(n, 3, 3)
 
 
-def prepare_scans(xyz, intensity, n_pts, voxel_size=VOXEL_SIZE, sn_radius=SN_RADIUS, sn_max_nn=SN_MAX_NN,
-                  orient=(0.0, 0.0, 1.0), stream=None):
-    """kitti_pc_bin_to_npy_with_downsample_sn.py:48-74 for S scans: voxel_down_sample(voxel_size), estimate_normals
-    (sn_radius, sn_max_nn) on the centres rounded to float32, orientation toward `orient`, and the intensity of the
-    nearest original point.  xyz [S,3,N] f32, intensity [S,N] f32, n_pts [S] int32 or None.  Returns (record
-    [S,7,N] float32 = (x, y, z, intensity, nx, ny, nz), entries past m_pts zero; m_pts [S] int32)."""
+def downsample_scans(xyz, intensity, n_pts, voxel_size=VOXEL_SIZE, sn_radius=SN_RADIUS, sn_max_nn=SN_MAX_NN,
+                     orient=(0.0, 0.0, 1.0), stream=None):
+    """The voxel -> normals -> nearest chain of the KITTI preparation scripts for S scans: voxel_down_sample
+    (voxel_size), estimate_normals(sn_radius, sn_max_nn) on the centres rounded to float32, orientation toward
+    `orient`, and the intensity of the nearest original point.  xyz [S,3,N] f32, intensity [S,N] f32, n_pts [S] int32
+    or None.  Returns dict(xyz [S,3,N] f64 (Open3D's float64 centres), m_pts [S] int32, normals [S,3,N] f64,
+    intensity [S,N] f32), entries past m_pts zero."""
     _positive(voxel_size, "voxel_size")
     _normal_params(sn_radius, sn_max_nn, orient)
     S, N = _cloud_batch(xyz, n_pts)
@@ -171,13 +172,22 @@ def prepare_scans(xyz, intensity, n_pts, voxel_size=VOXEL_SIZE, sn_radius=SN_RAD
     with torch.cuda.device(xyz.device), torch.cuda.stream(stream):
         down = voxel_downsample(xyz, n_pts, voxel_size, stream=stream)
         m = down["m_pts"]
-        d32 = down["xyz"].to(torch.float32)
-        nrm = estimate_normals(d32, m, sn_radius, sn_max_nn, orient, stream=stream)
+        nrm = estimate_normals(down["xyz"].to(torch.float32), m, sn_radius, sn_max_nn, orient, stream=stream)
         idx = nearest(down["xyz"], m, xyz, n_pts, stream=stream)
         valid = torch.arange(N, device=xyz.device)[None] < m[:, None]
         inten = torch.gather(intensity, 1, idx.clamp(min=0).long()).masked_fill(~valid, 0)
-        rec = torch.cat([d32, inten[:, None], nrm.to(torch.float32)], 1)
-    return rec, m
+    return dict(xyz=down["xyz"], m_pts=m, normals=nrm, intensity=inten)
+
+
+def prepare_scans(xyz, intensity, n_pts, voxel_size=VOXEL_SIZE, sn_radius=SN_RADIUS, sn_max_nn=SN_MAX_NN,
+                  orient=(0.0, 0.0, 1.0), stream=None):
+    """kitti_pc_bin_to_npy_with_downsample_sn.py:48-74 for S scans: downsample_scans, with the centres and normals
+    rounded to float32.  xyz [S,3,N] f32, intensity [S,N] f32, n_pts [S] int32 or None.  Returns (record [S,7,N]
+    float32 = (x, y, z, intensity, nx, ny, nz), entries past m_pts zero; m_pts [S] int32)."""
+    d = downsample_scans(xyz, intensity, n_pts, voxel_size, sn_radius, sn_max_nn, orient, stream)
+    with torch.cuda.device(xyz.device), torch.cuda.stream(stream):
+        rec = torch.cat([d["xyz"].to(torch.float32), d["intensity"][:, None], d["normals"].to(torch.float32)], 1)
+    return rec, d["m_pts"]
 
 
 def _to_device_cloud(pointcloud):

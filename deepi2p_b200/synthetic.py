@@ -630,6 +630,46 @@ def write_kitti_root(root, seqs=(0, 9, 10), n_frames=90, seed=0, n_rings=8, n_az
     return {seq: n_frames for seq in seqs}
 
 
+def write_kitti_velodyne_root(root, velodyne_root, seq, scans, sizes, K=(718.856, 718.856, 607.1928, 185.2157),
+                              images="npy"):
+    """A KITTI root for the camera-frame build (deepi2p_b200.kitti_depth): velodyne_root/sequences/<seq>/velodyne/
+    <frame>.bin from `scans` ([4, n] float32 each), root/calib/<seq>/calib.txt and the frames' images.  The calibration
+    has the intrinsics K = (fx, fy, cx, cy) for every camera; P0 and P2 have no translation (so P2 = I and
+    Pc = Tr exactly), P1 and P3 KITTI's baselines; Tr is the axis permutation x_cam = -y, y_cam = -z, z_cam = x.
+    sizes: per frame (H, W), or ((H2, W2), (H3, W3)) per camera.  images "npy" writes zero uint8 [H, W, 3] frames to
+    data_odometry_color_npy, "png" grey PNGs to the official data_odometry_color layout."""
+    if images not in ("npy", "png"):
+        raise ValueError(f"images must be 'npy' or 'png' (got {images!r})")
+    s = "%02d" % seq
+    fx, fy, cx, cy = K
+    lines = []
+    for k, tx in enumerate((0.0, -0.537, 0.0, -0.47)):
+        tz = (0.0, 0.0, 0.0, 3.4e-3)[k]
+        ty = (0.0, 0.0, 0.0, 2.0e-5)[k]
+        m = [fx, 0.0, cx, fx * tx + cx * tz, 0.0, fy, cy, fy * ty + cy * tz, 0.0, 0.0, 1.0, tz]
+        lines.append(f"P{k}: " + " ".join("%.12e" % v for v in m))
+    lines.append("Tr: " + " ".join("%.12e" % v for v in (0, -1, 0, 0, 0, 0, -1, 0, 1, 0, 0, 0)))
+    os.makedirs(os.path.join(root, "calib", s), exist_ok=True)
+    with open(os.path.join(root, "calib", s, "calib.txt"), "w") as f:
+        f.write("\n".join(lines) + "\n")
+    vdir = os.path.join(velodyne_root, "sequences", s, "velodyne")
+    os.makedirs(vdir, exist_ok=True)
+    for i, scan in enumerate(scans):
+        np.ascontiguousarray(np.asarray(scan, dtype="<f4").T).tofile(os.path.join(vdir, "%06d.bin" % i))
+    folder = "data_odometry_color_npy" if images == "npy" else "data_odometry_color"
+    for c, cam in enumerate(("image_2", "image_3")):
+        idir = os.path.join(root, folder, "sequences", s, cam)
+        os.makedirs(idir, exist_ok=True)
+        for i, hw in enumerate(sizes):
+            h, w = hw[c] if isinstance(hw[0], (tuple, list)) else hw
+            if images == "npy":
+                np.save(os.path.join(idir, "%06d.npy" % i), np.zeros((h, w, 3), dtype=np.uint8))
+            else:
+                with open(os.path.join(idir, "%06d.png" % i), "wb") as f:
+                    f.write(encode_png(np.zeros((h, w), dtype=np.uint8)))
+    return root
+
+
 def write_oxford_root(root, train=("2014-05-19-13-20-57", "2014-06-26-08-53-56"), val=("2014-07-14-14-49-50",),
                       n_clouds=24, cams_per_cloud=3, seed=0, n_rings=8, n_azimuth=256, image_hw=(960, 1280),
                       n_images=3, quality=90):

@@ -1002,6 +1002,37 @@ int monodepth_cloud_f32(const float* disp, int S, int h, int w, int H, int W, co
                         const double* K, double* scale, float* out32, void* workspace, size_t workspace_bytes,
                         dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * KITTI camera-frame records and LiDAR depth maps (data/kitti/kitti_pc_bin_to_npy_in_img_frame.py) for T (scan,
+ * camera) pairs of one image size H x W; pair t reads scan t / (T / S) of S, T a multiple of S.  DESIGN.md 4.33
+ * states the contract; deepi2p_b200/kitti_depth.py chains the calls.  All arithmetic is fp64 without FMA, each sum
+ * in the association stated; all pointers [dev].
+ *
+ * kitti_depth_project_f32: xyz [S][3][n_stride] f32 (n_pts [S] i32 <= n_stride < 2^30), Pc [T][16] f64 (row-major
+ *   4x4, rows 0-2 read), K [T][9] f32.  Point i of pair t has X, Y, Z = ((P0 x + P1 y) + P2 z) + P3 per row, u, v, w
+ *   = ((double)K0 X + K1 Y) + K2 Z per row, and counts when Z > 0.1, w != 0, and rint(u / w), rint(v / w) (halves to
+ *   even) land in the image, at d = sqrt(dx dx + dy dy) from the pixel centre.  out [T][2][H][W] is scratch for
+ *   kitti_depth_fill_f32: plane 1 the float32 minimum m of float32(d) per pixel (all-ones bits when empty), plane 0
+ *   the winner's code (the largest i with d < m, else the smallest i with float32(d) = m).
+ * kitti_depth_fill_f32: the same arguments, after kitti_depth_project_f32 on the same stream (each fill needs its own
+ *   project: a filled out[] gives NaN depths when filled again).  Writes out [T][2][H][W]
+ *   f32: a filled pixel (float32(Z of its winner), m); an empty one the depth of its nearest filled pixel (smallest
+ *   column, then smallest row, among the nearest) and float32(sqrt(d2)); with no filled pixel at all (0,
+ *   sqrt((r + 1)^2 + c^2)).  H, W <= 32767 with (H-1)^2 + (W-1)^2 < 2^31.  workspace >=
+ *   kitti_depth_fill_workspace_bytes(T, H, W).
+ * kitti_depth_records_f32: xyz, nrm [S][3][m_stride] f64 (the voxel centres and their normals), intensity
+ *   [S][m_stride] f32, m_pts [S] i32 <= m_stride.  out [T][7][m_stride] f32 = (((P0 x + P1 y) + P2 z) + P3 per row,
+ *   intensity, -ny, -nz, nx), each rounded once; zeros past m_pts.
+ * ------------------------------------------------------------------------------------------ */
+size_t kitti_depth_fill_workspace_bytes(int T, int H, int W);
+int kitti_depth_project_f32(const float* xyz, int64_t n_stride, const int32_t* n_pts, int S, const double* Pc,
+                            const float* K, int T, int H, int W, float* out, dib_stream_t stream);
+int kitti_depth_fill_f32(const float* xyz, int64_t n_stride, const int32_t* n_pts, int S, const double* Pc,
+                         const float* K, int T, int H, int W, float* out, void* workspace, size_t workspace_bytes,
+                         dib_stream_t stream);
+int kitti_depth_records_f32(const double* xyz, const double* nrm, const float* intensity, const int32_t* m_pts,
+                            int64_t m_stride, int S, const double* Pc, int T, float* out, dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
