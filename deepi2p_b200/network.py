@@ -31,6 +31,10 @@ from . import classifier, frustum, point_ops, resnet
 SHAPES = {"kitti": dict(img_H=160, img_W=512), "oxford": dict(img_H=384, img_W=640),
           "nuscenes": dict(img_H=160, img_W=320)}
 
+# KeypointDetector(point_layers=...): "torch" runs the per-point chains as the model's own layers; "fused" runs them
+# through point_ops.point_chain (DESIGN.md 4.34)
+POINT_LAYERS = ("torch", "fused")
+
 # forward chunk of classify_and_register: at the Oxford shape (20480 points, 384 x 640) one chunk of 64 samples peaks
 # at 13.5 GB above the inputs on an H100 (BENCH_E2E.json, DESIGN.md 4.18)
 DEFAULT_CHUNK = 64
@@ -207,9 +211,12 @@ class KeypointDetector(nn.Module):
 
     def __init__(self, img_H=160, img_W=512, fine_scale=32, fine=True, node_a_num=128, node_b_num=128, k_ab=16,
                  k_interp_ab=3, k_interp_point_a=3, k_interp_point_b=3, normalization="batch", activation="relu",
-                 norm_momentum=0.1, resnet_weights=None):
+                 norm_momentum=0.1, resnet_weights=None, point_layers="torch"):
         super().__init__()
         _check_menu(normalization, activation)
+        if point_layers not in POINT_LAYERS:
+            raise ValueError(f"point_layers must be one of {POINT_LAYERS}, got {point_layers!r}")
+        self.point_layers = point_layers
         H_f, W_f = classifier.fine_grid(img_H, img_W, fine_scale)
         L = H_f * W_f
         s32, s16 = _resnet_map_size(img_H, img_W, 32), _resnet_map_size(img_H, img_W, 16)
@@ -234,6 +241,29 @@ class KeypointDetector(nn.Module):
         if resnet_weights is not None:
             sd = torch.load(os.fspath(resnet_weights), map_location="cpu", weights_only=True)
             self.img_encoder.backbone.load_state_dict(sd, strict=True)
+        # point_chain's dropout stream (seed, offset); not part of the state_dict, so checkpoints load in either mode
+        self.register_buffer("point_chain_state", torch.zeros(2, dtype=torch.int64), persistent=False)
+
+    def _fused_head(self, pc, node_a, node_b, pa_idx, pb_idx, up_node_a_features, up_node_b_features, first_pn_out,
+                    second_pn_out):
+        """per_point_pn over (pa, pb, first_pn_out, second_pn_out) with point_layers="fused"."""
+        head = list(self.per_point_pn.layers)
+        Ca, Cb = up_node_a_features.shape[1], up_node_b_features.shape[1]
+        if not self.training:
+            wa, ia = point_ops.interpolation_weights(pa_idx, pc, node_a)
+            wb, ib = point_ops.interpolation_weights(pb_idx, pc, node_b)
+            return point_ops.point_chain([(up_node_a_features, wa, ia), (up_node_b_features, wb, ib), first_pn_out,
+                                          second_pn_out], head, False)
+        # pa and pb are interpolations of node features, so their block of the first layer is applied at the nodes
+        # and the projected rows are interpolated: the 736-row input is never built.  channel_product runs on the
+        # chain kernels, so the step stays deterministic without cuBLAS.
+        W1 = head[0].conv.weight[:, :, 0]
+        pa = point_ops.upsample_by_interpolation(pa_idx, pc, node_a,
+                                                 point_ops.channel_product(W1[:, :Ca], up_node_a_features))
+        pb = point_ops.upsample_by_interpolation(pb_idx, pc, node_b,
+                                                 point_ops.channel_product(W1[:, Ca:Ca + Cb], up_node_b_features))
+        return point_ops.point_chain([first_pn_out, second_pn_out], head, True, self.point_chain_state, add=pa + pb,
+                                     in_col=Ca + Cb)
 
     def forward(self, pc, intensity, sn, node_a, node_b, img):
         B, Ma, Mb = pc.shape[0], node_a.shape[2], node_b.shape[2]
@@ -244,9 +274,18 @@ class KeypointDetector(nn.Module):
         # point encoder (networks_pc.py:58-115)
         ca = point_ops.cluster_assign_forward(pc, node_a, k=self.k_interp_point_a)
         min_idx = ca["min_idx"]
-        first_pn_out = enc.first_pointnet(torch.cat((ca["pc_decentered"], intensity, sn), dim=1))
+        fused = self.point_layers == "fused"
+        if fused:
+            first_pn_out = point_ops.point_chain([ca["pc_decentered"], intensity, sn], list(enc.first_pointnet.layers),
+                                                 self.training, self.point_chain_state)
+        else:
+            first_pn_out = enc.first_pointnet(torch.cat((ca["pc_decentered"], intensity, sn), dim=1))
         _, scattered = point_ops.cluster_max_pool(first_pn_out, min_idx, Ma, broadcast=True)
-        second_pn_out = enc.second_pointnet(torch.cat((first_pn_out, scattered), dim=1))
+        if fused:
+            second_pn_out = point_ops.point_chain([first_pn_out, scattered], list(enc.second_pointnet.layers),
+                                                  self.training, self.point_chain_state)
+        else:
+            second_pn_out = enc.second_pointnet(torch.cat((first_pn_out, scattered), dim=1))
         node_a_features = point_ops.cluster_max_pool(second_pn_out, min_idx, Ma)
         node_b_features = enc.knnlayer(node_b, ca["cluster_mean"], node_a_features, self.k_ab)
         final_pn_out = enc.final_pointnet(torch.cat((node_b, node_b_features), dim=1))
@@ -269,14 +308,19 @@ class KeypointDetector(nn.Module):
 
         # decoder (networks_united.py:158-197)
         pb_idx = point_ops.cluster_assign_forward(pc, node_b, k=self.k_interp_point_b, want_centers=False)["min_k_idx"]
-        pb = point_ops.upsample_by_interpolation(pb_idx, pc, node_b, up_node_b_features)
+        if not fused:
+            pb = point_ops.upsample_by_interpolation(pb_idx, pc, node_b, up_node_b_features)
         att_a = self.node_a_attention_pn(torch.cat((node_a_features, img_global_a), dim=1))
         weighted_s16 = point_ops.attention_fusion(s16, att_a)
         ab_idx = point_ops.cluster_assign_forward(node_a, node_b, k=self.k_interp_ab, want_centers=False)["min_k_idx"]
         ab = point_ops.upsample_by_interpolation(ab_idx, node_a, node_b, up_node_b_features)
         up_node_a_features = self.node_a_pn(torch.cat((node_a_features, ab, weighted_s16), dim=1))
-        pa = point_ops.upsample_by_interpolation(ca["min_k_idx"], pc, node_a, up_node_a_features)
-        scores = self.per_point_pn(torch.cat((pa, pb, first_pn_out, second_pn_out), dim=1))
+        if fused:
+            scores = self._fused_head(pc, node_a, node_b, ca["min_k_idx"], pb_idx, up_node_a_features,
+                                      up_node_b_features, first_pn_out, second_pn_out)
+        else:
+            pa = point_ops.upsample_by_interpolation(ca["min_k_idx"], pc, node_a, up_node_a_features)
+            scores = self.per_point_pn(torch.cat((pa, pb, first_pn_out, second_pn_out), dim=1))
         if self.fine:
             return scores[:, 0:2, :], scores[:, 2:, :]
         return scores[:, 0:2, :]

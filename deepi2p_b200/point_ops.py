@@ -1116,3 +1116,410 @@ def node_mlp(sources, layers, M=None):
     _native.check(rc, "node_mlp_f32")
     del keep
     return out
+
+
+CHAIN_MAX_LAYERS = 3
+CHAIN_MAX_WIDTH = 256
+CHAIN_MAX_IN = 1024
+CHAIN_MAX_SOURCES = 4
+_PC_SRC, _PC_OP = 3, 6            # int64 slots per operand source / transform row (DIB_PC_SRC, DIB_PC_OP)
+_OP_PLAIN, _OP_ACT, _OP_BN_GRAD = 0, 1, 2
+_EP_WRITE, _EP_STATS, _EP_ACT_GRAD = 0, 1, 2
+_chain_part_ws, _chain_dw_ws = {}, {}
+
+
+def _chain_operand(srcs, mode=_OP_PLAIN, stats=None, y=None, drop=None, layer=0):
+    """The operand table of point_chain's kernels: dense [B,C,N] sources in row order, then the transform row.  drop:
+    (state int64 [2], p) or None."""
+    import numpy as np
+    t = np.zeros(len(srcs) * _PC_SRC + _PC_OP, dtype=np.int64)
+    for i, s in enumerate(srcs):
+        t[i * _PC_SRC:(i + 1) * _PC_SRC] = (s.data_ptr(), s.stride(0) if s.shape[0] > 1 else s.shape[1] * s.shape[2],
+                                            s.shape[1])
+    h = len(srcs) * _PC_SRC
+    t[h:h + _PC_OP] = (mode, 0 if stats is None else stats.data_ptr(), 0 if y is None else y.data_ptr(),
+                       0 if drop is None else drop[0].data_ptr(), 0 if drop is None else round(drop[1] * 1e6), layer)
+    return t
+
+
+def _chain_act_row(stats, drop, layer):
+    import numpy as np
+    return np.array((stats.data_ptr(), 0, 0 if drop is None else drop[0].data_ptr(),
+                     0 if drop is None else round(drop[1] * 1e6), layer), dtype=np.int64)
+
+
+def _chain_pack(W, widths):
+    """W [C_out, sum(widths)] packed by pointwise_mlp's packer for dense sources of those widths."""
+    return pack_pointwise_mlp([(c, 0, 0) for c in widths], [(W.detach(), None, False)]).packed
+
+
+def _chain_gemm(op, n_src, packed, bias, add, C, B, N, epilogue, act=None, act_y=None):
+    lib = _native.load()
+    dev = act_y.device if act_y is not None else torch.device("cuda", torch.cuda.current_device())
+    out = torch.empty((B, C, N), dtype=torch.float32, device=dev)
+    part = None
+    if epilogue != _EP_WRITE:
+        part = _workspace(_chain_part_ws, lib.point_chain_partial_bytes(B, N, C), dev, floor=0)
+    rc = lib.point_chain_gemm_f32(op.ctypes.data, n_src, None if packed is None else packed.data_ptr(),
+                                  None if bias is None else bias.data_ptr(), None if add is None else add.data_ptr(),
+                                  C, B, N, epilogue, None if act is None else act.ctypes.data,
+                                  None if act_y is None else act_y.data_ptr(), out.data_ptr(),
+                                  None if part is None else part.data_ptr(), 0 if part is None else part.numel(),
+                                  _stream_ptr())
+    _native.check(rc, "point_chain_gemm_f32")
+    return out, part
+
+
+def _chain_bn(part, B, N, C, norm, stats, grad):
+    lib = _native.load()
+    dev = stats.device
+    if grad:
+        dgamma, dbeta = torch.empty(C, dtype=torch.float32, device=dev), torch.empty(C, dtype=torch.float32, device=dev)
+        coef = torch.empty((3, C), dtype=torch.float32, device=dev)
+        rc = lib.point_chain_bn_f32(part.data_ptr(), B, N, C, 1, norm.weight.data_ptr(), norm.bias.data_ptr(),
+                                    float(norm.eps), 0.0, stats.data_ptr(), None, None, None, dgamma.data_ptr(),
+                                    dbeta.data_ptr(), coef.data_ptr(), _stream_ptr())
+        _native.check(rc, "point_chain_bn_f32")
+        return dgamma, dbeta, coef
+    nbt = norm.num_batches_tracked
+    rc = lib.point_chain_bn_f32(part.data_ptr(), B, N, C, 0, norm.weight.data_ptr(), norm.bias.data_ptr(),
+                                float(norm.eps), float(norm.momentum), stats.data_ptr(), norm.running_mean.data_ptr(),
+                                norm.running_var.data_ptr(), None if nbt is None else nbt.data_ptr(), None, None, None,
+                                _stream_ptr())
+    _native.check(rc, "point_chain_bn_f32")
+
+
+def _chain_dw(dy_op, x_op, n_src, B, N, C, K, want_db):
+    lib = _native.load()
+    dev = torch.device("cuda", torch.cuda.current_device())
+    dW = torch.empty((C, K), dtype=torch.float32, device=dev)
+    db = torch.empty(C, dtype=torch.float32, device=dev) if want_db else None
+    ws = _workspace(_chain_dw_ws, lib.point_chain_dw_workspace_bytes(B, N, C, K), dev, floor=0)
+    rc = lib.point_chain_dw_f32(dy_op.ctypes.data, x_op.ctypes.data, n_src, B, N, dW.data_ptr(),
+                                None if db is None else db.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr())
+    _native.check(rc, "point_chain_dw_f32")
+    return dW, db
+
+
+def _chain_product(op, n_src, W, widths, B, N):
+    """W [R, sum(widths)] . the operand, [B, R, N]: in blocks of CHAIN_MAX_WIDTH output rows, the kernel's limit."""
+    R = W.shape[0]
+    outs = [_chain_gemm(op, n_src, _chain_pack(W[r:r + CHAIN_MAX_WIDTH], widths), None, None,
+                        min(CHAIN_MAX_WIDTH, R - r), B, N, _EP_WRITE)[0] for r in range(0, R, CHAIN_MAX_WIDTH)]
+    return outs[0] if len(outs) == 1 else torch.cat(outs, dim=1)
+
+
+class _PointChain(torch.autograd.Function):
+    """Inputs: (layers, drop_state, n_src, in_col, add, *sources, *per-layer (W, b, gamma, beta)); gamma / beta are None for a
+    layer without BatchNorm.  The BN buffers of `layers` are updated in place."""
+
+    @staticmethod
+    def forward(ctx, layers, drop_state, n_src, in_col, add, *tensors):
+        sources = list(tensors[:n_src])
+        B, N = sources[0].shape[0], sources[0].shape[2]
+        dev = sources[0].device
+        # the masks of this call: a copy of (seed, offset) taken before the offset advances, so a replayed graph draws
+        # new ones and the backward recomputes these
+        drop = None
+        if any(layer.dropout is not None for layer in layers):
+            drop = drop_state.clone()
+            drop_state[1:].add_(1)
+        widths = [s.shape[1] for s in sources]
+        op = _chain_operand(sources)
+        ys, stats_all = [], []
+        with torch.cuda.device(dev):
+            for l, layer in enumerate(layers):
+                conv, norm = layer.conv, layer.norm
+                C = conv.out_channels
+                W = conv.weight.detach().reshape(C, -1)
+                packed = _chain_pack(W[:, in_col:in_col + sum(widths)] if l == 0 else W, widths)
+                bias = None if conv.bias is None else conv.bias.detach()
+                y, part = _chain_gemm(op, len(widths), packed, bias, add if l == 0 else None, C, B, N,
+                                      _EP_STATS if norm is not None else _EP_WRITE)
+                st = None
+                if norm is not None:
+                    st = torch.empty((4, C), dtype=torch.float32, device=dev)
+                    with torch.no_grad():
+                        _chain_bn(part, B, N, C, norm, st, grad=False)
+                    d = None if layer.dropout is None else (drop, float(layer.dropout.p))
+                    op = _chain_operand([y], _OP_ACT, st, drop=d, layer=l)
+                else:
+                    op = _chain_operand([y])
+                ys.append(y)
+                stats_all.append(st)
+                widths = [C]
+            last = layers[-1]
+            if last.norm is not None:
+                out, _ = _chain_gemm(op, 1, None, None, None, last.conv.out_channels, B, N, _EP_WRITE)
+            else:
+                out = ys[-1]
+        # the sources and the pre-norm outputs go through save_for_backward only: autograd then catches an in-place change
+        # to a source before the backward, and the chain's output, which can be one of the outputs, is not held on ctx
+        # (that would tie the autograd graph into a reference cycle)
+        ctx.layers, ctx.n_src, ctx.in_col, ctx.has_add = layers, n_src, in_col, add is not None
+        ctx.stats, ctx.drop, ctx.shape = stats_all, drop, (B, N)
+        ctx.save_for_backward(*sources, *ys)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        layers, (B, N), n_src = ctx.layers, ctx.shape, ctx.n_src
+        saved = ctx.saved_tensors
+        sources, ys = saved[:n_src], saved[n_src:]
+        dev = ys[0].device
+        L = len(layers)
+        grads = [None] * (4 * L)
+        g_src = [None] * n_src
+        g_add = None
+        with torch.cuda.device(dev):
+            G = grad_out.float().contiguous()
+            dz = None
+            for l in range(L - 1, -1, -1):
+                layer = layers[l]
+                conv, norm = layer.conv, layer.norm
+                C = conv.out_channels
+                y, st = ys[l], ctx.stats[l]
+                d = None if layer.dropout is None else (ctx.drop, float(layer.dropout.p))
+                if norm is not None:
+                    if l == L - 1:
+                        dz, part = _chain_gemm(_chain_operand([G]), 1, None, None, None, C, B, N, _EP_ACT_GRAD,
+                                               _chain_act_row(st, d, l), y)
+                    dgamma, dbeta, coef = _chain_bn(part, B, N, C, norm, st, grad=True)
+                    dy_op = _chain_operand([dz], _OP_BN_GRAD, coef, y)
+                    grads[4 * l + 2], grads[4 * l + 3] = dgamma, dbeta
+                else:
+                    dy_op = _chain_operand([G])
+                if l == 0:
+                    x_op, nx = _chain_operand(sources), n_src
+                else:
+                    prev = layers[l - 1]
+                    dp = None if prev.dropout is None else (ctx.drop, float(prev.dropout.p))
+                    x_op, nx = _chain_operand([ys[l - 1]], _OP_ACT, ctx.stats[l - 1], drop=dp, layer=l - 1), 1
+                K = conv.in_channels if l > 0 else sum(s.shape[1] for s in sources)
+                c0 = ctx.in_col if l == 0 else 0
+                dW, db = _chain_dw(dy_op, x_op, nx, B, N, C, K, conv.bias is not None)
+                if K != conv.in_channels:             # the columns the sources feed; the rest get their gradient
+                    full = dW.new_zeros((C, conv.in_channels))     # through `add`
+                    full[:, c0:c0 + K] = dW
+                    dW = full
+                grads[4 * l], grads[4 * l + 1] = dW.view_as(conv.weight), db
+                W = conv.weight.detach().reshape(C, conv.in_channels)[:, c0:c0 + K]
+                if l > 0:
+                    prev = layers[l - 1]
+                    dp = None if prev.dropout is None else (ctx.drop, float(prev.dropout.p))
+                    dz, part = _chain_gemm(dy_op, 1, _chain_pack(W.t().contiguous(), [C]), None, None, K, B, N,
+                                           _EP_ACT_GRAD, _chain_act_row(ctx.stats[l - 1], dp, l - 1), ys[l - 1])
+                else:
+                    if ctx.has_add and ctx.needs_input_grad[4]:
+                        g_add = G if norm is None else _chain_gemm(dy_op, 1, None, None, None, C, B, N, _EP_WRITE)[0]
+                    if any(ctx.needs_input_grad[5:5 + n_src]):
+                        gx = _chain_product(dy_op, 1, W.t(), [C], B, N)
+                        r = 0
+                        for i, s in enumerate(sources):
+                            if ctx.needs_input_grad[5 + i]:
+                                g_src[i] = gx[:, r:r + s.shape[1]]
+                            r += s.shape[1]
+        return (None, None, None, None, g_add, *g_src, *grads)
+
+
+def _check_chain_args(sources, layers, drop_state, add, in_col, training):
+    if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= CHAIN_MAX_LAYERS:
+        raise ValueError(f"layers: need a list of 1 to {CHAIN_MAX_LAYERS} point layers")
+    if not isinstance(sources, (list, tuple)) or not 1 <= len(sources) <= CHAIN_MAX_SOURCES:
+        raise ValueError(f"sources: need a list of 1 to {CHAIN_MAX_SOURCES} sources")
+    c_in = 0
+    for i, layer in enumerate(layers):
+        conv = getattr(layer, "conv", None)
+        if not isinstance(conv, torch.nn.Conv1d) or conv.kernel_size != (1,) or conv.groups != 1:
+            raise TypeError(f"layers[{i}]: need a point layer with a 1x1 Conv1d `conv`")
+        if not 1 <= conv.out_channels <= CHAIN_MAX_WIDTH:
+            raise ValueError(f"layers[{i}]: need 1 <= C_out <= {CHAIN_MAX_WIDTH}, got {conv.out_channels}")
+        if i > 0 and conv.in_channels != layers[i - 1].conv.out_channels:
+            raise ValueError(f"layers[{i}]: has {conv.in_channels} input channels, layers[{i - 1}] gives "
+                             f"{layers[i - 1].conv.out_channels}")
+        if i < len(layers) - 1 and layer.norm is None:
+            raise ValueError(f"layers[{i}]: only the last layer may go without BatchNorm + ReLU")
+        if layer.norm is not None:
+            if not isinstance(layer.norm, torch.nn.BatchNorm1d) or not layer.norm.affine \
+                    or not layer.norm.track_running_stats:
+                raise TypeError(f"layers[{i}]: the norm must be an affine BatchNorm1d with running statistics")
+            if training and layer.norm.momentum is None:
+                raise ValueError(f"layers[{i}]: a cumulative BatchNorm (momentum None) is not supported")
+        if layer.dropout is not None and layer.norm is None:
+            raise ValueError(f"layers[{i}]: dropout needs BatchNorm + ReLU on the same layer")
+        if i == 0:
+            c_in = conv.in_channels
+    if c_in > CHAIN_MAX_IN:
+        raise ValueError(f"layers[0]: more than {CHAIN_MAX_IN} input channels")
+    rows, B, N, dev = 0, None, None, layers[0].conv.weight.device
+    for i, s in enumerate(sources):
+        if not isinstance(s, torch.Tensor):
+            raise TypeError(f"sources[{i}] must be a torch.Tensor")
+        if s.dim() != 3 or s.shape[1] < 1:
+            raise ValueError(f"sources[{i}] must be [B,C,N] with C >= 1")
+        if s.dtype != torch.float32:
+            raise TypeError(f"sources[{i}] must have dtype torch.float32")
+        if s.device != dev:
+            raise ValueError(f"sources[{i}] must be on {dev}, the layers' device")
+        if B is None:
+            B, N = s.shape[0], s.shape[2]
+        elif (s.shape[0], s.shape[2]) != (B, N):
+            raise ValueError(f"sources[{i}] has B, N = {s.shape[0]}, {s.shape[2]}; sources[0] has {B}, {N}")
+        rows += s.shape[1]
+    if not isinstance(in_col, int) or isinstance(in_col, bool) or in_col < 0:
+        raise TypeError(f"in_col must be a non-negative int, got {in_col!r}")
+    if add is None and (in_col != 0 or rows != c_in):
+        raise ValueError(f"sources: {rows} rows from column {in_col}; without `add` they must be all {c_in} columns "
+                         f"of layers[0]")
+    if in_col + rows > c_in:
+        raise ValueError(f"sources: {rows} rows from column {in_col} exceed layers[0]'s {c_in} input columns")
+    if not 1 <= B <= MLP_MAX_BATCH or N < 1:
+        raise ValueError(f"sources: need 1 <= B <= {MLP_MAX_BATCH} and N >= 1, got B = {B}, N = {N}")
+    if add is not None:
+        if not isinstance(add, torch.Tensor):
+            raise TypeError("add must be a torch.Tensor or None")
+        if add.dtype != torch.float32:
+            raise TypeError("add must have dtype torch.float32")
+        if tuple(add.shape) != (B, layers[0].conv.out_channels, N) or add.device != dev:
+            raise ValueError(f"add must be [{B}, {layers[0].conv.out_channels}, {N}] on {dev}")
+    if training and any(layer.dropout is not None for layer in layers):
+        if not isinstance(drop_state, torch.Tensor):
+            raise TypeError("drop_state must be a torch.Tensor: int64 [2] (seed, offset) on the layers' device")
+        if drop_state.dtype != torch.int64 or tuple(drop_state.shape) != (2,) or drop_state.device != dev \
+                or not drop_state.is_contiguous():
+            raise ValueError("drop_state must be a contiguous int64 [2] (seed, offset) on the layers' device")
+    for i, layer in enumerate(layers):
+        conv, norm = layer.conv, layer.norm
+        for name, t in (("weight", conv.weight), ("bias", conv.bias)) + (
+                (("norm.weight", norm.weight), ("norm.bias", norm.bias), ("norm.running_mean", norm.running_mean),
+                 ("norm.running_var", norm.running_var)) if norm is not None else ()):
+            if t is not None and (not t.is_cuda or t.dtype != torch.float32):
+                raise TypeError(f"layers[{i}].{name} must be a float32 CUDA tensor")
+    return B, N
+
+
+def new_dropout_state(seed, device):
+    """A point_chain dropout state: int64 [2] (seed, offset 0) on `device`."""
+    return torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
+
+
+def point_chain(sources, layers, training, drop_state=None, add=None, in_col=0):
+    """A chain of one to three of the classifier's point layers (network._PointLayer: 1x1 Conv1d, then BatchNorm1d +
+    ReLU and Dropout where the layer has them) over [B,C,N] points (DESIGN.md 4.34).
+
+    sources: 1 to 4 float32 CUDA tensors [B,C_i,N] whose rows, in order, are layer 1's input (never concatenated).
+    layers: the chain's _PointLayer modules as they are; only the last may lack BatchNorm + ReLU.
+
+    training=True runs the layers in train mode as one differentiable op: products on the tensor cores in TF32 with
+    float32 accumulation whatever torch's TF32 flags say; BatchNorm with the batch's statistics (fp64 per-tile sums
+    reduced in a fixed order), the running statistics and num_batches_tracked updated as nn.BatchNorm1d does; dropout
+    masks from counter-based Philox keyed by drop_state (int64 [2] (seed, offset) on the device, needed when a layer
+    has dropout), whose offset the op advances on the device; add: an optional [B,C_1,N] term added to layer 1 before
+    its BatchNorm, standing for the input columns the sources do not feed (the sources feed columns [in_col, in_col +
+    their rows) of layer 1's weight, and layer 1's weight gradient is zero outside them).  Only each layer's pre-norm output is kept for the backward, which returns gradients for every
+    parameter, every source and `add`, deterministically (no atomics, fixed summation orders).  The masks differ from
+    torch's Dropout's.
+
+    Up to 1024 source rows; every layer's C_out is at most 256.
+
+    training=False is the eval-mode chain: fold_pointnet + pointwise_mlp, and `add` is not taken (give pointwise_mlp's
+    interpolated sources instead).  It has no backward, so under grad mode a source or layer parameter that requires
+    grad raises RuntimeError instead of returning an output cut off from autograd.  Errors name the argument: ValueError for shapes and widths,
+    TypeError for types and dtypes."""
+    if training:
+        B, N = _check_chain_args(sources, layers, drop_state, add, in_col, True)
+        flat = []
+        for layer in layers:
+            norm = layer.norm
+            flat += [layer.conv.weight, layer.conv.bias, None if norm is None else norm.weight,
+                     None if norm is None else norm.bias]
+        srcs = []
+        for s in sources:
+            if (N > 1 and s.stride(2) != 1) or (s.shape[1] > 1 and s.stride(1) != N) \
+                    or (B > 1 and s.stride(0) < s.shape[1] * N):
+                s = s.contiguous()
+            srcs.append(s)
+        return _PointChain.apply(list(layers), drop_state, len(srcs), in_col, None if add is None else add.contiguous(),
+                                 *srcs, *flat)
+    if add is not None or in_col != 0:
+        raise ValueError("add, in_col: the eval-mode chain takes interpolated sources instead of an additive term")
+    if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= CHAIN_MAX_LAYERS:
+        raise ValueError(f"layers: need a list of 1 to {CHAIN_MAX_LAYERS} point layers")
+    if torch.is_grad_enabled():
+        flat = [t for s in sources for t in ((s,) if isinstance(s, torch.Tensor) else s)]
+        if any(isinstance(t, torch.Tensor) and t.requires_grad for t in flat) or \
+                any(p.requires_grad for layer in layers for p in layer.parameters()):
+            raise RuntimeError("point_chain in eval mode (training=False) has no backward: call it under "
+                               "torch.no_grad(), or detach the sources and freeze the layers")
+    import types
+    from .network import fold_pointnet
+    return pointwise_mlp(list(sources), fold_pointnet(types.SimpleNamespace(layers=list(layers))))
+
+
+class _ChannelProduct(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, W, x):
+        B, K, M = x.shape
+        with torch.cuda.device(x.device):
+            out = _chain_product(_chain_operand([x.detach()]), 1, W.detach(), [K], B, M)
+        ctx.save_for_backward(W, x)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        W, x = ctx.saved_tensors
+        B, K, M = x.shape
+        C = W.shape[0]
+        gW = gx = None
+        with torch.cuda.device(x.device):
+            G = grad_out.float().contiguous()
+            g_op = _chain_operand([G])
+            if ctx.needs_input_grad[0]:
+                gW, _ = _chain_dw(g_op, _chain_operand([x.detach()]), 1, B, M, C, K, False)
+            if ctx.needs_input_grad[1]:
+                gx = _chain_product(g_op, 1, W.detach().t(), [C], B, M)
+        return gW, gx
+
+
+def channel_product(W, x):
+    """W [C, K] . x [B, K, M] -> [B, C, M] float32: a 1x1 layer without bias over the M columns of each sample, on the
+    chain kernels of point_chain (TF32 tensor-core products with float32 accumulation, the weight gradient summed over
+    the columns in a fixed order), so it is deterministic without cuBLAS.  Differentiable in W and x; 1 <= K, C <=
+    CHAIN_MAX_IN.  KeypointDetector(point_layers="fused") applies the head's pa / pb weight columns at the nodes with
+    it."""
+    for t, name in ((W, "W"), (x, "x")):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor")
+        if t.dtype != torch.float32:
+            raise TypeError(f"{name} must have dtype torch.float32")
+    for t, name in ((W, "W"), (x, "x")):
+        if not t.is_cuda:
+            raise ValueError(f"{name} must be a CUDA tensor")
+    if W.dim() != 2 or x.dim() != 3 or W.shape[1] != x.shape[1]:
+        raise ValueError(f"W must be [C, K] and x [B, K, M] with the same K, got {tuple(W.shape)} and {tuple(x.shape)}")
+    if not 1 <= W.shape[0] <= CHAIN_MAX_IN or not 1 <= W.shape[1] <= CHAIN_MAX_IN:
+        raise ValueError(f"W: need 1 <= C, K <= {CHAIN_MAX_IN}, got {tuple(W.shape)}")
+    if not 1 <= x.shape[0] <= MLP_MAX_BATCH or x.shape[2] < 1:
+        raise ValueError(f"x: need 1 <= B <= {MLP_MAX_BATCH} and M >= 1, got {tuple(x.shape)}")
+    if x.device != W.device:
+        raise ValueError(f"x must be on {W.device}, W's device")
+    return _ChannelProduct.apply(W, x.contiguous())
+
+
+def point_chain_dropout_mask(drop_state, layer, p, B, C, N):
+    """The keep bits point_chain draws for layer `layer` (0-based in its chain) of dropout probability p under
+    drop_state (the (seed, offset) pair as it was when the call began): uint8 [B,C,N], 1 = kept.  For references that
+    have to use the same mask."""
+    if not isinstance(drop_state, torch.Tensor) or drop_state.dtype != torch.int64 or tuple(drop_state.shape) != (2,) \
+            or not drop_state.is_cuda:
+        raise ValueError("drop_state must be a CUDA int64 [2] (seed, offset)")
+    if not 0 <= p < 1:
+        raise ValueError(f"p: need 0 <= p < 1, got {p}")
+    lib = _native.load()
+    dev = drop_state.device
+    with torch.cuda.device(dev):
+        out = torch.empty((B, C, N), dtype=torch.uint8, device=dev)
+        rc = lib.point_chain_dropout_mask(drop_state.contiguous().data_ptr(), int(layer), float(p), B, C, N,
+                                          out.data_ptr(), _stream_ptr())
+    _native.check(rc, "point_chain_dropout_mask")
+    return out

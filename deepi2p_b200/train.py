@@ -21,7 +21,7 @@ import time
 import numpy as np
 import torch
 
-from . import classifier, kitti, network, nuscenes, oxford
+from . import classifier, kitti, network, nuscenes, oxford, point_ops
 
 DATASETS = ("kitti", "oxford", "nuscenes")
 
@@ -217,6 +217,8 @@ class Trainer:
         self.graph, self._eager_steps = None, 0
         self.sums = torch.zeros(5, dtype=torch.float64, device=self.device)
         self._consumed = torch.cuda.Event()
+        if model.point_layers == "fused":              # point_chain's dropout stream starts from the run's seed
+            model.point_chain_state.copy_(point_ops.new_dropout_state(self.seed, self.device))
 
     # -- state --------------------------------------------------------------------------------------------------------
     def _set_lr(self, lr):
@@ -236,6 +238,8 @@ class Trainer:
         self.epoch, self.step_count, self.seed = st["epoch"] + 1, st["step"], st["seed"]
         torch.cuda.set_rng_state(st["cuda_rng"], self.device)
         self.best = float(st["extra"].get("best", 0.0))
+        if "point_chain_state" in st["extra"]:
+            self.model.point_chain_state.copy_(st["extra"]["point_chain_state"])
         self.graph, self._eager_steps = None, 0
 
     # -- input buffers -------------------------------------------------------------------------------------------------
@@ -365,6 +369,7 @@ class Trainer:
             torch.save(self.model.state_dict(), path)
             save_resume(os.path.join(self.out_dir, "resume.pth"), self.model, self.optimizer, epoch, self.step_count,
                         self.lr, self.seed, dict(best=self.best, dataset=self.dataset, version=self.version,
-                                                 batch_size=self.batch_size))
+                                                 batch_size=self.batch_size,
+                                                 point_chain_state=self.model.point_chain_state.cpu()))
             self.epoch = epoch + 1
         return path

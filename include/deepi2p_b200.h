@@ -1033,6 +1033,63 @@ int kitti_depth_fill_f32(const float* xyz, int64_t n_stride, const int32_t* n_pt
 int kitti_depth_records_f32(const double* xyz, const double* nrm, const float* intensity, const int32_t* m_pts,
                             int64_t m_stride, int S, const double* Pc, int T, float* out, dib_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training path of the classifier's per-point layers (the PointNets of models/layers_pc.py:345-408 in train mode;
+ * SURVEY.md 8f N29).  DESIGN.md 4.34 states the contract; point_ops.point_chain strings the calls together.  One 1x1
+ * layer per call over the N points of B samples; [dev] pointers; weights packed by pointwise_mlp_pack_f32 (one layer,
+ * dense sources only, so rounded to TF32 once).  The products run on the tensor cores in TF32 with f32 accumulation;
+ * every sum across points is in a fixed order (fp64 per 64-point tile, then the tiles in order), with no atomics.
+ *
+ * operand: [host] int64, n_src rows of DIB_PC_SRC (DATA f32 [B][CHANNELS][N] at batch stride BSTRIDE), in row order,
+ *   then one DIB_PC_OP row: MODE 0 plain rows; 1 act: dropout(relu(scale y + shift)) of one BN layer's pre-norm rows
+ *   with STATS [4][C] f32 (mean, invstd, scale, shift as point_chain_bn_f32 writes them), DROP_STATE int64 [2] (seed,
+ *   offset) or 0, DROP_PPM = p * 1e6, LAYER (the mask's layer id); 2 bn_grad: k1 dZ + k2 Y + k3 of dZ rows with Y
+ *   [B][C][N] and STATS = coef [3][C].  A transformed operand has one source.
+ * act: [host] int64 DIB_PC_ACT (STATS, unused, DROP_STATE, DROP_PPM, LAYER).  Dropout keeps (layer, b, c, n) when
+ *   word 0 of Philox4x32-10 at counter (n, c | layer << 24, b, offset lo) with key (seed lo, seed hi ^ offset hi) is
+ *   >= p 2^32, and scales the kept values by 1 / (1 - p).
+ *
+ * point_chain_gemm_f32: out [B][C][N] = W . operand + bias + add (packed NULL: the operand itself, C = its rows;
+ *   bias, add [B][C][N] may be NULL).  epilogue 0 writes; 1 also writes per-tile sums of v and v^2 to partials; 2 (the
+ *   backward of the BN layer `act` with pre-norm act_y [B][C][N]) writes dZ = v * keep / (1 - p) * (scale y + shift >
+ *   0) and per-tile sums of dZ and dZ (y - mean) invstd.  C <= 256, operand rows <= 1024, 1 <= B <= 65535.
+ * point_chain_bn_f32: the tile sums -> grad 0: stats [4][C], running_mean / running_var updated with `momentum` (the
+ *   variance unbiased), num_batches_tracked[0] += 1 when not NULL; grad 1: dgamma, dbeta and coef [3][C].
+ * point_chain_dw_f32: dW [C][K] = sum over b, n of dy[c] x[k] and db [C] = sum of dy[c] (db may be NULL); dy is a
+ *   one-source operand of C rows, x an operand of K rows with n_src sources.  Split over the points, the splits
+ *   summed in order in fp64.  workspace: 16-byte aligned, >= point_chain_dw_workspace_bytes.
+ * point_chain_dropout_mask: out uint8 [B][C][N] = the keep bits of layer `layer` under drop_state (for tests).
+ * ------------------------------------------------------------------------------------------ */
+#define DIB_PC_SRC 3
+#define DIB_PC_SRC_DATA 0
+#define DIB_PC_SRC_BSTRIDE 1
+#define DIB_PC_SRC_CHANNELS 2
+#define DIB_PC_OP 6
+#define DIB_PC_OP_MODE 0
+#define DIB_PC_OP_STATS 1
+#define DIB_PC_OP_Y 2
+#define DIB_PC_OP_DROP_STATE 3
+#define DIB_PC_OP_DROP_PPM 4
+#define DIB_PC_OP_LAYER 5
+#define DIB_PC_ACT 5
+#define DIB_PC_ACT_STATS 0
+#define DIB_PC_ACT_C 1
+#define DIB_PC_ACT_DROP_STATE 2
+#define DIB_PC_ACT_DROP_PPM 3
+#define DIB_PC_ACT_LAYER 4
+size_t point_chain_partial_bytes(int B, int N, int C);
+int point_chain_gemm_f32(const int64_t* operand, int n_src, const void* packed, const float* bias, const float* add,
+                         int C, int B, int N, int epilogue, const int64_t* act, const float* act_y, float* out,
+                         void* partials, size_t partial_bytes, dib_stream_t stream);
+int point_chain_bn_f32(const void* partials, int B, int N, int C, int grad, const float* gamma, const float* beta,
+                       float eps, float momentum, float* stats, float* running_mean, float* running_var,
+                       int64_t* num_batches_tracked, float* dgamma, float* dbeta, float* coef, dib_stream_t stream);
+size_t point_chain_dw_workspace_bytes(int B, int N, int C, int K);
+int point_chain_dw_f32(const int64_t* dy, const int64_t* x, int n_src, int B, int N, float* dW, float* db,
+                       void* workspace, size_t workspace_bytes, dib_stream_t stream);
+int point_chain_dropout_mask(const int64_t* drop_state, int layer, float p, int B, int C, int N, uint8_t* out,
+                             dib_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,6 +4,7 @@ GPU, with the reference's schedule, test pass, loss lines and checkpoint names (
     python scripts/train_classifier.py --dataset {kitti,oxford,nuscenes} --root R --out DIR
         [--epochs 101] [--batch B] [--seed 0] [--version V] [--coarse-only] [--resnet-weights FILE]
         [--record-dir NAME] [--nuscenes-version V] [--resume DIR/resume.pth] [--store {cuda,pinned}]
+        [--point-layers {torch,fused}]
 
 Every epoch writes DIR/v{version}-gpu{gpu}-epoch{epoch}-{test coarse accuracy}.pth (the detector's state_dict, which
 network.load_checkpoint and the reference's load_model read) and DIR/resume.pth (model, optimiser, epoch, step
@@ -37,6 +38,8 @@ def parse_args(argv=None):
     ap.add_argument("--resume", default=None, help="a resume.pth to continue from")
     ap.add_argument("--store", default=None, choices=("cuda", "pinned"),
                     help="keep the scan records in one device or pinned store (KITTI, Oxford)")
+    ap.add_argument("--point-layers", default="torch", choices=network.POINT_LAYERS,
+                    help="fused: the per-point chains as point_ops.point_chain (TF32, its own dropout stream)")
     a = ap.parse_args(argv)
     if a.epochs < 1:
         ap.error("--epochs must be >= 1")
@@ -56,7 +59,7 @@ def main(argv=None):
     if not torch.cuda.is_available():
         raise SystemExit("train_classifier.py needs a CUDA device")
     model = network.KeypointDetector(**network.SHAPES[a.dataset], fine=not a.coarse_only,
-                                     resnet_weights=a.resnet_weights).cuda()
+                                     resnet_weights=a.resnet_weights, point_layers=a.point_layers).cuda()
     src = lambda mode: train.batch_source(a.dataset, a.root, mode, store=a.store, record_dir=a.record_dir,
                                           nuscenes_version=a.nuscenes_version)
     trainset, testset = src("train"), src("val")
