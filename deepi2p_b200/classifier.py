@@ -3,8 +3,9 @@
 classifier_loss replaces the tail of MMClassifer.foraward_pass (models/multimodal_classifier.py:135-191, the
 coarse-only variant :482-508): the projected coarse and fine labels, kornia's focal loss on the coarse scores, the
 cross-entropy of the fine scores over the inside points, the accuracies and the predictions, with no host
-synchronisation, so a training step can be captured in a CUDA graph.  The kernels are in csrc/classifier_loss.cu;
-there is no CPU fallback.
+synchronisation, so a training step can be captured in a CUDA graph.  prediction_accuracy counts given predictions
+against the same labels for evaluation (DESIGN.md 4.35).  The kernels are in csrc/classifier_loss.cu; there is no
+CPU fallback.
 """
 import math
 import numbers
@@ -183,3 +184,84 @@ def classifier_loss(coarse_scores, fine_scores, pc, P, K, H, W, fine_scale=32, c
     extras = {}
     loss, coarse, fine = _ClassifierLoss.apply(coarse_scores, fine_scores, pc, P12, K9, cfg, extras)
     return dict(loss=loss, coarse=coarse, fine=fine if fine_scores is not None else None, **extras)
+
+
+def prediction_accuracy(pc, P, K, H, W, coarse_pred, fine_pred=None, fine_scale=32, *, return_labels=False):
+    """Per-sample accuracy counts of given predictions against classifier_loss's labels (DESIGN.md 4.35), for
+    evaluation: the fused heads arg-max inside their kernels, so there are no scores to hand to classifier_loss.
+
+    pc [S,3,N] float32, P [S,3,4] or [S,4,4] and K [S,3,3] float32 or float64 (read as fp64), coarse_pred int8 [S,N],
+    fine_pred int32 [S,N] or None (coarse only), all on one CUDA device.  Returns a dict of int32 [S] tensors:
+    n_inside, coarse_correct (predictions equal to the label over all N points) and fine_correct (over the inside
+    points; None without fine_pred), equal to classifier_loss's counts for scores whose torch.max arg-max are the
+    predictions.  With return_labels, also coarse_labels int8 [S,N] and fine_labels int32 [S,N] (the cell inside, -1
+    outside).  One kernel launch and no host synchronisation: the call is capturable in a CUDA graph."""
+    for t, name in ((pc, "pc"), (P, "P"), (K, "K"), (coarse_pred, "coarse_pred")):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor")
+    if pc.dtype != torch.float32 or pc.dim() != 3 or pc.shape[1] != 3:
+        raise RuntimeError("pc must be a float32 [S,3,N] tensor")
+    S, N = pc.shape[0], pc.shape[2]
+    if P.dtype not in (torch.float32, torch.float64) or P.dim() != 3 or P.shape[0] != S or P.shape[2] != 4 \
+            or P.shape[1] not in (3, 4):
+        raise RuntimeError("P must be a float32 or float64 [S,3,4] or [S,4,4] tensor")
+    if K.dtype not in (torch.float32, torch.float64) or tuple(K.shape) != (S, 3, 3):
+        raise RuntimeError("K must be a float32 or float64 [S,3,3] tensor")
+    if coarse_pred.dtype != torch.int8 or tuple(coarse_pred.shape) != (S, N):
+        raise RuntimeError("coarse_pred must be an int8 [S,N] tensor with the S and N of pc")
+    if fine_pred is not None and (not isinstance(fine_pred, torch.Tensor) or fine_pred.dtype != torch.int32
+                                  or tuple(fine_pred.shape) != (S, N)):
+        raise RuntimeError("fine_pred must be an int32 [S,N] tensor with the S and N of pc")
+    if not (S >= 1 and N >= 1 and S * N < 2 ** 31):
+        raise RuntimeError(f"need S, N >= 1 and S * N < 2^31, got S = {S}, N = {N}")
+    if not (H >= 1 and W >= 1 and fine_scale > 0):
+        raise ValueError(f"need H, W >= 1 and fine_scale > 0, got H = {H}, W = {W}, fine_scale = {fine_scale}")
+    want_fine = fine_pred is not None or return_labels
+    H_f, W_f = fine_grid(H, W, fine_scale) if want_fine else (0, 0)
+    if want_fine and (math.floor((W - 1) / fine_scale) >= W_f or math.floor((H - 1) / fine_scale) >= H_f):
+        raise ValueError(f"the last pixel row or column of the {H} x {W} image falls outside the {H_f} x {W_f} "
+                         f"cell grid of fine_scale {fine_scale}")
+    dev = pc.device
+    for t, name in ((pc, "pc"), (P, "P"), (K, "K"), (coarse_pred, "coarse_pred"), (fine_pred, "fine_pred")):
+        if t is None:
+            continue
+        if not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor")
+        if t.device != dev:
+            raise RuntimeError(f"{name} must be on {dev}")
+    lib = _native.load()
+    with torch.cuda.device(dev):
+        P12 = P[:, :3, :].to(torch.float64).reshape(S, 12).contiguous()
+        K9 = K.to(torch.float64).reshape(S, 9).contiguous()
+        pc, coarse_pred = pc.contiguous(), coarse_pred.contiguous()
+        fine_pred = fine_pred.contiguous() if fine_pred is not None else None
+        i32 = dict(dtype=torch.int32, device=dev)
+        out = dict(n_inside=torch.empty((S,), **i32), coarse_correct=torch.empty((S,), **i32),
+                   fine_correct=torch.empty((S,), **i32) if fine_pred is not None else None)
+        if return_labels:
+            out.update(coarse_labels=torch.empty((S, N), dtype=torch.int8, device=dev),
+                       fine_labels=torch.empty((S, N), **i32))
+        rc = lib.classifier_prediction_accuracy_f32(
+            pc.data_ptr(), P12.data_ptr(), K9.data_ptr(), coarse_pred.data_ptr(), _ptr(fine_pred), S, N, float(H),
+            float(W), float(fine_scale), H_f, W_f, _ptr(out.get("coarse_labels")), _ptr(out.get("fine_labels")),
+            out["n_inside"].data_ptr(), out["coarse_correct"].data_ptr(), _ptr(out["fine_correct"]), _stream_ptr())
+    _native.check(rc, "classifier_prediction_accuracy_f32")
+    return out
+
+
+def overall_accuracy(n_inside, coarse_correct, fine_correct, N):
+    """visualize_and_save_data.py's "Overall coarse accuracy, fine accuracy" (:137-147, 216-217) from per-sample counts
+    (host arrays or CPU tensors, in sample order) of samples with N points each: the per-sample accuracies, coarse
+    correct / N and fine correct / inside, summed in sample order in float64 and divided by the sample count.  A sample
+    with no inside point has the fine accuracy np.mean([]) = NaN, which carries into the overall fine accuracy, as in
+    the script.  fine_correct None (a coarse-only model) gives a NaN fine accuracy.  Returns (coarse, fine) floats."""
+    n_inside = [int(v) for v in n_inside]
+    coarse_correct = [int(v) for v in coarse_correct]
+    S = len(coarse_correct)
+    if S == 0 or len(n_inside) != S or (fine_correct is not None and len(fine_correct) != S):
+        raise ValueError("need the same number (at least one) of n_inside, coarse_correct and fine_correct counts")
+    coarse = fine = 0.0
+    for s in range(S):
+        coarse += coarse_correct[s] / N         # np.mean of a 0/1 vector: the count over N, correctly rounded
+        fine += int(fine_correct[s]) / n_inside[s] if fine_correct is not None and n_inside[s] else math.nan
+    return coarse / S, fine / S

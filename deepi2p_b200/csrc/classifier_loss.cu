@@ -11,6 +11,8 @@
 //                        writes the per-sample counts, the three losses, the accuracies and the inside total.
 //   cls_backward_kernel  one thread per point: both gradients in one pass, the fine softmax recomputed from the logits
 //                        and the saved log-sum-exp, the scale factors read from device memory.
+//   cls_accuracy_kernel  one CTA per sample (DESIGN.md 4.35): the same label pass compared with given predictions,
+//                        for evaluation, where the fused heads return predictions and no scores.
 // No atomics: every sum has an order fixed by the shape.  Per-point arithmetic is fp32, sums over points fp64.  The
 // file is compiled with --fmad=false (build.py NOFMA_SOURCES) so that the coarse label is inside_mask_kernel's
 // decision bit for bit.
@@ -75,6 +77,20 @@ struct FineState {
   }
 };
 
+// The label pass of cls_forward_kernel and cls_accuracy_kernel.  coarse_label: point n of sample b inside the image by
+// project.cuh's rule, with its pixel (u, v); fine_label: the cell floor(u / s) + floor(v / s) * Wf of an inside point,
+// -1 otherwise.
+__device__ __forceinline__ bool coarse_label(const float* __restrict__ pc, const double* __restrict__ P12,
+                                             const double* __restrict__ K9, int b, int n, int N, double H, double W,
+                                             double* u, double* v) {
+  const float* p = pc + (size_t)b * 3 * N + n;
+  return project_inside(P12 + (size_t)b * 12, K9 + (size_t)b * 9, p[0], p[N], p[2 * (size_t)N], H, W, u, v);
+}
+
+__device__ __forceinline__ int fine_label(bool in, double u, double v, double s, int Wf) {
+  return in ? (int)floor(u / s) + (int)floor(v / s) * Wf : -1;
+}
+
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll
@@ -97,9 +113,8 @@ __global__ void __launch_bounds__(kClsThreads)
   double focal = 0.0, ce = 0.0;
   int inside = 0, c_ok = 0, f_ok = 0;
   if (n < N) {
-    const float* p = pc + (size_t)b * 3 * N + n;
     double u, v;
-    const bool in = project_inside(P12 + (size_t)b * 12, K9 + (size_t)b * 9, p[0], p[N], p[2 * (size_t)N], H, W, &u, &v);
+    const bool in = coarse_label(pc, P12, K9, b, n, N, H, W, &u, &v);
     const size_t bn = (size_t)b * N + n;
     const float* zc = coarse + (size_t)b * cbs + n;
     const float z0 = zc[0], z1 = zc[N];
@@ -111,7 +126,7 @@ __global__ void __launch_bounds__(kClsThreads)
     inside = in ? 1 : 0;
     c_ok = cp == inside ? 1 : 0;
     if (fine) {
-      const int label = in ? (int)floor(u / s) + (int)floor(v / s) * Wf : -1;
+      const int label = fine_label(in, u, v, s, Wf);
       const float* row = fine + (size_t)b * fbs + n;
       FineState st;
       int l = 0;
@@ -254,6 +269,53 @@ __global__ void __launch_bounds__(kClsThreads)
   }
 }
 
+// One CTA per sample: the label pass over the sample's points, compared with given predictions (coarse: pred ==
+// label; fine: counted over the inside points), the counts summed per warp and then in warp order.  Integer sums only,
+// so the order does not matter for the result; one CTA per sample needs no second launch and no atomics.
+constexpr int kAccThreads = 512;
+
+__global__ void __launch_bounds__(kAccThreads)
+    cls_accuracy_kernel(const float* __restrict__ pc, const double* __restrict__ P12, const double* __restrict__ K9,
+                        const int8_t* __restrict__ coarse_pred, const int32_t* __restrict__ fine_pred, int N, double H,
+                        double W, double s, int Wf, int8_t* __restrict__ coarse_lab, int32_t* __restrict__ fine_lab,
+                        int32_t* __restrict__ n_inside, int32_t* __restrict__ coarse_correct,
+                        int32_t* __restrict__ fine_correct) {
+  __shared__ int sh[3][kAccThreads / 32];
+  const int b = blockIdx.x;
+  const bool want_fine = fine_pred || fine_lab;
+  int inside = 0, c_ok = 0, f_ok = 0;
+  for (int n = threadIdx.x; n < N; n += kAccThreads) {
+    double u, v;
+    const bool in = coarse_label(pc, P12, K9, b, n, N, H, W, &u, &v);
+    const size_t bn = (size_t)b * N + n;
+    if (coarse_lab) coarse_lab[bn] = in ? 1 : 0;
+    inside += in ? 1 : 0;
+    c_ok += (int)coarse_pred[bn] == (in ? 1 : 0) ? 1 : 0;
+    if (want_fine) {
+      const int label = fine_label(in, u, v, s, Wf);
+      if (fine_lab) fine_lab[bn] = label;
+      if (fine_pred && in && fine_pred[bn] == label) ++f_ok;
+    }
+  }
+  inside = warp_sum(inside);
+  c_ok = warp_sum(c_ok);
+  f_ok = warp_sum(f_ok);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+    sh[0][warp] = inside; sh[1][warp] = c_ok; sh[2][warp] = f_ok;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int i0 = 0, i1 = 0, i2 = 0;
+    for (int w = 0; w < kAccThreads / 32; ++w) {
+      i0 += sh[0][w]; i1 += sh[1][w]; i2 += sh[2][w];
+    }
+    n_inside[b] = i0;
+    coarse_correct[b] = i1;
+    if (fine_correct) fine_correct[b] = i2;
+  }
+}
+
 inline int cls_blocks(int N) { return (N + kClsThreads - 1) / kClsThreads; }
 
 }  // namespace dib
@@ -316,6 +378,32 @@ int classifier_loss_forward_f32(const float* coarse, int64_t coarse_batch_stride
   cls_reduce_kernel<<<1, kClsThreads, 0, stream>>>(part_d, part_i, B, N, nblk, fine ? 1 : 0, coarse_loss_alpha, loss,
                                                    coarse_loss, fine_loss, accuracy, n_inside, coarse_correct,
                                                    fine ? fine_correct : nullptr, n_inside_total);
+  DIB_CHECK_CUDA(cudaGetLastError());
+  return DIB_OK;
+}
+
+int classifier_prediction_accuracy_f32(const float* pc, const double* P12, const double* K9, const int8_t* coarse_pred,
+                                       const int32_t* fine_pred, int B, int N, double H, double W, double fine_scale,
+                                       int H_f, int W_f, int8_t* coarse_labels, int32_t* fine_labels,
+                                       int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
+                                       dib_stream_t stream_) {
+  using namespace dib;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  DIB_REQUIRE(B >= 1 && N >= 1 && (long long)B * N < (1LL << 31),
+              "classifier_prediction_accuracy: need B, N >= 1 and B * N below 2^31");
+  DIB_REQUIRE(pc && P12 && K9 && coarse_pred && n_inside && coarse_correct,
+              "classifier_prediction_accuracy: NULL argument");
+  DIB_REQUIRE(!fine_pred || fine_correct, "classifier_prediction_accuracy: fine_pred needs fine_correct");
+  DIB_REQUIRE(H >= 1.0 && W >= 1.0 && fine_scale > 0.0,
+              "classifier_prediction_accuracy: need H, W >= 1 and fine_scale > 0");
+  if (fine_pred || fine_labels) {
+    DIB_REQUIRE(H_f >= 1 && W_f >= 1 && floor((W - 1.0) / fine_scale) < W_f && floor((H - 1.0) / fine_scale) < H_f,
+                "classifier_prediction_accuracy: the last pixel row / column falls outside the %d x %d cell grid",
+                H_f, W_f);
+  }
+  cls_accuracy_kernel<<<B, kAccThreads, 0, stream>>>(pc, P12, K9, coarse_pred, fine_pred, N, H, W, fine_scale, W_f,
+                                                     coarse_labels, fine_labels, n_inside, coarse_correct,
+                                                     fine_pred ? fine_correct : nullptr);
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
 }

@@ -595,6 +595,21 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
 
     Returns dict(P [S,4,4] f64, cost [S] f64, coarse_pred int8 [S,N], fine_pred int32 [S,N] or None, degenerate
     int32 [S]); a sample with no point predicted inside gets P = I, cost 1e4 and degenerate = 1."""
+    coarse_pred, fine_pred = classify_batch(model, pc, intensity, sn, node_a, node_b, img, chunk=chunk, head=head)
+    H, W = img.shape[2], img.shape[3]
+    N = pc.shape[2]
+    reg = frustum.register_batch(pc.contiguous(), coarse_pred, N, K, H, W, n_inits=n_inits, seed=seed, t_lb=t_lb,
+                                 t_ub=t_ub, is_2d=True)
+    return dict(P=reg["P"], cost=reg["cost"], coarse_pred=coarse_pred, fine_pred=fine_pred,
+                degenerate=reg["degenerate"])
+
+
+def classify_batch(model, pc, intensity, sn, node_a, node_b, img, chunk=DEFAULT_CHUNK, head="torch"):
+    """The forward of classify_and_register alone: an assembled batch (the inputs classify_and_register takes) ->
+    (coarse_pred int8 [S,N], fine_pred int32 [S,N] or None for a coarse-only model), on the batch's device.  It runs
+    in eval mode under no_grad over chunks of `chunk` samples with the numeric contract `head` selects (see
+    classify_and_register) and restores the model's training flag, so the predictions can go to any registration
+    method: frustum.register_batch, pnp.pnp_ransac_batch or the ICP baseline's source cloud."""
     S, N = pc.shape[0], pc.shape[2]
     chunk = int(chunk)
     if chunk < 1:
@@ -607,7 +622,7 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
     for t, name in ((intensity, "intensity"), (sn, "sn"), (node_a, "node_a"), (node_b, "node_b"), (img, "img")):
         if t.shape[0] != S:
             raise ValueError(f"{name} has {t.shape[0]} samples, pc has {S}")
-    H, W = img.shape[2], img.shape[3]
+    img.shape[3]            # an image batch without H and W raises IndexError here, before the forward
     was_training = model.training
     model.eval()
     try:
@@ -629,7 +644,4 @@ def classify_and_register(model, pc, intensity, sn, node_a, node_b, img, K, chun
                 del out
     finally:
         model.train(was_training)
-    reg = frustum.register_batch(pc.contiguous(), coarse_pred, N, K, H, W, n_inits=n_inits, seed=seed, t_lb=t_lb,
-                                 t_ub=t_ub, is_2d=True)
-    return dict(P=reg["P"], cost=reg["cost"], coarse_pred=coarse_pred, fine_pred=fine_pred,
-                degenerate=reg["degenerate"])
+    return coarse_pred, fine_pred

@@ -587,6 +587,11 @@ int image_assemble_u8(const uint8_t* src, size_t src_bytes, const int64_t* offse
  * classifier_loss_backward_f32: grad_coarse [B][2][N] and grad_fine [B][L][N] f32 (either may be NULL), contiguous,
  *   for the upstream gradients grad_loss, grad_coarse_loss, grad_fine_loss (each a [dev] f32 scalar) of the
  *   forward's three losses, from its labels, lse and n_inside_total.
+ * classifier_prediction_accuracy_f32 (DESIGN.md 4.35): the forward's label pass compared with given predictions
+ *   coarse_pred int8 [B][N] and fine_pred int32 [B][N] (NULL: coarse only).  Writes int32 n_inside [B],
+ *   coarse_correct [B] (pred == label over all N points) and fine_correct [B] (pred == label over the inside points;
+ *   with fine_pred only), and, where not NULL, coarse_labels int8 [B][N] and fine_labels int32 [B][N].  The grid
+ *   check on H_f, W_f applies when fine_pred or fine_labels is given.  One launch; no workspace.
  * ------------------------------------------------------------------------------------------ */
 size_t classifier_loss_workspace_bytes(int B, int N);
 int classifier_loss_forward_f32(const float* coarse, int64_t coarse_batch_stride, const float* fine,
@@ -603,6 +608,11 @@ int classifier_loss_backward_f32(const float* coarse, int64_t coarse_batch_strid
                                  const float* grad_loss, const float* grad_coarse_loss, const float* grad_fine_loss,
                                  double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
                                  float* grad_coarse, float* grad_fine, dib_stream_t stream);
+int classifier_prediction_accuracy_f32(const float* pc, const double* P12, const double* K9, const int8_t* coarse_pred,
+                                       const int32_t* fine_pred, int B, int N, double H, double W, double fine_scale,
+                                       int H_f, int W_f, int8_t* coarse_labels, int32_t* fine_labels,
+                                       int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
+                                       dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Batched JPEG decoding (the Oxford and nuScenes loaders' Image.open(<frame>.jpg)).  DESIGN.md 4.19 states the

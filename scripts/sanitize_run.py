@@ -111,5 +111,17 @@ if which in ("all", "icp"):
     init = torch.from_numpy(np.stack([np.concatenate([fr["P_gt"][None], icp.random_inits(1, 2, s)[0]]) for s in range(3)])).cuda()
     o = icp.icp_register_batch(src, n_src, tgt, m_tgt, init, max_iteration=8, return_all=True)
     print("icp", o["best"].cpu().tolist(), o["stats"][..., 0].cpu().tolist())
+if which in ("all", "accuracy"):
+    from deepi2p_b200 import classifier
+    rng = np.random.default_rng(2)
+    for S, N, fine in ((2, 1537, True), (3, 5, True), (1, 700, False)):    # N off the CTA's 512-point stride
+        pc = torch.from_numpy(rng.uniform(-20, 20, (S, 3, N)).astype(np.float32)).cuda()
+        P = torch.eye(4, dtype=torch.float64).repeat(S, 1, 1).cuda()
+        K = torch.tensor([[300.0, 0, 256], [0, 300.0, 80], [0, 0, 1]], dtype=torch.float64).repeat(S, 1, 1).cuda()
+        cp = torch.from_numpy(rng.integers(0, 2, (S, N)).astype(np.int8)).cuda()
+        fp = torch.from_numpy(rng.integers(0, 80, (S, N)).astype(np.int32)).cuda() if fine else None
+        a = classifier.prediction_accuracy(pc, P, K, 160, 512, cp, fp, return_labels=S != 3)
+        print("accuracy", a["n_inside"].cpu().tolist(), a["coarse_correct"].cpu().tolist(),
+              None if a["fine_correct"] is None else a["fine_correct"].cpu().tolist())
 torch.cuda.synchronize()
 print("done")
