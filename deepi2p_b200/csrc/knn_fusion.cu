@@ -25,6 +25,7 @@
 #include "common.cuh"
 #include "nearest_k.cuh"
 #include "tf32_mma.cuh"
+#include "tf32_pack.cuh"
 
 namespace dib {
 
@@ -143,15 +144,9 @@ __global__ void __launch_bounds__(kKfThreads, 1) kf_kernel(const __grid_constant
 #pragma unroll
           for (int nt = 0; nt < 4; ++nt) {
             const int n = nt * 8 + 2 * t4 + (i & 1);
-            float v = acc[mt][nt][i];
-            if (split) {
-              const int g = n / Kg;
-              if (g < G) v += proj[m * G + g];
-            }
-            v += bias;
-            if (L.relu) v = v < 0.f ? 0.f : v;             // NaN < 0 is false: NaN stays, as torch.relu
-            if (m >= L.C) v = 0.f;                         // padding rows feed zero weights: keep them finite
-            out[m * kKfStride + n] = last ? v : tf32_rna(v);
+            // the projected max of the column's node comes in like a bias
+            out[m * kKfStride + n] = layer_value(acc[mt][nt][i], split && n / Kg < G,
+                                                 [&] { return proj[m * G + n / Kg]; }, bias, L.relu, m >= L.C, last);
           }
         }
       }
@@ -190,38 +185,12 @@ __global__ void kf_max_kernel(const float* __restrict__ partial, int tiles, int 
   out[i] = v;
 }
 
-// W [C_out][ld] columns [col0, col0 + K) -> the A-fragment order with KT k tiles, rounded to TF32, zero padding
-__global__ void kf_pack_kernel(const float* __restrict__ W, int ld, int col0, int C_out, int K, int KT, int total,
-                               float* __restrict__ out) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= total) return;
-  int row, col;
-  a_frag_row_col(e, KT, row, col);
-  out[e] = row < C_out && col < K ? tf32_rna(W[(size_t)row * ld + col0 + col]) : 0.f;
-}
-
-// W [C_out][ld] columns [0, K) -> transposed [K][Cpad], rounded to TF32, zero padding; and the bias padded to Cpad
-__global__ void kf_pack_t_kernel(const float* __restrict__ W, int ld, int C_out, int K, int Cpad,
-                                 float* __restrict__ out) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= K * Cpad) return;
-  const int c = e / Cpad, m = e - c * Cpad;
-  out[e] = m < C_out ? tf32_rna(W[(size_t)m * ld + c]) : 0.f;
-}
-
-__global__ void kf_bias_kernel(const float* __restrict__ b, int C, int Cpad, float* __restrict__ out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < Cpad) out[c] = c < C && b != nullptr ? b[c] : 0.f;
-}
-
 // Where every layer lives in the packed buffer (floats); a function of the widths alone.
 struct KfPlan {
   int c_in, c_in_pad, n_layers, n_before;
-  int C[kKfMaxLayers], Cpad[kKfMaxLayers], KT[kKfMaxLayers], relu[kKfMaxLayers];
-  size_t w_off[kKfMaxLayers], b_off[kKfMaxLayers], projT_off, packed_floats;
+  PackedLayer layer[kKfMaxLayers];
+  size_t projT_off, packed_floats;
 };
-
-static inline int kf_pad(int x, int m) { return (x + m - 1) / m * m; }
 
 // n_after = 0: a plain chain of n_before layers (pointwise_mlp_max)
 static int kf_plan(const char* who, int c_in, const int64_t* layers, int n_before, int n_after, KfPlan* pl) {
@@ -230,50 +199,31 @@ static int kf_plan(const char* who, int c_in, const int64_t* layers, int n_befor
               "%s: need 1 to 3 layers on each side of the max", who);
   DIB_REQUIRE(c_in >= 1 && c_in <= kKfMaxWidth, "%s: need 1 <= input rows <= 512", who);
   pl->c_in = c_in;
-  pl->c_in_pad = kf_pad(c_in, 8);
+  pl->c_in_pad = pad_to(c_in, 8);
   pl->n_layers = n_before + n_after;
   pl->n_before = n_before;
   size_t off = 0;
-  for (int l = 0; l < pl->n_layers; ++l) {
-    const int64_t* d = layers + (size_t)l * DIB_MLP_LAYER;
-    DIB_REQUIRE(d[DIB_MLP_LAYER_COUT] >= 1 && d[DIB_MLP_LAYER_COUT] <= kKfMaxWidth,
-                "%s: a layer needs 1 <= C_out <= 512", who);
-    DIB_REQUIRE(d[DIB_MLP_LAYER_RELU] == 0 || d[DIB_MLP_LAYER_RELU] == 1, "%s: relu must be 0 or 1", who);
-    pl->C[l] = (int)d[DIB_MLP_LAYER_COUT];
-    pl->Cpad[l] = kf_pad(pl->C[l], 16);
-    pl->relu[l] = (int)d[DIB_MLP_LAYER_RELU];
-    pl->KT[l] = (l == 0 ? pl->c_in_pad : pl->Cpad[l - 1]) / 8;
-    pl->w_off[l] = off;
-    off += (size_t)pl->Cpad[l] * pl->KT[l] * 8;
-    pl->b_off[l] = off;
-    off += pl->Cpad[l];
-  }
+  const int rc = plan_packed_layers(who, kKfMaxWidth, layers, pl->n_layers, pl->c_in_pad, &off, pl->layer);
+  if (rc != DIB_OK) return rc;
   pl->projT_off = off;
-  if (n_after > 0) off += (size_t)pl->C[n_before - 1] * pl->Cpad[n_before];
+  if (n_after > 0) off += (size_t)pl->layer[n_before - 1].C * pl->layer[n_before].Cpad;
   pl->packed_floats = off;
   return DIB_OK;
 }
 
 static int kf_pack(const char* who, const KfPlan& pl, const int64_t* layers, float* out, cudaStream_t stream) {
   for (int l = 0; l < pl.n_layers; ++l) {
+    const PackedLayer& L = pl.layer[l];
     const int64_t* d = layers + (size_t)l * DIB_MLP_LAYER;
     const float* W = (const float*)(uintptr_t)d[DIB_MLP_LAYER_W];
-    const float* bias = (const float*)(uintptr_t)d[DIB_MLP_LAYER_B];
     DIB_REQUIRE(W != nullptr, "%s: a layer's W is NULL", who);
-    const int K = l == 0 ? pl.c_in : pl.C[l - 1];
+    const int K = l == 0 ? pl.c_in : pl.layer[l - 1].C;
     const bool split = l == pl.n_before;                   // W = [W_p | W_x], [C_out][2 C_before]
     const int ld = split ? 2 * K : K;
-    const int total = pl.Cpad[l] * pl.KT[l] * 8;
-    kf_pack_kernel<<<(total + 255) / 256, 256, 0, stream>>>(W, ld, split ? K : 0, pl.C[l], K, pl.KT[l], total,
-                                                            out + pl.w_off[l]);
-    DIB_CHECK_CUDA(cudaGetLastError());
-    if (split) {
-      const int tt = K * pl.Cpad[l];
-      kf_pack_t_kernel<<<(tt + 255) / 256, 256, 0, stream>>>(W, ld, pl.C[l], K, pl.Cpad[l], out + pl.projT_off);
-      DIB_CHECK_CUDA(cudaGetLastError());
-    }
-    kf_bias_kernel<<<(pl.Cpad[l] + 255) / 256, 256, 0, stream>>>(bias, pl.C[l], pl.Cpad[l], out + pl.b_off[l]);
-    DIB_CHECK_CUDA(cudaGetLastError());
+    int r = pack_tf32_a(W, ld, L.C, L.KT, pack_cols(split ? K : 0, K), out + L.w_off, stream);
+    if (r == DIB_OK && split) r = pack_tf32_t(W, ld, 0, L.C, K, L.Cpad, out + pl.projT_off, stream);
+    if (r == DIB_OK) r = pack_bias((const float*)(uintptr_t)d[DIB_MLP_LAYER_B], L.C, L.Cpad, out + L.b_off, stream);
+    if (r != DIB_OK) return r;
   }
   return DIB_OK;
 }
@@ -285,9 +235,10 @@ static void kf_fill_layers(const KfPlan& pl, const float* pk, KfParams& p) {
   p.n_before = pl.n_before;
   int x_rows = pl.c_in_pad, y_rows = 0;
   for (int l = 0; l < pl.n_layers; ++l) {
-    p.layer[l] = KfLayer{pk + pl.w_off[l], pk + pl.b_off[l], pl.C[l], pl.Cpad[l], pl.KT[l], pl.relu[l]};
+    const PackedLayer& L = pl.layer[l];
+    p.layer[l] = KfLayer{pk + L.w_off, pk + L.b_off, L.C, L.Cpad, L.KT, L.relu};
     int& rows = (l & 1) ? x_rows : y_rows;
-    rows = pl.Cpad[l] > rows ? pl.Cpad[l] : rows;
+    rows = L.Cpad > rows ? L.Cpad : rows;
   }
   p.projT = pk + pl.projT_off;
   p.x_floats = x_rows * kKfStride;
@@ -297,7 +248,7 @@ static void kf_fill_layers(const KfPlan& pl, const float* pk, KfParams& p) {
 static int kf_launch(const KfPlan& pl, KfParams& p, int B, int tiles, cudaStream_t stream) {
   size_t floats = (size_t)p.x_floats + p.y_floats;
   if (!p.dense && pl.n_layers > pl.n_before)
-    floats += (size_t)p.G * (pl.C[pl.n_before - 1] + pl.Cpad[pl.n_before]);
+    floats += (size_t)p.G * (pl.layer[pl.n_before - 1].C + pl.layer[pl.n_before].Cpad);
   const size_t smem = floats * sizeof(float);              // <= 2 x 512 x 40 + 2 x 512 x 8 floats = 192 KB
   if (smem > 48 * 1024)
     DIB_CHECK_CUDA(cudaFuncSetAttribute(kf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -428,7 +379,7 @@ int pointwise_mlp_max_f32(const int64_t* sources, int n_sources, const int64_t* 
   DIB_REQUIRE(out != nullptr, "pointwise_mlp_max: out is NULL");
   DIB_REQUIRE(packed && ((uintptr_t)packed & 15) == 0 && packed_bytes >= pl.packed_floats * sizeof(float),
               "pointwise_mlp_max: packed is NULL, misaligned or smaller than pointwise_mlp_max_packed_bytes");
-  const int C_out = pl.C[n_layers - 1];
+  const int C_out = pl.layer[n_layers - 1].C;
   const size_t need = pointwise_mlp_max_workspace_bytes(C_out, B, N);
   DIB_REQUIRE(workspace && ((uintptr_t)workspace & 15) == 0, "pointwise_mlp_max: workspace is NULL or misaligned");
   if (workspace_bytes < need) {

@@ -19,6 +19,7 @@
 
 #include "common.cuh"
 #include "tf32_mma.cuh"
+#include "tf32_pack.cuh"
 
 namespace dib {
 
@@ -31,6 +32,7 @@ constexpr int kNmMaxBcast = 65536;    // per-sample input rows
 constexpr int kNmMaxLayers = 3;
 constexpr int kNmMaxDense = 4;
 constexpr int kNmProjB = 8;           // samples per thread of nm_proj_kernel: each weight is read once per 8 samples
+static_assert(kNmMaxDense <= kPackMaxSegs, "the dense sources are column segments of W1");
 
 struct NmLayer { const float* W; const float* bias; int C; int Cpad; int KT; int relu; };
 struct NmParams {
@@ -96,12 +98,8 @@ __global__ void __launch_bounds__(kNmThreads, 1) nm_kernel(const __grid_constant
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) {
               const int n = nt * 8 + 2 * t4 + (i & 1);
-              float v = acc[h][mt][nt][i];
-              if (proj != nullptr) v += add;
-              v += bias;
-              if (L.relu) v = v < 0.f ? 0.f : v;           // NaN < 0 is false: NaN stays, as torch.relu
-              if (m >= L.C) v = 0.f;                       // padding rows feed zero weights: keep them finite
-              buf[m * kNmStride + n] = last ? v : tf32_rna(v);
+              buf[m * kNmStride + n] = layer_value(acc[h][mt][nt][i], proj != nullptr, [&] { return add; }, bias,
+                                                   L.relu, m >= L.C, last);
             }
           }
         }
@@ -139,51 +137,14 @@ __global__ void nm_proj_kernel(const float* __restrict__ v, long long bstride, i
     if (b0 + j < B) proj[(size_t)(b0 + j) * Cpad + m] = acc[j];
 }
 
-// Dense columns of W [C_out][ld]: dense input row r comes from W's column w_col0[s] + r - row0[s] of the source s that
-// holds it.  Layers after the first have one "source" covering every column.
-struct NmColumns { int n; int row0[kNmMaxDense + 1]; int w_col0[kNmMaxDense]; };
-
-// -> the A-fragment order with KT k tiles, rounded to TF32, zero padding
-__global__ void nm_pack_kernel(const float* __restrict__ W, int ld, NmColumns cols, int C_out, int KT, int total,
-                               float* __restrict__ out) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= total) return;
-  int row, col;
-  a_frag_row_col(e, KT, row, col);
-  float v = 0.f;
-  if (row < C_out && col < cols.row0[cols.n]) {
-    int s = 0;
-    for (int q = 1; q < cols.n; ++q)
-      if (col >= cols.row0[q]) s = q;
-    v = tf32_rna(W[(size_t)row * ld + cols.w_col0[s] + col - cols.row0[s]]);
-  }
-  out[e] = v;
-}
-
-// W [C_out][ld] columns [col0, col0 + K) -> transposed [K][Cpad], rounded to TF32, zero padding
-__global__ void nm_pack_t_kernel(const float* __restrict__ W, int ld, int col0, int C_out, int K, int Cpad,
-                                 float* __restrict__ out) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= K * Cpad) return;
-  const int c = e / Cpad, m = e - c * Cpad;
-  out[e] = m < C_out ? tf32_rna(W[(size_t)m * ld + col0 + c]) : 0.f;
-}
-
-__global__ void nm_bias_kernel(const float* __restrict__ b, int C, int Cpad, float* __restrict__ out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < Cpad) out[c] = c < C && b != nullptr ? b[c] : 0.f;
-}
-
 // Where every layer lives in the packed buffer (floats) and which sources are dense; a function of the source
 // widths, their kinds and the layer widths alone.
 struct NmPlan {
   int n_dense, c_dense, c_dense_pad, c_bcast, c_in, n_layers;
-  NmColumns dense;
-  int C[kNmMaxLayers], Cpad[kNmMaxLayers], KT[kNmMaxLayers], relu[kNmMaxLayers];
-  size_t w_off[kNmMaxLayers], b_off[kNmMaxLayers], wbt_off, packed_floats;
+  PackSegs dense;                     // dense input row r is W1's column dense.col[s] + r - dense.start[s]
+  PackedLayer layer[kNmMaxLayers];
+  size_t wbt_off, packed_floats;
 };
-
-static inline int nm_pad(int x, int m) { return (x + m - 1) / m * m; }
 
 static int nm_plan(const char* who, const int64_t* sources, int n_sources, const int64_t* layers, int n_layers,
                    NmPlan* pl) {
@@ -205,35 +166,23 @@ static int nm_plan(const char* who, const int64_t* sources, int n_sources, const
     } else {
       DIB_REQUIRE(pl->c_dense + C <= kNmMaxWidth, "%s: the dense sources have more than 1024 rows", who);
       DIB_REQUIRE(pl->n_dense < kNmMaxDense, "%s: at most 4 dense sources", who);
-      pl->dense.row0[pl->n_dense] = pl->c_dense;
-      pl->dense.w_col0[pl->n_dense] = c_in;
+      pl->dense.start[pl->n_dense] = pl->c_dense;
+      pl->dense.col[pl->n_dense] = c_in;
       ++pl->n_dense;
       pl->c_dense += C;
     }
     c_in += C;
   }
   pl->dense.n = pl->n_dense;
-  pl->dense.row0[pl->n_dense] = pl->c_dense;
+  pl->dense.start[pl->n_dense] = pl->c_dense;
   pl->c_in = c_in;
-  pl->c_dense_pad = nm_pad(pl->c_dense, 8);
+  pl->c_dense_pad = pad_to(pl->c_dense, 8);
   pl->n_layers = n_layers;
   size_t off = 0;
-  for (int l = 0; l < n_layers; ++l) {
-    const int64_t* d = layers + (size_t)l * DIB_MLP_LAYER;
-    DIB_REQUIRE(d[DIB_MLP_LAYER_COUT] >= 1 && d[DIB_MLP_LAYER_COUT] <= kNmMaxWidth,
-                "%s: a layer needs 1 <= C_out <= 1024", who);
-    DIB_REQUIRE(d[DIB_MLP_LAYER_RELU] == 0 || d[DIB_MLP_LAYER_RELU] == 1, "%s: relu must be 0 or 1", who);
-    pl->C[l] = (int)d[DIB_MLP_LAYER_COUT];
-    pl->Cpad[l] = nm_pad(pl->C[l], 16);
-    pl->relu[l] = (int)d[DIB_MLP_LAYER_RELU];
-    pl->KT[l] = (l == 0 ? pl->c_dense_pad : pl->Cpad[l - 1]) / 8;
-    pl->w_off[l] = off;
-    off += (size_t)pl->Cpad[l] * pl->KT[l] * 8;
-    pl->b_off[l] = off;
-    off += pl->Cpad[l];
-  }
+  const int rc = plan_packed_layers(who, kNmMaxWidth, layers, n_layers, pl->c_dense_pad, &off, pl->layer);
+  if (rc != DIB_OK) return rc;
   pl->wbt_off = off;
-  off += (size_t)pl->c_bcast * pl->Cpad[0];
+  off += (size_t)pl->c_bcast * pl->layer[0].Cpad;
   pl->packed_floats = off;
   return DIB_OK;
 }
@@ -241,40 +190,27 @@ static int nm_plan(const char* who, const int64_t* sources, int n_sources, const
 static int nm_pack(const NmPlan& pl, const int64_t* sources, int n_sources, const int64_t* layers, float* out,
                    cudaStream_t stream) {
   for (int l = 0; l < pl.n_layers; ++l) {
+    const PackedLayer& L = pl.layer[l];
     const int64_t* d = layers + (size_t)l * DIB_MLP_LAYER;
     const float* W = (const float*)(uintptr_t)d[DIB_MLP_LAYER_W];
-    const float* bias = (const float*)(uintptr_t)d[DIB_MLP_LAYER_B];
     DIB_REQUIRE(W != nullptr, "node_mlp_pack: a layer's W is NULL");
-    const int ld = l == 0 ? pl.c_in : pl.C[l - 1];
-    NmColumns cols = {};
-    if (l == 0) {
-      cols = pl.dense;
-    } else {
-      cols.n = 1;
-      cols.row0[1] = ld;
-    }
-    const int total = pl.Cpad[l] * pl.KT[l] * 8;
-    if (total > 0) {
-      nm_pack_kernel<<<(total + 255) / 256, 256, 0, stream>>>(W, ld, cols, pl.C[l], pl.KT[l], total,
-                                                              out + pl.w_off[l]);
-      DIB_CHECK_CUDA(cudaGetLastError());
-    }
+    const int ld = l == 0 ? pl.c_in : pl.layer[l - 1].C;
+    int r = pack_tf32_a(W, ld, L.C, L.KT, l == 0 ? pl.dense : pack_cols(0, ld), out + L.w_off, stream);
+    if (r != DIB_OK) return r;
     if (l == 0) {                                          // the broadcast columns, transposed, in input order
       for (int s = 0, col = 0, row = 0; s < n_sources; ++s) {
         const int64_t* d = sources + (size_t)s * DIB_MLP_SRC;
         const int C = (int)d[DIB_MLP_SRC_CHANNELS];
         if (d[DIB_MLP_SRC_BCAST]) {
-          const int tt = C * pl.Cpad[0];
-          nm_pack_t_kernel<<<(tt + 255) / 256, 256, 0, stream>>>(W, ld, col, pl.C[0], C, pl.Cpad[0],
-                                                                 out + pl.wbt_off + (size_t)row * pl.Cpad[0]);
-          DIB_CHECK_CUDA(cudaGetLastError());
+          r = pack_tf32_t(W, ld, col, L.C, C, L.Cpad, out + pl.wbt_off + (size_t)row * L.Cpad, stream);
+          if (r != DIB_OK) return r;
           row += C;
         }
         col += C;
       }
     }
-    nm_bias_kernel<<<(pl.Cpad[l] + 255) / 256, 256, 0, stream>>>(bias, pl.C[l], pl.Cpad[l], out + pl.b_off[l]);
-    DIB_CHECK_CUDA(cudaGetLastError());
+    r = pack_bias((const float*)(uintptr_t)d[DIB_MLP_LAYER_B], L.C, L.Cpad, out + L.b_off, stream);
+    if (r != DIB_OK) return r;
   }
   return DIB_OK;
 }
@@ -315,7 +251,7 @@ int node_mlp_pack_f32(const int64_t* sources, int n_sources, const int64_t* laye
 size_t node_mlp_workspace_bytes(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, int B) {
   dib::NmPlan pl;
   if (B < 1 || dib::nm_plan("node_mlp", sources, n_sources, layers, n_layers, &pl) != DIB_OK) return 0;
-  return pl.c_bcast > 0 ? (size_t)B * pl.Cpad[0] * sizeof(float) : 0;
+  return pl.c_bcast > 0 ? (size_t)B * pl.layer[0].Cpad * sizeof(float) : 0;
 }
 
 int node_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, const void* packed,
@@ -340,10 +276,11 @@ int node_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, i
   DIB_REQUIRE(packed && ((uintptr_t)packed & 15) == 0 && packed_bytes >= pl.packed_floats * sizeof(float),
               "node_mlp: packed is NULL, misaligned or smaller than node_mlp_packed_bytes");
   const float* pk = (const float*)packed;
+  const int Cpad0 = pl.layer[0].Cpad;
   float* proj = nullptr;
   if (pl.c_bcast > 0) {
     DIB_REQUIRE(workspace && ((uintptr_t)workspace & 15) == 0, "node_mlp: workspace is NULL or misaligned");
-    if (workspace_bytes < (size_t)B * pl.Cpad[0] * sizeof(float)) {
+    if (workspace_bytes < (size_t)B * Cpad0 * sizeof(float)) {
       set_error("node_mlp: workspace too small");
       return DIB_ENOMEM;
     }
@@ -352,11 +289,10 @@ int node_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, i
       const int64_t* d = sources + (size_t)s * DIB_MLP_SRC;
       if (!d[DIB_MLP_SRC_BCAST]) continue;
       const int C = (int)d[DIB_MLP_SRC_CHANNELS];
-      const dim3 grid((pl.Cpad[0] + 255) / 256, (B + kNmProjB - 1) / kNmProjB);
+      const dim3 grid((Cpad0 + 255) / 256, (B + kNmProjB - 1) / kNmProjB);
       nm_proj_kernel<<<grid, 256, 0, stream>>>((const float*)(uintptr_t)d[DIB_MLP_SRC_DATA],
                                                (long long)d[DIB_MLP_SRC_BSTRIDE], C,
-                                               pk + pl.wbt_off + (size_t)row * pl.Cpad[0], pl.Cpad[0], B, row == 0,
-                                               proj);
+                                               pk + pl.wbt_off + (size_t)row * Cpad0, Cpad0, B, row == 0, proj);
       DIB_CHECK_CUDA(cudaGetLastError());
       row += C;
     }
@@ -367,7 +303,7 @@ int node_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, i
     if (d[DIB_MLP_SRC_BCAST]) continue;
     p.src[k] = (const float*)(uintptr_t)d[DIB_MLP_SRC_DATA];
     p.bstride[k] = (long long)d[DIB_MLP_SRC_BSTRIDE];
-    p.src_row0[k] = pl.dense.row0[k];
+    p.src_row0[k] = pl.dense.start[k];
     ++k;
   }
   p.src_row0[pl.n_dense] = pl.c_dense;
@@ -377,9 +313,10 @@ int node_mlp_f32(const int64_t* sources, int n_sources, const int64_t* layers, i
   p.n_layers = pl.n_layers;
   int rows = pl.c_dense_pad, widest = 0;
   for (int l = 0; l < pl.n_layers; ++l) {
-    p.layer[l] = NmLayer{pk + pl.w_off[l], pk + pl.b_off[l], pl.C[l], pl.Cpad[l], pl.KT[l], pl.relu[l]};
-    rows = pl.Cpad[l] > rows ? pl.Cpad[l] : rows;
-    widest = pl.Cpad[l] > widest ? pl.Cpad[l] : widest;
+    const PackedLayer& L = pl.layer[l];
+    p.layer[l] = NmLayer{pk + L.w_off, pk + L.b_off, L.C, L.Cpad, L.KT, L.relu};
+    rows = L.Cpad > rows ? L.Cpad : rows;
+    widest = L.Cpad > widest ? L.Cpad : widest;
   }
   p.proj = proj;
   p.out = out;

@@ -3,8 +3,9 @@
 // input the virtual concatenation of dense sources and interpolated node features, and the arg-max of network.predict
 // as an output mode.  Nothing wider than the sources and the predictions touches global memory.
 //
-//   mlp_pack_kernel   W [C_out][ld] f32 -> the m16n8k8 A-fragment order [m tile][k tile][lane][4], each weight rounded
-//                     to TF32 once (tf32_rna), zero in the padding.  A lane's fragment is one 16-byte load.
+//   packing           (tf32_pack.cu) W [C_out][ld] f32 -> the m16n8k8 A-fragment order [m tile][k tile][lane][4],
+//                     each weight rounded to TF32 once (tf32_rna), zero in the padding.  A lane's fragment is one
+//                     16-byte load.
 //   mlp_kernel        CTA = 64 points of one sample, 8 warps as 4 (output channels, 64 each) x 2 (points, 32 each).
 //                     Layer 1:  z = W1[:, dense rows] x  (tensor cores; the dense rows staged 64 at a time, rounded to
 //                     TF32)  +  sum over interpolated sources s, neighbours j of w_sj P_s[idx_sj]  (f32 fma chain in
@@ -24,6 +25,7 @@
 
 #include "common.cuh"
 #include "tf32_mma.cuh"
+#include "tf32_pack.cuh"
 
 namespace dib {
 
@@ -37,6 +39,7 @@ constexpr int kMlpMaxSources = 4;
 constexpr int kMlpMaxLayers = 3;
 constexpr int kMlpMaxK = 8;
 constexpr int kMlpMaxNodes = 2048;
+static_assert(kMlpMaxSources <= kPackMaxSegs, "the dense sources are column segments of W1");
 
 enum { kOutActivations = 0, kOutTransposed = 1, kOutArgmax = 2 };
 
@@ -146,7 +149,8 @@ __global__ void __launch_bounds__(kMlpThreads, 2) mlp_kernel(const __grid_consta
       const int KT = p.layer[l - 1].Cpad >> 3;
       mma_block_64x32<kMlpStride>(acc, in, Wp, KT, MT, 0, KT, wm, n_base, lane);
     }
-    if (l == 0 && p.n_interp > 0) __syncthreads();             // the gathered tile is complete (and visible)
+    const bool interp = l == 0 && p.n_interp > 0;
+    if (interp) __syncthreads();                               // the gathered tile is complete (and visible)
     float* out = (l & 1) ? bufB : bufA;
     const bool last = l == p.n_layers - 1;
 #pragma unroll
@@ -159,12 +163,8 @@ __global__ void __launch_bounds__(kMlpThreads, 2) mlp_kernel(const __grid_consta
 #pragma unroll
           for (int nt = 0; nt < 4; ++nt) {
             const int n = n_base + nt * 8 + 2 * t + (i & 1);
-            float v = acc[mt][nt][i];
-            if (l == 0 && p.n_interp > 0) v += bufB[n * IS + m];
-            v += bias;
-            if (L.relu) v = v < 0.f ? 0.f : v;                 // NaN < 0 is false: NaN stays, as torch.relu
-            if (m >= L.C) v = 0.f;                             // padding rows feed zero weights: keep them finite
-            out[m * kMlpStride + n] = last ? v : tf32_rna(v);
+            out[m * kMlpStride + n] = layer_value(acc[mt][nt][i], interp, [&] { return bufB[n * IS + m]; }, bias,
+                                                  L.relu, m >= L.C, last);
           }
         }
       }
@@ -215,40 +215,13 @@ __global__ void __launch_bounds__(kMlpThreads, 2) mlp_kernel(const __grid_consta
   }
 }
 
-// One thread per packed float.  Packed column c of the matrix is column seg_orig[s] + (c - seg_start[s]) of W for the
-// segment s holding c (the dense sources of layer 1 are up to four column ranges of W1).
-struct MlpPackSeg { int start[kMlpMaxSources + 1]; int orig[kMlpMaxSources]; int n; };
-
-__global__ void mlp_pack_kernel(const float* __restrict__ W, int ld, int C_out, int K, int KT, int total,
-                                MlpPackSeg seg, float* __restrict__ out) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= total) return;
-  int row, col;
-  a_frag_row_col(e, KT, row, col);
-  float v = 0.f;
-  if (row < C_out && col < K) {
-    int s = 0;
-    for (int q = 1; q < seg.n; ++q)
-      if (col >= seg.start[q]) s = q;
-    v = tf32_rna(W[(size_t)row * ld + seg.orig[s] + col - seg.start[s]]);
-  }
-  out[e] = v;
-}
-
-__global__ void mlp_bias_kernel(const float* __restrict__ b, int C, int Cpad, float* __restrict__ out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < Cpad) out[c] = c < C && b != nullptr ? b[c] : 0.f;
-}
-
 // Where everything lives in the packed buffer (floats) and the workspace (bytes); a function of the widths alone.
 struct MlpPlan {
   int n_src, n_layers, n_dense, n_interp, Kd, c_in;
   int src_C[kMlpMaxSources], src_M[kMlpMaxSources], src_k[kMlpMaxSources], src_col[kMlpMaxSources];
-  int C[kMlpMaxLayers], Cpad[kMlpMaxLayers], relu[kMlpMaxLayers];
-  size_t proj_off[kMlpMaxSources], w_off[kMlpMaxLayers], b_off[kMlpMaxLayers], packed_floats;
+  PackedLayer layer[kMlpMaxLayers];
+  size_t proj_off[kMlpMaxSources], packed_floats;
 };
-
-static inline int pad_to(int x, int m) { return (x + m - 1) / m * m; }
 
 static int mlp_plan(const int64_t* sources, int n_sources, const int64_t* layers, int n_layers, MlpPlan* pl) {
   DIB_REQUIRE(sources && layers, "pointwise_mlp: NULL descriptor table");
@@ -275,27 +248,21 @@ static int mlp_plan(const int64_t* sources, int n_sources, const int64_t* layers
     }
   }
   DIB_REQUIRE(pl->c_in <= kMlpMaxIn, "pointwise_mlp: the concatenated input has more than 1024 rows");
-  for (int l = 0; l < n_layers; ++l) {
-    const int64_t* d = layers + (size_t)l * DIB_MLP_LAYER;
-    DIB_REQUIRE(d[DIB_MLP_LAYER_COUT] >= 1 && d[DIB_MLP_LAYER_COUT] <= kMlpMaxWidth,
-                "pointwise_mlp: a layer needs 1 <= C_out <= 256");
-    DIB_REQUIRE(d[DIB_MLP_LAYER_RELU] == 0 || d[DIB_MLP_LAYER_RELU] == 1, "pointwise_mlp: relu must be 0 or 1");
-    pl->C[l] = (int)d[DIB_MLP_LAYER_COUT];
-    pl->Cpad[l] = pad_to(pl->C[l], 16);
-    pl->relu[l] = (int)d[DIB_MLP_LAYER_RELU];
-  }
   size_t off = 0;
+  const int rc =
+      plan_packed_layers("pointwise_mlp", kMlpMaxWidth, layers, n_layers, pad_to(pl->Kd, 8), &off, pl->layer);
+  if (rc != DIB_OK) return rc;
+  // the interpolated sources' blocks of W1 come first, then the layers
+  size_t proj = 0;
   for (int s = 0; s < n_sources; ++s) {
-    pl->proj_off[s] = off;
-    if (pl->src_M[s] > 0) off += (size_t)pl->Cpad[0] * pad_to(pl->src_C[s], 8);
+    pl->proj_off[s] = proj;
+    if (pl->src_M[s] > 0) proj += (size_t)pl->layer[0].Cpad * pad_to(pl->src_C[s], 8);
   }
   for (int l = 0; l < n_layers; ++l) {
-    pl->w_off[l] = off;
-    off += (size_t)pl->Cpad[l] * (l == 0 ? pad_to(pl->Kd, 8) : pl->Cpad[l - 1]);
-    pl->b_off[l] = off;
-    off += pl->Cpad[l];
+    pl->layer[l].w_off += proj;
+    pl->layer[l].b_off += proj;
   }
-  pl->packed_floats = off;
+  pl->packed_floats = proj + off;
   return DIB_OK;
 }
 
@@ -342,43 +309,34 @@ int pointwise_mlp_pack_f32(const int64_t* sources, int n_sources, const int64_t*
     return DIB_ENOMEM;
   }
   float* out = (float*)packed;
-  // K columns of W packed into KT >= ceil(K / 8) k tiles (the kernel's count for this matrix)
-  auto pack = [&](const float* W, int ld, int C_out, int K, int KT, const MlpPackSeg& seg, float* dst) -> int {
-    const int total = pad_to(C_out, 16) * KT * 8;
-    if (total == 0) return DIB_OK;
-    mlp_pack_kernel<<<(total + 255) / 256, 256, 0, stream>>>(W, ld, C_out, K, KT, total, seg, dst);
-    DIB_CHECK_CUDA(cudaGetLastError());
-    return DIB_OK;
-  };
   for (int l = 0; l < n_layers; ++l) {
+    const PackedLayer& L = pl.layer[l];
     const int64_t* d = layers + (size_t)l * DIB_MLP_LAYER;
     const float* W = (const float*)(uintptr_t)d[DIB_MLP_LAYER_W];
-    const float* bias = (const float*)(uintptr_t)d[DIB_MLP_LAYER_B];
     DIB_REQUIRE(W != nullptr, "pointwise_mlp_pack: a layer's W is NULL");
-    MlpPackSeg seg = {};
+    int r;
     if (l == 0) {
+      PackSegs dense = {};
       for (int s = 0; s < n_sources; ++s) {
         if (pl.src_M[s] > 0) {
-          MlpPackSeg one = {};
-          one.n = 1; one.orig[0] = pl.src_col[s];
-          const int r = pack(W, pl.c_in, pl.C[0], pl.src_C[s], pad_to(pl.src_C[s], 8) / 8, one, out + pl.proj_off[s]);
+          r = pack_tf32_a(W, pl.c_in, L.C, pad_to(pl.src_C[s], 8) / 8, pack_cols(pl.src_col[s], pl.src_C[s]),
+                          out + pl.proj_off[s], stream);
           if (r != DIB_OK) return r;
         } else {                               // the dense segments start at the running sums of the dense widths
-          seg.orig[seg.n] = pl.src_col[s];
-          seg.start[seg.n + 1] = seg.start[seg.n] + pl.src_C[s];
-          seg.n++;
+          dense.col[dense.n] = pl.src_col[s];
+          dense.start[dense.n + 1] = dense.start[dense.n] + pl.src_C[s];
+          dense.n++;
         }
       }
-      const int r = pack(W, pl.c_in, pl.C[0], pl.Kd, pad_to(pl.Kd, 8) / 8, seg, out + pl.w_off[0]);
-      if (r != DIB_OK) return r;
+      r = pack_tf32_a(W, pl.c_in, L.C, L.KT, dense, out + L.w_off, stream);
     } else {
       // rows [C, Cpad) of the previous layer are zero activations; their weight columns are zero padding
-      seg.n = 1;
-      const int r = pack(W, pl.C[l - 1], pl.C[l], pl.C[l - 1], pl.Cpad[l - 1] / 8, seg, out + pl.w_off[l]);
-      if (r != DIB_OK) return r;
+      const int K = pl.layer[l - 1].C;
+      r = pack_tf32_a(W, K, L.C, L.KT, pack_cols(0, K), out + L.w_off, stream);
     }
-    mlp_bias_kernel<<<(pl.Cpad[l] + 255) / 256, 256, 0, stream>>>(bias, pl.C[l], pl.Cpad[l], out + pl.b_off[l]);
-    DIB_CHECK_CUDA(cudaGetLastError());
+    if (r != DIB_OK) return r;
+    r = pack_bias((const float*)(uintptr_t)d[DIB_MLP_LAYER_B], L.C, L.Cpad, out + L.b_off, stream);
+    if (r != DIB_OK) return r;
   }
   return DIB_OK;
 }
@@ -388,7 +346,7 @@ size_t pointwise_mlp_workspace_bytes(const int64_t* sources, int n_sources, cons
   dib::MlpPlan pl;
   if (B <= 0 || dib::mlp_plan(sources, n_sources, layers, n_layers, &pl) != DIB_OK) return 0;
   size_t bytes = 0;
-  for (int s = 0; s < n_sources; ++s) bytes += (size_t)B * pl.src_M[s] * pl.Cpad[0] * sizeof(float);
+  for (int s = 0; s < n_sources; ++s) bytes += (size_t)B * pl.src_M[s] * pl.layer[0].Cpad * sizeof(float);
   return bytes;
 }
 
@@ -401,7 +359,7 @@ int pointwise_mlp_f32(const int64_t* sources, int n_sources, const int64_t* laye
   const int rc = mlp_plan(sources, n_sources, layers, n_layers, &pl);
   if (rc != DIB_OK) return rc;
   DIB_REQUIRE(B >= 0 && B <= 65535 && N >= 0, "pointwise_mlp: need 0 <= B <= 65535 and N >= 0");
-  const int C_last = pl.C[n_layers - 1];
+  const int C_last = pl.layer[n_layers - 1].C;
   DIB_REQUIRE(c_split >= 0 && c_split <= C_last && c_split <= 128,
               "pointwise_mlp: need 0 <= c_split <= min(C_out, 128) (0 selects the activations)");
   if (B == 0 || N == 0) return DIB_OK;
@@ -436,13 +394,13 @@ int pointwise_mlp_f32(const int64_t* sources, int n_sources, const int64_t* laye
       q.N = pl.src_M[s];
       q.n_dense = 1; q.Kd = pl.src_C[s]; q.n_layers = 1;
       q.dense[0] = MlpDense{data, (long long)d[DIB_MLP_SRC_BSTRIDE], pl.src_C[s], 0};
-      q.layer[0] = MlpLayer{pk + pl.proj_off[s], nullptr, pl.C[0], pl.Cpad[0], 0};
+      q.layer[0] = MlpLayer{pk + pl.proj_off[s], nullptr, pl.layer[0].C, pl.layer[0].Cpad, 0};
       q.out_mode = kOutTransposed;
       q.out = (float*)ws;
       const int r = mlp_launch(q, B, stream);
       if (r != DIB_OK) return r;
       p.interp[p.n_interp++] = MlpInterp{(const float*)ws, w, idx, pl.src_M[s], pl.src_k[s]};
-      ws += (size_t)B * pl.src_M[s] * pl.Cpad[0] * sizeof(float);
+      ws += (size_t)B * pl.src_M[s] * pl.layer[0].Cpad * sizeof(float);
     } else {
       DIB_REQUIRE(d[DIB_MLP_SRC_BSTRIDE] >= (int64_t)pl.src_C[s] * N,
                   "pointwise_mlp: a source's batch stride is smaller than channels x N");
@@ -452,8 +410,10 @@ int pointwise_mlp_f32(const int64_t* sources, int n_sources, const int64_t* laye
     }
   }
   p.n_layers = n_layers;
-  for (int l = 0; l < n_layers; ++l)
-    p.layer[l] = MlpLayer{pk + pl.w_off[l], pk + pl.b_off[l], pl.C[l], pl.Cpad[l], pl.relu[l]};
+  for (int l = 0; l < n_layers; ++l) {
+    const PackedLayer& L = pl.layer[l];
+    p.layer[l] = MlpLayer{pk + L.w_off, pk + L.b_off, L.C, L.Cpad, L.relu};
+  }
   p.out_mode = c_split == 0 ? kOutActivations : kOutArgmax;
   p.c_split = c_split;
   p.out = out;

@@ -1,6 +1,7 @@
-// TF32 tensor-core helpers shared by the fused per-point chains (pointwise_mlp.cu, knn_fusion.cu; DESIGN.md 4.21,
-// 4.26): the operand rounding rule, the m16n8k8 instruction, the A-fragment order weights are packed in, and the
-// warp's 64-row x 32-column product over activations kept in shared memory.
+// TF32 tensor-core helpers shared by the fused per-point chains (pointwise_mlp.cu, knn_fusion.cu, node_mlp.cu,
+// point_chain.cu; DESIGN.md 4.21): the operand rounding rule, the m16n8k8 instruction, the A-fragment order weights
+// are packed in (by tf32_pack.cu), the warp's 64-row x 32-column product over activations kept in shared memory, and
+// the value a layer stores between layers.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -70,6 +71,19 @@ __device__ __forceinline__ void mma_block_64x32(float (&acc)[4][4][4], const flo
 #pragma unroll
     for (int mt = 0; mt < 4; ++mt) a[mt] = an[mt];
   }
+}
+
+// The value a fused layer stores for one output row and column: the product v, plus add() when has_add (read only
+// then), plus the bias; ReLU keeps NaN (NaN < 0 is false), as torch.relu; a padding row (m >= C) is zero, since it
+// feeds zero weights and must stay finite; rounded to TF32 unless it is the chain's last layer.
+template <class Add>
+__device__ __forceinline__ float layer_value(float v, bool has_add, Add add, float bias, bool relu, bool padding,
+                                             bool last) {
+  if (has_add) v += add();
+  v += bias;
+  if (relu) v = v < 0.f ? 0.f : v;
+  if (padding) v = 0.f;
+  return last ? v : tf32_rna(v);
 }
 
 }  // namespace dib

@@ -560,50 +560,56 @@ def _mlp_source_shapes(sources):
     return spec, B, N
 
 
-def _mlp_layer_widths(layers, c_in):
-    """[(C_out, relu)] of a list of (W [C_out,C_in], b [C_out] or None, relu); ValueError on a bad width."""
-    if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= MLP_MAX_LAYERS:
-        raise ValueError(f"layers: need a list of 1 to {MLP_MAX_LAYERS} layers")
+def _layer_widths(layers, c_in, max_width, name, lo, hi):
+    """[(C_out, relu)] of lo to hi layers (W [C_out,C_in], b [C_out] or None, relu), widths in [1, max_width];
+    ValueError otherwise.  The first layer takes c_in rows."""
+    if not isinstance(layers, (list, tuple)) or not lo <= len(layers) <= hi:
+        raise ValueError(f"{name}: need a list of {lo} to {hi} layers")
     meta = []
     for i, layer in enumerate(layers):
         if not isinstance(layer, (list, tuple)) or len(layer) != 3:
-            raise ValueError(f"layers[{i}]: need (W, b, relu)")
+            raise ValueError(f"{name}[{i}]: need (W, b, relu)")
         W, b, relu = layer
         if not isinstance(W, torch.Tensor) or W.dim() != 2 or W.shape[1] != c_in:
-            raise ValueError(f"layers[{i}]: W must be [C_out, {c_in}]")
-        if not 1 <= W.shape[0] <= MLP_MAX_WIDTH:
-            raise ValueError(f"layers[{i}]: need 1 <= C_out <= {MLP_MAX_WIDTH}, got {W.shape[0]}")
+            raise ValueError(f"{name}[{i}]: W must be [C_out, {c_in}]")
+        if not 1 <= W.shape[0] <= max_width:
+            raise ValueError(f"{name}[{i}]: need 1 <= C_out <= {max_width}, got {W.shape[0]}")
         if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (W.shape[0],)):
-            raise ValueError(f"layers[{i}]: b must be [{W.shape[0]}] or None")
+            raise ValueError(f"{name}[{i}]: b must be [{W.shape[0]}] or None")
         c_in = W.shape[0]
         meta.append((c_in, bool(relu)))
     return meta
 
 
-def _mlp_tables(spec, meta):
+def _mlp_tables(spec, meta, slots=(2, 3, 6)):
+    """The int64 source and layer tables of the fused ops (DIB_MLP_SRC, DIB_MLP_LAYER rows): each entry of spec in
+    the source slots `slots` (CHANNELS, NODES, K by default), (C_out, relu) per layer; the addresses are filled in by
+    the caller."""
     import numpy as np
     src = np.zeros((len(spec), _MLP_SRC), dtype=np.int64)
-    for i, (C, M, k) in enumerate(spec):
-        src[i, 2], src[i, 3], src[i, 6] = C, M, k
+    for i, row in enumerate(spec):
+        for j, v in zip(slots, row):
+            src[i, j] = v
     lay = np.zeros((len(meta), _MLP_LAYER), dtype=np.int64)
     for i, (C, relu) in enumerate(meta):
         lay[i, 2], lay[i, 3] = C, int(relu)
     return src, lay
 
 
-class PackedPointwiseMLP:
-    """The layers of one pointwise_mlp chain in the kernel's order on the device (weights rounded to TF32 once), for
-    sources of the widths `spec` = [(C, M, k)] (M = k = 0 for a dense source).  pack_pointwise_mlp builds it."""
+class PackedLayers:
+    """The layers of one fused chain in its kernel's order on the device (weights rounded to TF32 once), as
+    pack_pointwise_mlp, pack_knn_fusion, pack_pointwise_mlp_max or pack_node_mlp built them: kind names the op, key
+    the input they were packed for (the source spec of pointwise_mlp and node_mlp, the input rows of knn_fusion and
+    pointwise_mlp_max), meta = [(C_out, relu)] over every layer, n_before of them before knn_fusion's per-node max
+    (all of them for the other ops), packed the device buffer."""
 
-    def __init__(self, spec, meta, packed):
-        self.spec, self.meta, self.packed = list(spec), list(meta), packed
+    def __init__(self, kind, key, meta, n_before, packed):
+        self.kind, self.key, self.meta, self.n_before, self.packed = kind, key, list(meta), n_before, packed
 
 
-def pack_pointwise_mlp(spec, layers):
-    """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] for sources of the widths `spec`
-    (as PackedPointwiseMLP.spec); pointwise_mlp does this itself when given the raw layers."""
-    spec = [tuple(int(v) for v in s) for s in spec]
-    meta = _mlp_layer_widths(layers, sum(c for c, _, _ in spec))
+def _pack(kind, key, layers, meta, lay, args, n_before=None):
+    """Pack `layers` (of the checked widths meta) with lib.<kind>_packed_bytes(*args) and lib.<kind>_pack_f32(*args,
+    packed, bytes, stream), args naming the layer table lay, whose W and b addresses are filled in here."""
     dev = layers[0][0].device
     keep = []
     for W, b, _ in layers:
@@ -611,23 +617,65 @@ def pack_pointwise_mlp(spec, layers):
             if t is None:
                 continue
             if t.requires_grad and torch.is_grad_enabled():
-                raise RuntimeError("pointwise_mlp has no backward: call it under torch.no_grad() or detach the layers")
+                raise RuntimeError(f"{kind} has no backward: call it under torch.no_grad() or detach the layers")
             if not t.is_cuda or t.device != dev or t.dtype != torch.float32:
                 raise RuntimeError("the layers must be float32 CUDA tensors on one device")
         keep.append((W.detach().contiguous(), None if b is None else b.detach().contiguous()))
-    src, lay = _mlp_tables(spec, meta)
     for i, (W, b) in enumerate(keep):
         lay[i, 0], lay[i, 1] = W.data_ptr(), 0 if b is None else b.data_ptr()
     lib = _native.load()
-    need = lib.pointwise_mlp_packed_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta))
+    need = getattr(lib, kind + "_packed_bytes")(*args)
     if need == 0:
-        raise ValueError("pointwise_mlp: " + lib.dib_last_error().decode("utf-8", "replace"))
+        raise ValueError(f"{kind}: " + lib.dib_last_error().decode("utf-8", "replace"))
     with torch.cuda.device(dev):
         packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
-        rc = lib.pointwise_mlp_pack_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.data_ptr(), need,
-                                        _stream_ptr())
-    _native.check(rc, "pointwise_mlp_pack_f32")
-    return PackedPointwiseMLP(spec, meta, packed)
+        rc = getattr(lib, kind + "_pack_f32")(*args, packed.data_ptr(), need, _stream_ptr())
+    _native.check(rc, kind + "_pack_f32")
+    del keep
+    return PackedLayers(kind, key, meta, len(meta) if n_before is None else n_before, packed)
+
+
+def _prepacked(layers, kind, key):
+    """layers if it is a PackedLayers that pack_<kind> built for `key`, None if it is not a PackedLayers; ValueError
+    for layers packed for another op or input."""
+    if not isinstance(layers, PackedLayers):
+        return None
+    if layers.kind != kind or layers.key != key:
+        raise ValueError(f"the layers were packed as {layers.kind} for {layers.key}, need {kind} for {key}")
+    return layers
+
+
+def _check_sources(name, tensors):
+    """RuntimeError unless every tensor is a float32 CUDA tensor on the first one's device, with no gradient to
+    keep (the fused ops have no backward); returns that device."""
+    dev = tensors[0].device
+    for t in tensors:
+        if t.requires_grad and torch.is_grad_enabled():
+            raise RuntimeError(f"{name} has no backward: call it under torch.no_grad() or detach the inputs")
+        if not t.is_cuda or t.device != dev:
+            raise RuntimeError(f"{name}: every input must be a CUDA tensor on {dev}")
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name}: every input must be float32")
+    return dev
+
+
+def _dense_source(s, B, N):
+    """(s, batch stride) of a dense source [B,C,N] (or [B,C] with N = 1) as the kernels read it: rows of N contiguous
+    columns C apart, so a channel slice of a wider contiguous tensor is read in place; any other layout is copied."""
+    C = s.shape[1]
+    if (N > 1 and s.stride(2) != 1) or (C > 1 and s.stride(1) != N) or (B > 1 and s.stride(0) < C * N):
+        s = s.contiguous()
+    return s, s.stride(0) if B > 1 else C * N
+
+
+def pack_pointwise_mlp(spec, layers):
+    """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] for sources of the widths `spec` =
+    [(C, M, k)] (M = k = 0 for a dense source) into a PackedLayers; pointwise_mlp does this itself when given the raw
+    layers."""
+    spec = [tuple(int(v) for v in s) for s in spec]
+    meta = _layer_widths(layers, sum(c for c, _, _ in spec), MLP_MAX_WIDTH, "layers", 1, MLP_MAX_LAYERS)
+    src, lay = _mlp_tables(spec, meta)
+    return _pack("pointwise_mlp", spec, layers, meta, lay, (src.ctypes.data, len(spec), lay.ctypes.data, len(meta)))
 
 
 def pointwise_mlp(sources, layers, output="activations", c_split=None, return_scores=False):
@@ -639,7 +687,7 @@ def pointwise_mlp(sources, layers, output="activations", c_split=None, return_sc
     a wider contiguous tensor is read in place) or a tuple (features [B,C,M], w [B,N,k], idx [B,N,k]) whose rows are
     the interpolation upsample_by_interpolation computes (w, idx from interpolation_weights; k <= 8, M <= 2048, a
     point with idx = -1 has NaN rows).  At most 1024 rows in all.  layers: [(W [C_out,C_in], b [C_out] or None, relu)]
-    with every C_out in [1, 256], or a PackedPointwiseMLP.
+    with every C_out in [1, 256], or a PackedLayers from pack_pointwise_mlp.
 
     output="activations" returns the last layer [B,C_out,N].  output="argmax" returns (int8 [B,N], int32 [B,N] or
     None): the arg-max over channels [0, c_split) and over [c_split, C_out) (None when that range is empty) by
@@ -650,13 +698,9 @@ def pointwise_mlp(sources, layers, output="activations", c_split=None, return_sc
     (NaN stays NaN) and the arg-max are float32.  No backward: an input that requires grad raises RuntimeError unless
     grad mode is off.  Shape and bound errors raise ValueError before anything is launched."""
     spec, B, N = _mlp_source_shapes(sources)
-    if isinstance(layers, PackedPointwiseMLP):
-        if layers.spec != spec:
-            raise ValueError(f"the layers were packed for sources {layers.spec}, got {spec}")
-        packed = layers
-    else:
-        packed = None
-    meta = packed.meta if packed is not None else _mlp_layer_widths(layers, sum(c for c, _, _ in spec))
+    packed = _prepacked(layers, "pointwise_mlp", spec)
+    meta = packed.meta if packed is not None else _layer_widths(layers, sum(c for c, _, _ in spec), MLP_MAX_WIDTH,
+                                                                "layers", 1, MLP_MAX_LAYERS)
     C_out = meta[-1][0]
     if output not in ("activations", "argmax"):
         raise ValueError(f"output must be 'activations' or 'argmax', got {output!r}")
@@ -682,11 +726,9 @@ def pointwise_mlp(sources, layers, output="activations", c_split=None, return_sc
         if isinstance(s, torch.Tensor):
             if s.dtype != torch.float32:
                 raise RuntimeError(f"sources[{i}] must have dtype {torch.float32}")
-            C = s.shape[1]
-            if (N > 1 and s.stride(2) != 1) or (C > 1 and s.stride(1) != N) or (B > 1 and s.stride(0) < C * N):
-                s = s.contiguous()
+            s, src[i, 1] = _dense_source(s, B, N)
             keep.append(s)
-            src[i, 0], src[i, 1] = s.data_ptr(), s.stride(0) if B > 1 else C * N
+            src[i, 0] = s.data_ptr()
         else:
             F, w, idx = s
             if F.dtype != torch.float32 or w.dtype != torch.float32 or idx.dtype != torch.int32:
@@ -727,85 +769,22 @@ KNN_FUSION_MAX_SIDE = 3
 _mlp_max_ws = {}
 
 
-def _chain_widths(layers, c_in, name, lo=1):
-    """[(C_out, relu)] of lo to 3 layers (W [C_out,C_in], b [C_out] or None, relu), widths in [1, 512]; ValueError
-    otherwise.  The first layer takes c_in rows."""
-    if not isinstance(layers, (list, tuple)) or not lo <= len(layers) <= KNN_FUSION_MAX_SIDE:
-        raise ValueError(f"{name}: need a list of {lo} to {KNN_FUSION_MAX_SIDE} layers")
-    meta = []
-    for i, layer in enumerate(layers):
-        if not isinstance(layer, (list, tuple)) or len(layer) != 3:
-            raise ValueError(f"{name}[{i}]: need (W, b, relu)")
-        W, b, relu = layer
-        if not isinstance(W, torch.Tensor) or W.dim() != 2 or W.shape[1] != c_in:
-            raise ValueError(f"{name}[{i}]: W must be [C_out, {c_in}]")
-        if not 1 <= W.shape[0] <= KNN_FUSION_MAX_WIDTH:
-            raise ValueError(f"{name}[{i}]: need 1 <= C_out <= {KNN_FUSION_MAX_WIDTH}, got {W.shape[0]}")
-        if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (W.shape[0],)):
-            raise ValueError(f"{name}[{i}]: b must be [{W.shape[0]}] or None")
-        c_in = W.shape[0]
-        meta.append((c_in, bool(relu)))
-    return meta
-
-
-class PackedChain:
-    """The layers of one knn_fusion or pointwise_mlp_max chain in the kernel's order on the device (weights rounded
-    to TF32 once), for c_in input rows: meta = [(C_out, relu)] over every layer, n_before of them before the per-node
-    max (all of them for pointwise_mlp_max).  pack_knn_fusion and pack_pointwise_mlp_max build it."""
-
-    def __init__(self, kind, c_in, meta, n_before, packed):
-        self.kind, self.c_in, self.meta, self.n_before, self.packed = kind, c_in, list(meta), n_before, packed
-
-
-def _pack_chain(kind, c_in, layers, meta, n_before):
-    dev = layers[0][0].device
-    keep = []
-    for W, b, _ in layers:
-        for t in (W, b):
-            if t is None:
-                continue
-            if t.requires_grad and torch.is_grad_enabled():
-                raise RuntimeError(f"{kind} has no backward: call it under torch.no_grad() or detach the layers")
-            if not t.is_cuda or t.device != dev or t.dtype != torch.float32:
-                raise RuntimeError("the layers must be float32 CUDA tensors on one device")
-        keep.append((W.detach().contiguous(), None if b is None else b.detach().contiguous()))
-    _, lay = _mlp_tables([], meta)
-    for i, (W, b) in enumerate(keep):
-        lay[i, 0], lay[i, 1] = W.data_ptr(), 0 if b is None else b.data_ptr()
-    lib = _native.load()
-    if kind == "knn_fusion":
-        args = (c_in, lay.ctypes.data, n_before, len(meta) - n_before)
-        need = lib.knn_fusion_packed_bytes(*args)
-    else:
-        args = (c_in, lay.ctypes.data, len(meta))
-        need = lib.pointwise_mlp_max_packed_bytes(*args)
-    if need == 0:
-        raise ValueError(f"{kind}: " + lib.dib_last_error().decode("utf-8", "replace"))
-    with torch.cuda.device(dev):
-        packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
-        stream = _stream_ptr()
-        if kind == "knn_fusion":
-            rc = lib.knn_fusion_pack_f32(*args, packed.data_ptr(), need, stream)
-        else:
-            rc = lib.pointwise_mlp_max_pack_f32(*args, packed.data_ptr(), need, stream)
-    _native.check(rc, kind + "_pack_f32")
-    del keep
-    return PackedChain(kind, c_in, meta, n_before, packed)
-
-
 def _knn_fusion_meta(C, before, after):
     if not isinstance(C, int) or not 1 <= C <= KNN_FUSION_MAX_WIDTH - 3:
         raise ValueError(f"knn_fusion: need 1 <= C <= {KNN_FUSION_MAX_WIDTH - 3} feature channels, got {C}")
-    mb = _chain_widths(before, 3 + C, "before")
-    ma = _chain_widths(after, 2 * mb[-1][0], "after")
+    mb = _layer_widths(before, 3 + C, KNN_FUSION_MAX_WIDTH, "before", 1, KNN_FUSION_MAX_SIDE)
+    ma = _layer_widths(after, 2 * mb[-1][0], KNN_FUSION_MAX_WIDTH, "after", 1, KNN_FUSION_MAX_SIDE)
     return mb + ma, len(mb)
 
 
 def pack_knn_fusion(C, before, after):
-    """Pack the folded layers of a kNN fusion module for C feature channels (network.fold_knn_fusion's lists) once;
-    knn_fusion does this itself when given the raw layers."""
+    """Pack the folded layers of a kNN fusion module for C feature channels (network.fold_knn_fusion's lists) once
+    into a PackedLayers; knn_fusion does this itself when given the raw layers."""
     meta, n_before = _knn_fusion_meta(int(C), before, after)
-    return _pack_chain("knn_fusion", 3 + int(C), list(before) + list(after), meta, n_before)
+    c_in = 3 + int(C)
+    _, lay = _mlp_tables([], meta)
+    return _pack("knn_fusion", c_in, list(before) + list(after), meta, lay,
+                 (c_in, lay.ctypes.data, n_before, len(meta) - n_before), n_before)
 
 
 def knn_fusion(query, database, features, K, layers, return_idx=False):
@@ -817,7 +796,7 @@ def knn_fusion(query, database, features, K, layers, return_idx=False):
     query [B,3,M], database [B,3,N], features [B,C,N] float32 CUDA; 1 <= K <= 32, K <= N <= 2048, 3 + C <= 512.
     layers: (before, after), each a list of 1 to 3 (W [C_out,C_in], b [C_out] or None, relu) with every C_out in
     [1, 512] (BatchNorm folded: network.fold_knn_fusion), the first after layer taking 2 C_b rows (max first), or a
-    PackedChain from pack_knn_fusion.  Returns out [B,C_out,M], and knn_group's knn_idx [B,M,K] int32 with
+    PackedLayers from pack_knn_fusion.  Returns out [B,C_out,M], and knn_group's knn_idx [B,M,K] int32 with
     return_idx=True.
 
     TF32 tensor-core products with float32 accumulation whatever torch's TF32 flags say: weights, the grouped values
@@ -839,25 +818,14 @@ def knn_fusion(query, database, features, K, layers, return_idx=False):
         raise ValueError(f"database: need K <= N <= {KNN_MAX_NODES}, got K = {K}, N = {N}")
     if not 1 <= B <= MLP_MAX_BATCH or M < 1:
         raise ValueError(f"need 1 <= B <= {MLP_MAX_BATCH} and M >= 1, got B = {B}, M = {M}")
-    if isinstance(layers, PackedChain):
-        if layers.kind != "knn_fusion" or layers.c_in != 3 + C:
-            raise ValueError(f"the layers were packed as {layers.kind} for {layers.c_in} input rows, need 3 + C = "
-                             f"{3 + C}")
-        packed = layers
+    packed = _prepacked(layers, "knn_fusion", 3 + C)
+    if packed is not None:
         meta, n_before = packed.meta, packed.n_before
     else:
         if not isinstance(layers, (list, tuple)) or len(layers) != 2:
-            raise ValueError("layers: need (before, after) or a PackedChain")
+            raise ValueError("layers: need (before, after) or a PackedLayers")
         meta, n_before = _knn_fusion_meta(C, *layers)
-        packed = None
-    for t in (query, database, features):
-        if t.requires_grad and torch.is_grad_enabled():
-            raise RuntimeError("knn_fusion has no backward: call it under torch.no_grad() or detach the inputs")
-        if t.dtype != torch.float32:
-            raise RuntimeError("query, database and features must be float32")
-        if not t.is_cuda or t.device != features.device:
-            raise RuntimeError("query, database and features must be CUDA tensors on one device")
-    dev = features.device
+    dev = _check_sources("knn_fusion", (features, query, database))
     query, database, features = query.contiguous(), database.contiguous(), features.contiguous()
     if packed is None:
         packed = pack_knn_fusion(C, *layers)
@@ -876,12 +844,14 @@ def knn_fusion(query, database, features, K, layers, return_idx=False):
 
 
 def pack_pointwise_mlp_max(c_in, layers):
-    """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] for c_in input rows once;
-    pointwise_mlp_max does this itself when given the raw layers."""
+    """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] for c_in input rows once into a
+    PackedLayers; pointwise_mlp_max does this itself when given the raw layers."""
     c_in = int(c_in)
     if not 1 <= c_in <= KNN_FUSION_MAX_WIDTH:
         raise ValueError(f"pointwise_mlp_max: need 1 <= input rows <= {KNN_FUSION_MAX_WIDTH}, got {c_in}")
-    return _pack_chain("pointwise_mlp_max", c_in, layers, _chain_widths(layers, c_in, "layers"), len(layers))
+    meta = _layer_widths(layers, c_in, KNN_FUSION_MAX_WIDTH, "layers", 1, KNN_FUSION_MAX_SIDE)
+    _, lay = _mlp_tables([], meta)
+    return _pack("pointwise_mlp_max", c_in, layers, meta, lay, (c_in, lay.ctypes.data, len(meta)))
 
 
 def pointwise_mlp_max(sources, layers):
@@ -891,7 +861,7 @@ def pointwise_mlp_max(sources, layers):
 
     sources: 1 to 4 dense float32 CUDA tensors [B,C,N] (a channel slice of a wider contiguous tensor is read in
     place), at most 512 rows in all.  layers: [(W [C_out,C_in], b [C_out] or None, relu)], every C_out in [1, 512],
-    or a PackedChain from pack_pointwise_mlp_max.  Returns [B,C_out,1] float32.  pointwise_mlp's TF32 rule; the max
+    or a PackedLayers from pack_pointwise_mlp_max.  Returns [B,C_out,1] float32.  pointwise_mlp's TF32 rule; the max
     is float32 with torch.max's NaN rule.  No backward; shape and bound errors raise ValueError before any launch."""
     if not isinstance(sources, (list, tuple)) or not all(isinstance(s, torch.Tensor) for s in sources):
         raise ValueError("sources: need a list of dense [B,C,N] tensors")
@@ -899,28 +869,16 @@ def pointwise_mlp_max(sources, layers):
     c_in = sum(c for c, _, _ in spec)
     if c_in > KNN_FUSION_MAX_WIDTH:
         raise ValueError(f"the concatenated input has {c_in} rows, more than {KNN_FUSION_MAX_WIDTH}")
-    if isinstance(layers, PackedChain):
-        if layers.kind != "pointwise_mlp_max" or layers.c_in != c_in:
-            raise ValueError(f"the layers were packed as {layers.kind} for {layers.c_in} input rows, got {c_in}")
-        packed, meta = layers, layers.meta
-    else:
-        packed, meta = None, _chain_widths(layers, c_in, "layers")
-    dev = sources[0].device
-    for t in sources:
-        if t.requires_grad and torch.is_grad_enabled():
-            raise RuntimeError("pointwise_mlp_max has no backward: call it under torch.no_grad() or detach the inputs")
-        if not t.is_cuda or t.device != dev:
-            raise RuntimeError(f"pointwise_mlp_max: every source must be a CUDA tensor on {dev}")
-        if t.dtype != torch.float32:
-            raise RuntimeError("pointwise_mlp_max: every source must be float32")
+    packed = _prepacked(layers, "pointwise_mlp_max", c_in)
+    meta = packed.meta if packed is not None else _layer_widths(layers, c_in, KNN_FUSION_MAX_WIDTH, "layers", 1,
+                                                                KNN_FUSION_MAX_SIDE)
+    dev = _check_sources("pointwise_mlp_max", sources)
     src, lay = _mlp_tables(spec, meta)
     keep = []
     for i, s in enumerate(sources):
-        C = s.shape[1]
-        if (N > 1 and s.stride(2) != 1) or (C > 1 and s.stride(1) != N) or (B > 1 and s.stride(0) < C * N):
-            s = s.contiguous()
+        s, src[i, 1] = _dense_source(s, B, N)
         keep.append(s)
-        src[i, 0], src[i, 1] = s.data_ptr(), s.stride(0) if B > 1 else C * N
+        src[i, 0] = s.data_ptr()
     if packed is None:
         packed = pack_pointwise_mlp_max(c_in, layers)
     if packed.packed.device != dev:
@@ -943,6 +901,7 @@ def pointwise_mlp_max(sources, layers):
 NODE_MLP_MAX_WIDTH = 1024         # dense input rows and every layer
 NODE_MLP_MAX_DENSE = 4
 NODE_MLP_MAX_PER_SAMPLE = 65536   # per-sample input rows
+_NODE_SLOTS = (2, 7)              # node_mlp's source rows: CHANNELS, BCAST
 _node_mlp_ws = {}
 
 
@@ -983,78 +942,17 @@ def _check_node_mlp_rows(spec):
         raise ValueError(f"the per-sample sources have more than {NODE_MLP_MAX_PER_SAMPLE} rows")
 
 
-def _node_mlp_widths(layers, c_in):
-    """[(C_out, relu)] of 1 to 3 layers (W [C_out,C_in], b [C_out] or None, relu), widths in [1, 1024]."""
-    if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= MLP_MAX_LAYERS:
-        raise ValueError(f"layers: need a list of 1 to {MLP_MAX_LAYERS} layers")
-    meta = []
-    for i, layer in enumerate(layers):
-        if not isinstance(layer, (list, tuple)) or len(layer) != 3:
-            raise ValueError(f"layers[{i}]: need (W, b, relu)")
-        W, b, relu = layer
-        if not isinstance(W, torch.Tensor) or W.dim() != 2 or W.shape[1] != c_in:
-            raise ValueError(f"layers[{i}]: W must be [C_out, {c_in}]")
-        if not 1 <= W.shape[0] <= NODE_MLP_MAX_WIDTH:
-            raise ValueError(f"layers[{i}]: need 1 <= C_out <= {NODE_MLP_MAX_WIDTH}, got {W.shape[0]}")
-        if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (W.shape[0],)):
-            raise ValueError(f"layers[{i}]: b must be [{W.shape[0]}] or None")
-        c_in = W.shape[0]
-        meta.append((c_in, bool(relu)))
-    return meta
-
-
-def _node_mlp_tables(spec, meta):
-    import numpy as np
-    src = np.zeros((len(spec), _MLP_SRC), dtype=np.int64)
-    for i, (C, bcast) in enumerate(spec):
-        src[i, 2], src[i, 7] = C, int(bcast)
-    _, lay = _mlp_tables([], meta)
-    return src, lay
-
-
-class PackedNodeMLP:
-    """The layers of one node_mlp chain in the kernel's order on the device (weights rounded to TF32 once, the per-
-    sample sources' columns of W1 split off and transposed), for sources of the widths and kinds `spec` = [(C,
-    per_sample)].  pack_node_mlp builds it."""
-
-    def __init__(self, spec, meta, packed):
-        self.spec, self.meta, self.packed = list(spec), list(meta), packed
-
-
 def pack_node_mlp(spec, layers):
     """Pack `layers` = [(W [C_out,C_in] float32 CUDA, b [C_out] or None, relu)] (network.fold_pointnet's list) for
-    sources of the widths and kinds `spec` = [(C, per_sample)] in input-row order; node_mlp does this itself when given
-    the raw layers."""
+    sources of the widths and kinds `spec` = [(C, per_sample)] in input-row order into a PackedLayers (the per-sample
+    sources' columns of W1 split off and transposed); node_mlp does this itself when given the raw layers."""
     spec = [(int(c), bool(bc)) for c, bc in spec]
     if not spec or any(c < 1 for c, _ in spec):
         raise ValueError("spec: need a non-empty list of (C >= 1, per_sample)")
     _check_node_mlp_rows(spec)
-    meta = _node_mlp_widths(layers, sum(c for c, _ in spec))
-    dev = layers[0][0].device
-    keep = []
-    for W, b, _ in layers:
-        for t in (W, b):
-            if t is None:
-                continue
-            if t.requires_grad and torch.is_grad_enabled():
-                raise RuntimeError("node_mlp has no backward: call it under torch.no_grad() or detach the layers")
-            if not t.is_cuda or t.device != dev or t.dtype != torch.float32:
-                raise RuntimeError("the layers must be float32 CUDA tensors on one device")
-        keep.append((W.detach().contiguous(), None if b is None else b.detach().contiguous()))
-    src, lay = _node_mlp_tables(spec, meta)
-    for i, (W, b) in enumerate(keep):
-        lay[i, 0], lay[i, 1] = W.data_ptr(), 0 if b is None else b.data_ptr()
-    lib = _native.load()
-    need = lib.node_mlp_packed_bytes(src.ctypes.data, len(spec), lay.ctypes.data, len(meta))
-    if need == 0:
-        raise ValueError("node_mlp: " + lib.dib_last_error().decode("utf-8", "replace"))
-    with torch.cuda.device(dev):
-        packed = torch.empty(need // 4, dtype=torch.float32, device=dev)
-        rc = lib.node_mlp_pack_f32(src.ctypes.data, len(spec), lay.ctypes.data, len(meta), packed.data_ptr(), need,
-                                   _stream_ptr())
-    _native.check(rc, "node_mlp_pack_f32")
-    del keep
-    return PackedNodeMLP(spec, meta, packed)
+    meta = _layer_widths(layers, sum(c for c, _ in spec), NODE_MLP_MAX_WIDTH, "layers", 1, MLP_MAX_LAYERS)
+    src, lay = _mlp_tables(spec, meta, _NODE_SLOTS)
+    return _pack("node_mlp", spec, layers, meta, lay, (src.ctypes.data, len(spec), lay.ctypes.data, len(meta)))
 
 
 def node_mlp(sources, layers, M=None):
@@ -1065,7 +963,8 @@ def node_mlp(sources, layers, M=None):
     sources: in the order of layer 1's input rows, float32 CUDA tensors that are either dense [B,C,M] (at most 4 with
     at most 1024 rows in all; a channel slice of a wider contiguous tensor is read in place) or per sample [B,C] (any
     number, at most 65536 rows in all; a [B,C,1] tensor is passed as t[:, :, 0], with no copy).  M is needed only when every source is per sample.
-    layers: [(W [C_out,C_in], b [C_out] or None, relu)] with every C_out in [1, 1024], or a PackedNodeMLP.  Returns
+    layers: [(W [C_out,C_in], b [C_out] or None, relu)] with every C_out in [1, 1024], or a PackedLayers from
+    pack_node_mlp.  Returns
     the last layer [B,C_out,M] float32.
 
     The dense rows' products run on the tensor cores in TF32 with float32 accumulation whatever torch's TF32 flags
@@ -1075,31 +974,16 @@ def node_mlp(sources, layers, M=None):
     backward: an input that requires grad raises RuntimeError unless grad mode is off.  Shape and bound errors raise
     ValueError before anything is launched."""
     spec, B, M = _node_mlp_source_shapes(sources, M)
-    if isinstance(layers, PackedNodeMLP):
-        if layers.spec != spec:
-            raise ValueError(f"the layers were packed for sources {layers.spec}, got {spec}")
-        packed, meta = layers, layers.meta
-    else:
-        packed, meta = None, _node_mlp_widths(layers, sum(c for c, _ in spec))
-    dev = sources[0].device
-    for t in sources:
-        if t.requires_grad and torch.is_grad_enabled():
-            raise RuntimeError("node_mlp has no backward: call it under torch.no_grad() or detach the inputs")
-        if not t.is_cuda or t.device != dev:
-            raise RuntimeError(f"node_mlp: every source must be a CUDA tensor on {dev}")
-        if t.dtype != torch.float32:
-            raise RuntimeError("node_mlp: every source must be float32")
-    src, lay = _node_mlp_tables(spec, meta)
+    packed = _prepacked(layers, "node_mlp", spec)
+    meta = packed.meta if packed is not None else _layer_widths(layers, sum(c for c, _ in spec), NODE_MLP_MAX_WIDTH,
+                                                                "layers", 1, MLP_MAX_LAYERS)
+    dev = _check_sources("node_mlp", sources)
+    src, lay = _mlp_tables(spec, meta, _NODE_SLOTS)
     keep = []
     for i, s in enumerate(sources):
-        C = s.shape[1]
-        if s.dim() == 3:
-            if (M > 1 and s.stride(2) != 1) or (C > 1 and s.stride(1) != M) or (B > 1 and s.stride(0) < C * M):
-                s = s.contiguous()
-        elif (C > 1 and s.stride(1) != 1) or (B > 1 and s.stride(0) < C):
-            s = s.contiguous()
+        s, src[i, 1] = _dense_source(s, B, M if s.dim() == 3 else 1)   # a per-sample source [B,C] is one column
         keep.append(s)
-        src[i, 0], src[i, 1] = s.data_ptr(), s.stride(0) if B > 1 else C * (M if s.dim() == 3 else 1)
+        src[i, 0] = s.data_ptr()
     if packed is None:
         packed = pack_node_mlp(spec, layers)
     if packed.packed.device != dev:
