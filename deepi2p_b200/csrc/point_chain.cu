@@ -33,7 +33,8 @@ constexpr int kPcTile = 64;
 constexpr int kPcStride = 72;
 constexpr int kPcThreads = 256;
 constexpr int kPcChunk = 64;
-constexpr int kPcMaxWidth = 256;
+constexpr int kPcMaxWidth = 256;      // output rows per CTA: a wider layer runs as row blocks (grid z)
+constexpr int kPcMaxRows = 1024;      // rows of a wide layer (point_chain_gemm_group_f32, point_chain_bn_f32)
 constexpr int kPcMaxSources = 4;
 constexpr int kDwTile = 64;
 constexpr int kDwPts = 32;
@@ -41,7 +42,7 @@ constexpr int kDwStride = 36;   // % 32 == 4: the fragment loads of both operand
 constexpr int kDwThreads = 128;
 constexpr int kDwTargetCtas = 1056;
 
-enum { kOpPlain = 0, kOpAct = 1, kOpBnGrad = 2 };
+enum { kOpPlain = 0, kOpAct = 1, kOpBnGrad = 2, kOpMaxGrad = DIB_PC_MODE_MAX_GRAD };
 enum { kEpWrite = 0, kEpStats = 1, kEpActGrad = 2 };
 
 // BN + ReLU + dropout of one layer, recomputed from its pre-norm Y: z = scale y + shift, a = relu(z), kept a / (1 - p)
@@ -55,12 +56,13 @@ struct ChainOperand {
   int n_src, K, mode;
   ChainAct act;                                   // kOpAct
   const float* y; const float* k1; const float* k2; const float* k3;   // kOpBnGrad: rows of Y [B][K][N]
+  const int* idx; int group;                      // kOpMaxGrad: p[0] and idx are [B][K][N / group]
 };
 
 struct ChainGemm {
   ChainOperand x;
   const float* W; const float* bias; const float* add;   // W packed [Cpad][pad8(K)] or NULL (elementwise, C == K)
-  int C, Cpad, N, ntiles, epilogue;
+  int C, Cpad, N, ntiles, epilogue, add_group;           // add [B][C][N / add_group]
   float* out; double* part;
   ChainAct eg; const float* ey;                           // kEpActGrad: the layer whose output's gradient v is
 };
@@ -81,6 +83,11 @@ __device__ __forceinline__ float chain_act(const ChainAct& a, float y, int b, in
 
 // Row `row` of the operand at point n of sample b (row < K, n < N).
 __device__ __forceinline__ float chain_load(const ChainOperand& x, int b, int row, int n, int N) {
+  if (x.mode == kOpMaxGrad) {                     // the group max's gradient, at the index the forward kept
+    const int j = n / x.group;
+    const size_t e = (size_t)b * x.bstride[0] + (size_t)row * (N / x.group) + j;
+    return x.idx[e] == n - j * x.group ? x.p[0][e] : 0.f;
+  }
   int s = 0;
 #pragma unroll
   for (int q = 1; q < kPcMaxSources; ++q)
@@ -98,12 +105,14 @@ __device__ __forceinline__ float chain_load(const ChainOperand& x, int b, int ro
 __global__ void __launch_bounds__(kPcThreads) chain_gemm_kernel(const __grid_constant__ ChainGemm p) {
   extern __shared__ __align__(16) float pc_smem[];
   float* xs = pc_smem;                               // [kPcChunk][kPcStride]
-  float* ta = xs + kPcChunk * kPcStride;             // [Cpad][kPcStride]: the values (dZ for kEpActGrad)
-  float* tb = ta + p.Cpad * kPcStride;               // kEpActGrad: dZ x^
+  float* ta = xs + kPcChunk * kPcStride;             // [block rows][kPcStride]: the values (dZ for kEpActGrad)
+  float* tb = ta + min(p.Cpad, kPcMaxWidth) * kPcStride;   // kEpActGrad: dZ x^
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3, wm = warp >> 1, n_base = (warp & 1) * 32;
   const int b = blockIdx.y, n0 = blockIdx.x * kPcTile, N = p.N;
-  const int MT = p.Cpad >> 4;
+  // row block blockIdx.z: output rows c0 .. c0 + Cb of the layer's C
+  const int c0 = blockIdx.z * kPcMaxWidth, Cb = min(kPcMaxWidth, p.C - c0);
+  const int MT = min(kPcMaxWidth, p.Cpad - c0) >> 4;
 
   if (p.W != nullptr) {
     float acc[4][4][4];
@@ -114,7 +123,7 @@ __global__ void __launch_bounds__(kPcThreads) chain_gemm_kernel(const __grid_con
 #pragma unroll
         for (int i = 0; i < 4; ++i) acc[mt][nt][i] = 0.f;
     const int K = p.x.K, KT = (K + 7) >> 3;
-    const float4* Wp = reinterpret_cast<const float4*>(p.W);
+    const float4* Wp = reinterpret_cast<const float4*>(p.W) + (size_t)(c0 >> 4) * KT * 32;
     for (int k0 = 0; k0 < K; k0 += kPcChunk) {
       const int kc8 = (min(kPcChunk, K - k0) + 7) & ~7;
       __syncthreads();
@@ -141,21 +150,22 @@ __global__ void __launch_bounds__(kPcThreads) chain_gemm_kernel(const __grid_con
   __syncthreads();
 
   // epilogue, one (channel, point) per thread step: bias, the additive term, the backward's masks; invalid -> 0
-  for (int i = tid; i < p.C * kPcTile; i += kPcThreads) {
-    const int c = i >> 6, n = i & 63, gn = n0 + n;
+  for (int i = tid; i < Cb * kPcTile; i += kPcThreads) {
+    const int c = i >> 6, n = i & 63, gn = n0 + n, gc = c0 + c;
     float v = 0.f, w = 0.f;
     if (gn < N) {
-      const size_t e = ((size_t)b * p.C + c) * N + gn;
-      v = p.W != nullptr ? ta[c * kPcStride + n] : chain_load(p.x, b, c, gn, N);
-      if (p.bias != nullptr) v += p.bias[c];
-      if (p.add != nullptr) v += p.add[e];
+      const size_t e = ((size_t)b * p.C + gc) * N + gn;
+      v = p.W != nullptr ? ta[c * kPcStride + n] : chain_load(p.x, b, gc, gn, N);
+      if (p.bias != nullptr) v += p.bias[gc];
+      if (p.add != nullptr)
+        v += p.add_group == 1 ? p.add[e] : p.add[((size_t)b * p.C + gc) * (N / p.add_group) + gn / p.add_group];
       if (p.epilogue == kEpActGrad) {
         const float y = p.ey[e];
-        const float z = fmaf(p.eg.scale[c], y, p.eg.shift[c]);
+        const float z = fmaf(p.eg.scale[gc], y, p.eg.shift[gc]);
         bool keep = z > 0.f;
-        if (keep && p.eg.drop_state != nullptr) keep = chain_keep(p.eg.drop_state, p.eg.layer, b, c, gn, p.eg.drop_thresh);
+        if (keep && p.eg.drop_state != nullptr) keep = chain_keep(p.eg.drop_state, p.eg.layer, b, gc, gn, p.eg.drop_thresh);
         v = keep ? (p.eg.drop_state != nullptr ? v * p.eg.drop_scale : v) : 0.f;
-        w = v * ((y - p.eg.mean[c]) * p.eg.invstd[c]);
+        w = v * ((y - p.eg.mean[gc]) * p.eg.invstd[gc]);
       }
       p.out[e] = v;
     }
@@ -166,16 +176,48 @@ __global__ void __launch_bounds__(kPcThreads) chain_gemm_kernel(const __grid_con
   __syncthreads();
   // fixed order per channel: points 0..63 of the tile, in fp64
   double* part = p.part + (size_t)(b * p.ntiles + blockIdx.x) * 2 * p.C;
-  for (int c = tid; c < p.C; c += kPcThreads) {
+  for (int c = tid; c < Cb; c += kPcThreads) {
     double s = 0.0, q = 0.0;
     for (int n = 0; n < kPcTile; ++n) {
       const double v = ta[c * kPcStride + n];
       s += v;
       q += p.epilogue == kEpStats ? v * v : (double)tb[c * kPcStride + n];
     }
-    part[c] = s;
-    part[p.C + c] = q;
+    part[c0 + c] = s;
+    part[p.C + c0 + c] = q;
   }
+}
+
+// One thread per (b, c, group of G columns): the operand's values over the group in column order (written to act when
+// act is not NULL) and their max by torch.max's rule: the first maximal value, a NaN (the first) over any number.
+__global__ void chain_group_max_kernel(const __grid_constant__ ChainOperand x, int B, int N, int G, float* act,
+                                       float* __restrict__ mx, int* __restrict__ idx) {
+  const int NG = N / G, C = x.K;
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)B * C * NG) return;
+  const int j = (int)(e % NG), c = (int)((e / NG) % C), b = (int)(e / ((long long)NG * C));
+  float best = 0.f;
+  int bi = 0;
+  for (int k = 0; k < G; ++k) {
+    const int n = j * G + k;
+    const float v = chain_load(x, b, c, n, N);
+    if (act != nullptr) act[((size_t)b * C + c) * N + n] = v;
+    if (k == 0 || v > best || (v != v && best == best)) { best = v; bi = k; }
+  }
+  mx[e] = best;
+  idx[e] = bi;
+}
+
+// out [B][C][N / G] = the operand's sum over each group of G columns, in column order in fp64, rounded once.
+__global__ void chain_group_sum_kernel(const __grid_constant__ ChainOperand x, int B, int N, int G,
+                                       float* __restrict__ out) {
+  const int NG = N / G, C = x.K;
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)B * C * NG) return;
+  const int j = (int)(e % NG), c = (int)((e / NG) % C), b = (int)(e / ((long long)NG * C));
+  double s = 0.0;
+  for (int k = 0; k < G; ++k) s += chain_load(x, b, c, j * G + k, N);
+  out[e] = (float)s;
 }
 
 // Forward (grad == 0): stats [4][C] = mean, invstd, scale, shift; running statistics; num_batches_tracked.
@@ -340,18 +382,27 @@ static int read_operand(const int64_t* d, int n_src, int N, ChainOperand* x) {
   DIB_REQUIRE(d != nullptr && n_src >= 1 && n_src <= kPcMaxSources, "point_chain: need 1 to 4 operand sources");
   *x = ChainOperand{};
   x->n_src = n_src;
+  const int64_t* h = d + (size_t)n_src * DIB_PC_SRC;                    // the transform row after the sources
+  x->mode = (int)h[DIB_PC_OP_MODE];
+  DIB_REQUIRE(x->mode >= kOpPlain && x->mode <= kOpMaxGrad, "point_chain: unknown operand transform");
+  int cols = N;                                                         // a source row's columns
+  if (x->mode == kOpMaxGrad) {
+    x->group = (int)h[DIB_PC_OP_LAYER];
+    x->idx = (const int*)(uintptr_t)h[DIB_PC_OP_Y];
+    DIB_REQUIRE(x->group >= 1 && N % x->group == 0 && x->idx != nullptr,
+                "point_chain: max_grad needs a group that divides N and the max's indices");
+    cols = N / x->group;
+  }
   for (int s = 0; s < n_src; ++s) {
     const int64_t* r = d + (size_t)s * DIB_PC_SRC;
     x->p[s] = (const float*)(uintptr_t)r[DIB_PC_SRC_DATA];
     x->bstride[s] = r[DIB_PC_SRC_BSTRIDE];
     x->row0[s] = x->K;
-    DIB_REQUIRE(x->p[s] != nullptr && r[DIB_PC_SRC_CHANNELS] >= 1 && r[DIB_PC_SRC_BSTRIDE] >= r[DIB_PC_SRC_CHANNELS] * N,
+    DIB_REQUIRE(x->p[s] != nullptr && r[DIB_PC_SRC_CHANNELS] >= 1 &&
+                r[DIB_PC_SRC_BSTRIDE] >= r[DIB_PC_SRC_CHANNELS] * cols,
                 "point_chain: a source is NULL, has no channel or a batch stride below channels x N");
     x->K += (int)r[DIB_PC_SRC_CHANNELS];
   }
-  const int64_t* h = d + (size_t)n_src * DIB_PC_SRC;                    // the transform row after the sources
-  x->mode = (int)h[DIB_PC_OP_MODE];
-  DIB_REQUIRE(x->mode >= kOpPlain && x->mode <= kOpBnGrad, "point_chain: unknown operand transform");
   DIB_REQUIRE(x->mode == kOpPlain || n_src == 1, "point_chain: a transformed operand has one source");
   if (x->mode == kOpAct) {
     const int64_t a[DIB_PC_ACT] = {h[DIB_PC_OP_STATS], x->K, h[DIB_PC_OP_DROP_STATE], h[DIB_PC_OP_DROP_PPM],
@@ -376,13 +427,11 @@ size_t point_chain_partial_bytes(int B, int N, int C) {
   return (size_t)B * ((N + dib::kPcTile - 1) / dib::kPcTile) * 2 * C * sizeof(double);
 }
 
-int point_chain_gemm_f32(const int64_t* operand, int n_src, const void* packed, const float* bias, const float* add,
-                         int C, int B, int N, int epilogue, const int64_t* act, const float* act_y, float* out,
-                         void* partials, size_t partial_bytes, dib_stream_t stream_) {
+static int chain_gemm(const int64_t* operand, int n_src, const void* packed, const float* bias, const float* add,
+                      int add_group, int C, int B, int N, int epilogue, const int64_t* act, const float* act_y,
+                      float* out, void* partials, size_t partial_bytes, cudaStream_t stream) {
   using namespace dib;
-  cudaStream_t stream = (cudaStream_t)stream_;
   DIB_REQUIRE(B >= 1 && B <= 65535 && N >= 1, "point_chain: need 1 <= B <= 65535 and N >= 1");
-  DIB_REQUIRE(C >= 1 && C <= kPcMaxWidth, "point_chain: need 1 <= C_out <= 256");
   DIB_REQUIRE(epilogue >= kEpWrite && epilogue <= kEpActGrad, "point_chain: unknown epilogue");
   DIB_REQUIRE(out != nullptr, "point_chain: out is NULL");
   ChainGemm p = {};
@@ -391,7 +440,8 @@ int point_chain_gemm_f32(const int64_t* operand, int n_src, const void* packed, 
   DIB_REQUIRE(p.x.K <= 1024, "point_chain: the operand has more than 1024 rows");
   DIB_REQUIRE(packed != nullptr || p.x.K == C, "point_chain: an elementwise call needs C == the operand's rows");
   DIB_REQUIRE(packed == nullptr || ((uintptr_t)packed & 15) == 0, "point_chain: packed is not 16-byte aligned");
-  p.W = (const float*)packed; p.bias = bias; p.add = add;
+  DIB_REQUIRE(add_group >= 1 && N % add_group == 0, "point_chain: add_group must divide N");
+  p.W = (const float*)packed; p.bias = bias; p.add = add; p.add_group = add_group;
   p.C = C; p.Cpad = (C + 15) / 16 * 16; p.N = N; p.ntiles = (N + kPcTile - 1) / kPcTile; p.epilogue = epilogue;
   p.out = out;
   if (epilogue != kEpWrite) {
@@ -407,10 +457,57 @@ int point_chain_gemm_f32(const int64_t* operand, int n_src, const void* packed, 
     if (rc != DIB_OK) return rc;
     p.ey = act_y;
   }
-  const size_t smem = ((size_t)kPcChunk * kPcStride + (size_t)(epilogue == kEpActGrad ? 2 : 1) * p.Cpad * kPcStride) *
+  const size_t rows = (size_t)(p.Cpad < kPcMaxWidth ? p.Cpad : kPcMaxWidth);
+  const size_t smem = ((size_t)kPcChunk * kPcStride + (size_t)(epilogue == kEpActGrad ? 2 : 1) * rows * kPcStride) *
                       sizeof(float);
   DIB_CHECK_CUDA(cudaFuncSetAttribute(chain_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  chain_gemm_kernel<<<dim3(p.ntiles, B), kPcThreads, smem, stream>>>(p);
+  chain_gemm_kernel<<<dim3(p.ntiles, B, (C + kPcMaxWidth - 1) / kPcMaxWidth), kPcThreads, smem, stream>>>(p);
+  DIB_CHECK_CUDA(cudaGetLastError());
+  return DIB_OK;
+}
+
+int point_chain_gemm_f32(const int64_t* operand, int n_src, const void* packed, const float* bias, const float* add,
+                         int C, int B, int N, int epilogue, const int64_t* act, const float* act_y, float* out,
+                         void* partials, size_t partial_bytes, dib_stream_t stream) {
+  DIB_REQUIRE(C >= 1 && C <= dib::kPcMaxWidth, "point_chain: need 1 <= C_out <= 256");
+  return chain_gemm(operand, n_src, packed, bias, add, 1, C, B, N, epilogue, act, act_y, out, partials, partial_bytes,
+                    (cudaStream_t)stream);
+}
+
+int point_chain_gemm_group_f32(const int64_t* operand, int n_src, const void* packed, const float* bias,
+                               const float* add, int add_group, int C, int B, int N, int epilogue, const int64_t* act,
+                               const float* act_y, float* out, void* partials, size_t partial_bytes,
+                               dib_stream_t stream) {
+  DIB_REQUIRE(C >= 1 && C <= dib::kPcMaxRows, "point_chain: need 1 <= C_out <= 1024");
+  return chain_gemm(operand, n_src, packed, bias, add, add_group, C, B, N, epilogue, act, act_y, out, partials,
+                    partial_bytes, (cudaStream_t)stream);
+}
+
+int point_chain_group_max_f32(const int64_t* operand, int B, int N, int group, float* act, float* max, int* idx,
+                              dib_stream_t stream) {
+  using namespace dib;
+  DIB_REQUIRE(B >= 1 && B <= 65535 && N >= 1 && group >= 1 && N % group == 0 && max != nullptr && idx != nullptr,
+              "point_chain_group_max: need 1 <= B <= 65535, a group that divides N >= 1, and max and idx");
+  ChainOperand x;
+  const int rc = read_operand(operand, 1, N, &x);
+  if (rc != DIB_OK) return rc;
+  DIB_REQUIRE(x.mode != kOpMaxGrad, "point_chain_group_max: the operand is a max's gradient");
+  const long long total = (long long)B * x.K * (N / group);
+  chain_group_max_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, B, N, group, act, max,
+                                                                                           idx);
+  DIB_CHECK_CUDA(cudaGetLastError());
+  return DIB_OK;
+}
+
+int point_chain_group_sum_f32(const int64_t* operand, int B, int N, int group, float* out, dib_stream_t stream) {
+  using namespace dib;
+  DIB_REQUIRE(B >= 1 && B <= 65535 && N >= 1 && group >= 1 && N % group == 0 && out != nullptr,
+              "point_chain_group_sum: need 1 <= B <= 65535, a group that divides N >= 1, and out");
+  ChainOperand x;
+  const int rc = read_operand(operand, 1, N, &x);
+  if (rc != DIB_OK) return rc;
+  const long long total = (long long)B * x.K * (N / group);
+  chain_group_sum_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, B, N, group, out);
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
 }
@@ -419,7 +516,7 @@ int point_chain_bn_f32(const void* partials, int B, int N, int C, int grad, cons
                        float eps, float momentum, float* stats, float* running_mean, float* running_var,
                        int64_t* num_batches_tracked, float* dgamma, float* dbeta, float* coef, dib_stream_t stream_) {
   using namespace dib;
-  DIB_REQUIRE(B >= 1 && N >= 1 && C >= 1 && C <= kPcMaxWidth, "point_chain_bn: need B, N >= 1 and 1 <= C <= 256");
+  DIB_REQUIRE(B >= 1 && N >= 1 && C >= 1 && C <= kPcMaxRows, "point_chain_bn: need B, N >= 1 and 1 <= C <= 1024");
   DIB_REQUIRE(partials && gamma && beta && stats, "point_chain_bn: a pointer is NULL");
   if (grad) DIB_REQUIRE(dgamma && dbeta && coef, "point_chain_bn: a gradient output is NULL");
   else DIB_REQUIRE(running_mean && running_var, "point_chain_bn: the running statistics are NULL");

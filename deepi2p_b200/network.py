@@ -32,8 +32,10 @@ SHAPES = {"kitti": dict(img_H=160, img_W=512), "oxford": dict(img_H=384, img_W=6
           "nuscenes": dict(img_H=160, img_W=320)}
 
 # KeypointDetector(point_layers=...): "torch" runs the per-point chains as the model's own layers; "fused" runs them
-# through point_ops.point_chain (DESIGN.md 4.34)
-POINT_LAYERS = ("torch", "fused")
+# through point_ops.point_chain (DESIGN.md 4.34); "fused_all" also runs the kNN module, final_pointnet + global max and
+# the four node-level PointNets through point_ops.point_branch in training, and the kernels of
+# FusedInference(encoder="fused", decoder="fused") in eval mode (DESIGN.md 4.36)
+POINT_LAYERS = ("torch", "fused", "fused_all")
 
 # forward chunk of classify_and_register: at the Oxford shape (20480 points, 384 x 640) one chunk of 64 samples peaks
 # at 13.5 GB above the inputs on an H100 (BENCH_E2E.json, DESIGN.md 4.18)
@@ -265,7 +267,61 @@ class KeypointDetector(nn.Module):
         return point_ops.point_chain([first_pn_out, second_pn_out], head, True, self.point_chain_state, add=pa + pb,
                                      in_col=Ca + Cb)
 
+    def _fused_knn(self, node_b, cluster_mean, node_a_features):
+        """The kNN module with point_layers="fused_all" in train mode: the before-chain gives its activations and their
+        max over K; the after-chain's max columns are W_p . max, projected once per node and added per group of K;
+        the after-chain gives only its max over K.  No [B,2C,M,K] concatenation and no after-chain activation is
+        built."""
+        knn, K = self.pc_encoder.knnlayer, self.k_ab
+        _, x = point_ops.knn_group(node_b, cluster_mean, node_a_features, K)          # [B,3+C,M,K]
+        B, C0, M = x.shape[0], x.shape[1], x.shape[2]
+        act, mx = point_ops.point_branch([x.reshape(B, C0, M * K)], list(knn.layers_before), self.point_chain_state,
+                                         max_group=K, output="both")
+        Cb = mx.shape[1]
+        proj = point_ops.channel_product(knn.layers_after[0].conv.weight[:, :Cb, 0, 0], mx)
+        return point_ops.point_branch([act], list(knn.layers_after), self.point_chain_state, cols=[Cb], add=proj,
+                                      add_group=K, max_group=K, output="max")
+
+    def _fused_node(self, pn, dense, cols, per_sample, M):
+        """A node-level PointNet with point_layers="fused_all" in train mode: the dense [B,C,M] inputs read in place at
+        their first columns `cols`, each per-sample input (column, [B,C]) projected once per sample by its weight
+        columns and added to layer 1 over all M nodes.  No expanded input and no concatenation is built."""
+        W1 = pn.layers[0].conv.weight[:, :, 0]
+        add = None
+        for c, v in per_sample:
+            t = point_ops.channel_product(W1[:, c:c + v.shape[1]], v.unsqueeze(2))
+            add = t if add is None else add + t
+        return point_ops.point_branch(dense, list(pn.layers), self.point_chain_state, cols=cols, add=add,
+                                      add_group=M if add is not None else 1)
+
+    def __getstate__(self):
+        state = super().__getstate__() if hasattr(super(), "__getstate__") else self.__dict__
+        state = dict(state)
+        state.pop("_fused_all_cache", None)          # device buffers derived from the parameters, rebuilt on use
+        return state
+
+    def _fused_all_eval(self, pc, intensity, sn, node_a, node_b, img):
+        """point_layers="fused_all" in eval mode: the scores of FusedInference(self, encoder="fused",
+        decoder="fused"), whose folded and packed layers are cached and rebuilt when a parameter or buffer changes.
+        As FusedInference, it takes node_a_num / node_b_num nodes only (the fused decoder's layers are packed for
+        them) and raises ValueError for other counts, which train mode and the other modes accept."""
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise RuntimeError("KeypointDetector(point_layers='fused_all') in eval mode has no backward: call it under "
+                               "torch.no_grad(), or freeze the parameters")
+        # the folded layers are kept on the model as plain dicts (no reference back to it, so no cycle) and left out
+        # of pickling (__getstate__); FusedInference is rebuilt per call around them
+        cache = self.__dict__.setdefault("_fused_all_cache", ({}, {}))
+        fi = FusedInference(self, encoder="fused", decoder="fused")
+        fi._packed, fi._stamp = cache
+        with torch.no_grad():
+            scores = fi._classify(pc, intensity, sn, node_a, node_b, img, True)[-1]
+        if self.fine:
+            return scores[:, 0:2, :], scores[:, 2:, :]
+        return scores[:, 0:2, :]
+
     def forward(self, pc, intensity, sn, node_a, node_b, img):
+        if self.point_layers == "fused_all" and not self.training:
+            return self._fused_all_eval(pc, intensity, sn, node_a, node_b, img)
         B, Ma, Mb = pc.shape[0], node_a.shape[2], node_b.shape[2]
         # the coordinates get no gradient in the reference (every use is detached); the ops require that
         pc, node_a, node_b = (t.detach().contiguous() for t in (pc, node_a, node_b))
@@ -274,7 +330,8 @@ class KeypointDetector(nn.Module):
         # point encoder (networks_pc.py:58-115)
         ca = point_ops.cluster_assign_forward(pc, node_a, k=self.k_interp_point_a)
         min_idx = ca["min_idx"]
-        fused = self.point_layers == "fused"
+        fused = self.point_layers in ("fused", "fused_all")
+        fused_all = self.point_layers == "fused_all"
         if fused:
             first_pn_out = point_ops.point_chain([ca["pc_decentered"], intensity, sn], list(enc.first_pointnet.layers),
                                                  self.training, self.point_chain_state)
@@ -287,9 +344,14 @@ class KeypointDetector(nn.Module):
         else:
             second_pn_out = enc.second_pointnet(torch.cat((first_pn_out, scattered), dim=1))
         node_a_features = point_ops.cluster_max_pool(second_pn_out, min_idx, Ma)
-        node_b_features = enc.knnlayer(node_b, ca["cluster_mean"], node_a_features, self.k_ab)
-        final_pn_out = enc.final_pointnet(torch.cat((node_b, node_b_features), dim=1))
-        global_feature = torch.max(final_pn_out, dim=2, keepdim=True)[0]            # [B,Cg,1]
+        if fused_all:
+            node_b_features = self._fused_knn(node_b, ca["cluster_mean"], node_a_features)
+            global_feature = point_ops.point_branch([node_b, node_b_features], list(enc.final_pointnet.layers),
+                                                    self.point_chain_state, max_group=Mb, output="max")
+        else:
+            node_b_features = enc.knnlayer(node_b, ca["cluster_mean"], node_a_features, self.k_ab)
+            final_pn_out = enc.final_pointnet(torch.cat((node_b, node_b_features), dim=1))
+            global_feature = torch.max(final_pn_out, dim=2, keepdim=True)[0]            # [B,Cg,1]
 
         # image encoder: the global feature is the mean over H and W (= AdaptiveAvgPool2d((1, 1)))
         s16, s32 = self.img_encoder.backbone(img)
@@ -301,20 +363,36 @@ class KeypointDetector(nn.Module):
         img_global_b = img_global.unsqueeze(2).expand(B, C_img, Mb)
 
         # node_b: attention over the stride-32 map, then the node_b PointNet (networks_united.py:147-155)
-        att_b = self.node_b_attention_pn(torch.cat((node_b_features, img_global_b), dim=1))
+        Cnb, Cg = node_b_features.shape[1], global_feature.shape[1]
+        if fused_all:
+            att_b = self._fused_node(self.node_b_attention_pn, [node_b_features], [0], [(Cnb, img_global)], Mb)
+        else:
+            att_b = self.node_b_attention_pn(torch.cat((node_b_features, img_global_b), dim=1))
         weighted_s32 = point_ops.attention_fusion(s32, att_b)
-        up_node_b_features = self.node_b_pn(torch.cat((node_b_features, global_feature.expand(B, -1, Mb),
-                                                       weighted_s32, img_global_b), dim=1))
+        if fused_all:
+            up_node_b_features = self._fused_node(
+                self.node_b_pn, [node_b_features, weighted_s32], [0, Cnb + Cg],
+                [(Cnb, global_feature[:, :, 0]), (Cnb + Cg + weighted_s32.shape[1], img_global)], Mb)
+        else:
+            up_node_b_features = self.node_b_pn(torch.cat((node_b_features, global_feature.expand(B, -1, Mb),
+                                                           weighted_s32, img_global_b), dim=1))
 
         # decoder (networks_united.py:158-197)
         pb_idx = point_ops.cluster_assign_forward(pc, node_b, k=self.k_interp_point_b, want_centers=False)["min_k_idx"]
         if not fused:
             pb = point_ops.upsample_by_interpolation(pb_idx, pc, node_b, up_node_b_features)
-        att_a = self.node_a_attention_pn(torch.cat((node_a_features, img_global_a), dim=1))
+        if fused_all:
+            att_a = self._fused_node(self.node_a_attention_pn, [node_a_features], [0],
+                                     [(node_a_features.shape[1], img_global)], Ma)
+        else:
+            att_a = self.node_a_attention_pn(torch.cat((node_a_features, img_global_a), dim=1))
         weighted_s16 = point_ops.attention_fusion(s16, att_a)
         ab_idx = point_ops.cluster_assign_forward(node_a, node_b, k=self.k_interp_ab, want_centers=False)["min_k_idx"]
         ab = point_ops.upsample_by_interpolation(ab_idx, node_a, node_b, up_node_b_features)
-        up_node_a_features = self.node_a_pn(torch.cat((node_a_features, ab, weighted_s16), dim=1))
+        if fused_all:
+            up_node_a_features = self._fused_node(self.node_a_pn, [node_a_features, ab, weighted_s16], None, [], Ma)
+        else:
+            up_node_a_features = self.node_a_pn(torch.cat((node_a_features, ab, weighted_s16), dim=1))
         if fused:
             scores = self._fused_head(pc, node_a, node_b, ca["min_k_idx"], pb_idx, up_node_a_features,
                                       up_node_b_features, first_pn_out, second_pn_out)

@@ -1007,7 +1007,8 @@ CHAIN_MAX_WIDTH = 256
 CHAIN_MAX_IN = 1024
 CHAIN_MAX_SOURCES = 4
 _PC_SRC, _PC_OP = 3, 6            # int64 slots per operand source / transform row (DIB_PC_SRC, DIB_PC_OP)
-_OP_PLAIN, _OP_ACT, _OP_BN_GRAD = 0, 1, 2
+_OP_PLAIN, _OP_ACT, _OP_BN_GRAD, _OP_MAX_GRAD = 0, 1, 2, 3     # _OP_MAX_GRAD: DIB_PC_MODE_MAX_GRAD
+BRANCH_MAX_WIDTH = 1024            # point_branch's layer widths (DIB_PC_MAX_WIDTH)
 _EP_WRITE, _EP_STATS, _EP_ACT_GRAD = 0, 1, 2
 _chain_part_ws, _chain_dw_ws = {}, {}
 
@@ -1033,25 +1034,66 @@ def _chain_act_row(stats, drop, layer):
 
 
 def _chain_pack(W, widths):
-    """W [C_out, sum(widths)] packed by pointwise_mlp's packer for dense sources of those widths."""
-    return pack_pointwise_mlp([(c, 0, 0) for c in widths], [(W.detach(), None, False)]).packed
+    """W [C_out, sum(widths)] packed by pointwise_mlp's packer for dense sources of those widths.  A layer wider than
+    CHAIN_MAX_WIDTH is packed in blocks of that many rows whose weight parts are concatenated: the A-fragment layout is
+    row-tile major, so that is the whole layer's layout, the one point_chain_gemm_group_f32's row blocks read."""
+    spec = [(c, 0, 0) for c in widths]
+    if W.shape[0] <= CHAIN_MAX_WIDTH:
+        return pack_pointwise_mlp(spec, [(W.detach(), None, False)]).packed
+    KT = (W.shape[1] + 7) // 8
+    parts = []
+    for r in range(0, W.shape[0], CHAIN_MAX_WIDTH):
+        blk = W[r:r + CHAIN_MAX_WIDTH]
+        rows = (blk.shape[0] + 15) // 16 * 16
+        parts.append(pack_pointwise_mlp(spec, [(blk.detach(), None, False)]).packed[:rows * KT * 8])
+    return torch.cat(parts)
 
 
-def _chain_gemm(op, n_src, packed, bias, add, C, B, N, epilogue, act=None, act_y=None):
+def _chain_gemm(op, n_src, packed, bias, add, C, B, N, epilogue, act=None, act_y=None, add_group=1):
     lib = _native.load()
     dev = act_y.device if act_y is not None else torch.device("cuda", torch.cuda.current_device())
     out = torch.empty((B, C, N), dtype=torch.float32, device=dev)
     part = None
     if epilogue != _EP_WRITE:
         part = _workspace(_chain_part_ws, lib.point_chain_partial_bytes(B, N, C), dev, floor=0)
-    rc = lib.point_chain_gemm_f32(op.ctypes.data, n_src, None if packed is None else packed.data_ptr(),
-                                  None if bias is None else bias.data_ptr(), None if add is None else add.data_ptr(),
-                                  C, B, N, epilogue, None if act is None else act.ctypes.data,
-                                  None if act_y is None else act_y.data_ptr(), out.data_ptr(),
-                                  None if part is None else part.data_ptr(), 0 if part is None else part.numel(),
-                                  _stream_ptr())
-    _native.check(rc, "point_chain_gemm_f32")
+    args = (None if act is None else act.ctypes.data, None if act_y is None else act_y.data_ptr(), out.data_ptr(),
+            None if part is None else part.data_ptr(), 0 if part is None else part.numel(), _stream_ptr())
+    head = (op.ctypes.data, n_src, None if packed is None else packed.data_ptr(),
+            None if bias is None else bias.data_ptr(), None if add is None else add.data_ptr())
+    if C <= CHAIN_MAX_WIDTH and add_group == 1:
+        rc, name = lib.point_chain_gemm_f32(*head, C, B, N, epilogue, *args), "point_chain_gemm_f32"
+    else:
+        rc = lib.point_chain_gemm_group_f32(*head, add_group, C, B, N, epilogue, *args)
+        name = "point_chain_gemm_group_f32"
+    _native.check(rc, name)
     return out, part
+
+
+def _chain_max_grad_operand(g, idx, group):
+    """The operand that reads a group max's gradient g [B,C,N/G] back over the group, at the indices idx."""
+    import numpy as np
+    return np.array((g.data_ptr(), g.shape[1] * g.shape[2], g.shape[1], _OP_MAX_GRAD, 0, idx.data_ptr(), 0, 0, group),
+                    dtype=np.int64)
+
+
+def _chain_group_max(op, B, N, C, group, want_act):
+    lib = _native.load()
+    dev = torch.device("cuda", torch.cuda.current_device())
+    act = torch.empty((B, C, N), dtype=torch.float32, device=dev) if want_act else None
+    mx = torch.empty((B, C, N // group), dtype=torch.float32, device=dev)
+    idx = torch.empty((B, C, N // group), dtype=torch.int32, device=dev)
+    rc = lib.point_chain_group_max_f32(op.ctypes.data, B, N, group, None if act is None else act.data_ptr(),
+                                       mx.data_ptr(), idx.data_ptr(), _stream_ptr())
+    _native.check(rc, "point_chain_group_max_f32")
+    return act, mx, idx
+
+
+def _chain_group_sum(op, B, N, C, group):
+    lib = _native.load()
+    out = torch.empty((B, C, N // group), dtype=torch.float32, device=torch.device("cuda", torch.cuda.current_device()))
+    rc = lib.point_chain_group_sum_f32(op.ctypes.data, B, N, group, out.data_ptr(), _stream_ptr())
+    _native.check(rc, "point_chain_group_sum_f32")
+    return out
 
 
 def _chain_bn(part, B, N, C, norm, stats, grad):
@@ -1093,12 +1135,20 @@ def _chain_product(op, n_src, W, widths, B, N):
     return outs[0] if len(outs) == 1 else torch.cat(outs, dim=1)
 
 
+def _gather_cols(W, cols, widths):
+    """The columns of W [C, C_in] that sources of `widths` starting at layer columns `cols` feed, in source order."""
+    if all(c == cols[0] + sum(widths[:i]) for i, c in enumerate(cols)):
+        return W[:, cols[0]:cols[0] + sum(widths)]
+    return torch.cat([W[:, c:c + w] for c, w in zip(cols, widths)], dim=1)
+
+
 class _PointChain(torch.autograd.Function):
-    """Inputs: (layers, drop_state, n_src, in_col, add, *sources, *per-layer (W, b, gamma, beta)); gamma / beta are None for a
-    layer without BatchNorm.  The BN buffers of `layers` are updated in place."""
+    """Inputs: (layers, drop_state, n_src, cols, add, add_group, max_group, output, *sources, *per-layer (W, b, gamma,
+    beta)); gamma / beta are None for a layer without BatchNorm; cols: layer 1's first column of each source.  The BN
+    buffers of `layers` are updated in place."""
 
     @staticmethod
-    def forward(ctx, layers, drop_state, n_src, in_col, add, *tensors):
+    def forward(ctx, layers, drop_state, n_src, cols, add, add_group, max_group, output, *tensors):
         sources = list(tensors[:n_src])
         B, N = sources[0].shape[0], sources[0].shape[2]
         dev = sources[0].device
@@ -1116,10 +1166,10 @@ class _PointChain(torch.autograd.Function):
                 conv, norm = layer.conv, layer.norm
                 C = conv.out_channels
                 W = conv.weight.detach().reshape(C, -1)
-                packed = _chain_pack(W[:, in_col:in_col + sum(widths)] if l == 0 else W, widths)
+                packed = _chain_pack(_gather_cols(W, cols, widths) if l == 0 else W, widths)
                 bias = None if conv.bias is None else conv.bias.detach()
                 y, part = _chain_gemm(op, len(widths), packed, bias, add if l == 0 else None, C, B, N,
-                                      _EP_STATS if norm is not None else _EP_WRITE)
+                                      _EP_STATS if norm is not None else _EP_WRITE, add_group=add_group)
                 st = None
                 if norm is not None:
                     st = torch.empty((4, C), dtype=torch.float32, device=dev)
@@ -1133,23 +1183,30 @@ class _PointChain(torch.autograd.Function):
                 stats_all.append(st)
                 widths = [C]
             last = layers[-1]
-            if last.norm is not None:
+            idx = None
+            if max_group is not None:            # the group max fused into the last layer's BN + ReLU pass
+                act, mx, idx = _chain_group_max(op, B, N, last.conv.out_channels, max_group, output == "both")
+                out = mx if output == "max" else (act, mx)
+            elif last.norm is not None:
                 out, _ = _chain_gemm(op, 1, None, None, None, last.conv.out_channels, B, N, _EP_WRITE)
             else:
                 out = ys[-1]
         # the sources and the pre-norm outputs go through save_for_backward only: autograd then catches an in-place change
         # to a source before the backward, and the chain's output, which can be one of the outputs, is not held on ctx
         # (that would tie the autograd graph into a reference cycle)
-        ctx.layers, ctx.n_src, ctx.in_col, ctx.has_add = layers, n_src, in_col, add is not None
+        ctx.layers, ctx.n_src, ctx.cols, ctx.has_add = layers, n_src, cols, add is not None
+        ctx.add_group, ctx.max_group, ctx.output = add_group, max_group, output
         ctx.stats, ctx.drop, ctx.shape = stats_all, drop, (B, N)
-        ctx.save_for_backward(*sources, *ys)
+        ctx.save_for_backward(*sources, *ys, *(() if idx is None else (idx,)))
         return out
 
     @staticmethod
-    def backward(ctx, grad_out):
+    def backward(ctx, *grad_outs):
         layers, (B, N), n_src = ctx.layers, ctx.shape, ctx.n_src
         saved = ctx.saved_tensors
-        sources, ys = saved[:n_src], saved[n_src:]
+        sources, ys = saved[:n_src], saved[n_src:n_src + len(layers)]
+        grad_out = grad_outs[-1]                 # the activations', or the group max's
+        g_dense = grad_outs[0].float().contiguous() if ctx.output == "both" else None
         dev = ys[0].device
         L = len(layers)
         grads = [None] * (4 * L)
@@ -1165,7 +1222,10 @@ class _PointChain(torch.autograd.Function):
                 y, st = ys[l], ctx.stats[l]
                 d = None if layer.dropout is None else (ctx.drop, float(layer.dropout.p))
                 if norm is not None:
-                    if l == L - 1:
+                    if l == L - 1 and ctx.max_group is not None:
+                        dz, part = _chain_gemm(_chain_max_grad_operand(G, saved[-1], ctx.max_group), 1, None, None,
+                                               g_dense, C, B, N, _EP_ACT_GRAD, _chain_act_row(st, d, l), y)
+                    elif l == L - 1:
                         dz, part = _chain_gemm(_chain_operand([G]), 1, None, None, None, C, B, N, _EP_ACT_GRAD,
                                                _chain_act_row(st, d, l), y)
                     dgamma, dbeta, coef = _chain_bn(part, B, N, C, norm, st, grad=True)
@@ -1179,15 +1239,23 @@ class _PointChain(torch.autograd.Function):
                     prev = layers[l - 1]
                     dp = None if prev.dropout is None else (ctx.drop, float(prev.dropout.p))
                     x_op, nx = _chain_operand([ys[l - 1]], _OP_ACT, ctx.stats[l - 1], drop=dp, layer=l - 1), 1
-                K = conv.in_channels if l > 0 else sum(s.shape[1] for s in sources)
-                c0 = ctx.in_col if l == 0 else 0
+                widths = [s.shape[1] for s in sources]
+                K = conv.in_channels if l > 0 else sum(widths)
                 dW, db = _chain_dw(dy_op, x_op, nx, B, N, C, K, conv.bias is not None)
-                if K != conv.in_channels:             # the columns the sources feed; the rest get their gradient
-                    full = dW.new_zeros((C, conv.in_channels))     # through `add`
-                    full[:, c0:c0 + K] = dW
+                # dW's columns are in source order: scatter them to the layer's columns unless the sources are its
+                # columns 0 .. C_in in order (the rest, where `add` stands for them, get zero)
+                if l == 0 and (K != conv.in_channels or
+                               list(ctx.cols) != [sum(widths[:i]) for i in range(len(widths))]):
+                    full = dW.new_zeros((C, conv.in_channels))
+                    r = 0
+                    for c0, w in zip(ctx.cols, widths):
+                        full[:, c0:c0 + w] = dW[:, r:r + w]
+                        r += w
                     dW = full
                 grads[4 * l], grads[4 * l + 1] = dW.view_as(conv.weight), db
-                W = conv.weight.detach().reshape(C, conv.in_channels)[:, c0:c0 + K]
+                W = conv.weight.detach().reshape(C, conv.in_channels)
+                if l == 0:
+                    W = _gather_cols(W, ctx.cols, widths)
                 if l > 0:
                     prev = layers[l - 1]
                     dp = None if prev.dropout is None else (ctx.drop, float(prev.dropout.p))
@@ -1195,15 +1263,19 @@ class _PointChain(torch.autograd.Function):
                                            _EP_ACT_GRAD, _chain_act_row(ctx.stats[l - 1], dp, l - 1), ys[l - 1])
                 else:
                     if ctx.has_add and ctx.needs_input_grad[4]:
-                        g_add = G if norm is None else _chain_gemm(dy_op, 1, None, None, None, C, B, N, _EP_WRITE)[0]
-                    if any(ctx.needs_input_grad[5:5 + n_src]):
+                        if ctx.add_group > 1:         # layer 1's dY summed over each group, in column order
+                            g_add = _chain_group_sum(dy_op, B, N, C, ctx.add_group)
+                        else:
+                            g_add = G if norm is None else _chain_gemm(dy_op, 1, None, None, None, C, B, N,
+                                                                       _EP_WRITE)[0]
+                    if any(ctx.needs_input_grad[8:8 + n_src]):
                         gx = _chain_product(dy_op, 1, W.t(), [C], B, N)
                         r = 0
                         for i, s in enumerate(sources):
-                            if ctx.needs_input_grad[5 + i]:
+                            if ctx.needs_input_grad[8 + i]:
                                 g_src[i] = gx[:, r:r + s.shape[1]]
                             r += s.shape[1]
-        return (None, None, None, None, g_add, *g_src, *grads)
+        return (None, None, None, None, g_add, None, None, None, *g_src, *grads)
 
 
 def _check_chain_args(sources, layers, drop_state, add, in_col, training):
@@ -1323,8 +1395,9 @@ def point_chain(sources, layers, training, drop_state=None, add=None, in_col=0):
                     or (B > 1 and s.stride(0) < s.shape[1] * N):
                 s = s.contiguous()
             srcs.append(s)
-        return _PointChain.apply(list(layers), drop_state, len(srcs), in_col, None if add is None else add.contiguous(),
-                                 *srcs, *flat)
+        cols = [in_col + sum(s.shape[1] for s in srcs[:i]) for i in range(len(srcs))]
+        return _PointChain.apply(list(layers), drop_state, len(srcs), cols, None if add is None else add.contiguous(),
+                                 1, None, "activations", *srcs, *flat)
     if add is not None or in_col != 0:
         raise ValueError("add, in_col: the eval-mode chain takes interpolated sources instead of an additive term")
     if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= CHAIN_MAX_LAYERS:
@@ -1338,6 +1411,112 @@ def point_chain(sources, layers, training, drop_state=None, add=None, in_col=0):
     import types
     from .network import fold_pointnet
     return pointwise_mlp(list(sources), fold_pointnet(types.SimpleNamespace(layers=list(layers))))
+
+
+def _check_branch_args(sources, layers, drop_state, cols, add, add_group, max_group, output):
+    if not isinstance(layers, (list, tuple)) or not 1 <= len(layers) <= CHAIN_MAX_LAYERS:
+        raise ValueError(f"layers: need a list of 1 to {CHAIN_MAX_LAYERS} point layers")
+    if not isinstance(sources, (list, tuple)) or not 1 <= len(sources) <= CHAIN_MAX_SOURCES:
+        raise ValueError(f"sources: need a list of 1 to {CHAIN_MAX_SOURCES} sources")
+    for i, layer in enumerate(layers):
+        conv, norm = getattr(layer, "conv", None), getattr(layer, "norm", None)
+        if not isinstance(conv, (torch.nn.Conv1d, torch.nn.Conv2d)) or any(k != 1 for k in conv.kernel_size) \
+                or conv.groups != 1:
+            raise TypeError(f"layers[{i}]: need a point layer with a 1x1 Conv1d or Conv2d `conv`")
+        if not 1 <= conv.out_channels <= BRANCH_MAX_WIDTH:
+            raise ValueError(f"layers[{i}]: need 1 <= C_out <= {BRANCH_MAX_WIDTH}, got {conv.out_channels}")
+        if i > 0 and conv.in_channels != layers[i - 1].conv.out_channels:
+            raise ValueError(f"layers[{i}]: has {conv.in_channels} input channels, layers[{i - 1}] gives "
+                             f"{layers[i - 1].conv.out_channels}")
+        if i < len(layers) - 1 and norm is None:
+            raise ValueError(f"layers[{i}]: only the last layer may go without BatchNorm + ReLU")
+        if norm is not None and (not isinstance(norm, (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d))
+                                 or not norm.affine or not norm.track_running_stats or norm.momentum is None):
+            raise TypeError(f"layers[{i}]: the norm must be an affine BatchNorm1d / 2d with running statistics and "
+                            f"a momentum")
+        if layer.dropout is not None and norm is None:
+            raise ValueError(f"layers[{i}]: dropout needs BatchNorm + ReLU on the same layer")
+    c_in, dev = layers[0].conv.in_channels, layers[0].conv.weight.device
+    B = N = None
+    for i, s in enumerate(sources):
+        if not isinstance(s, torch.Tensor) or s.dtype != torch.float32:
+            raise TypeError(f"sources[{i}] must be a float32 torch.Tensor")
+        if s.dim() != 3 or s.shape[1] < 1 or s.device != dev:
+            raise ValueError(f"sources[{i}] must be [B,C,N] with C >= 1 on {dev}, the layers' device")
+        if B is None:
+            B, N = s.shape[0], s.shape[2]
+        elif (s.shape[0], s.shape[2]) != (B, N):
+            raise ValueError(f"sources[{i}] has B, N = {s.shape[0]}, {s.shape[2]}; sources[0] has {B}, {N}")
+    if not 1 <= B <= MLP_MAX_BATCH or N < 1:
+        raise ValueError(f"sources: need 1 <= B <= {MLP_MAX_BATCH} and N >= 1, got B = {B}, N = {N}")
+    if sum(s.shape[1] for s in sources) > CHAIN_MAX_IN:
+        raise ValueError(f"sources: more than {CHAIN_MAX_IN} rows")
+    if not isinstance(cols, (list, tuple)) or len(cols) != len(sources) or \
+            any(not isinstance(c, int) or isinstance(c, bool) or c < 0 for c in cols):
+        raise ValueError("cols: need one non-negative int per source, its first column of layers[0]")
+    spans = sorted((c, c + s.shape[1]) for c, s in zip(cols, sources))
+    if spans[-1][1] > c_in or any(a[1] > b[0] for a, b in zip(spans, spans[1:])):
+        raise ValueError(f"cols: the sources' column ranges {spans} overlap or exceed layers[0]'s {c_in} columns")
+    if add is None and sum(s.shape[1] for s in sources) != c_in:
+        raise ValueError(f"sources: without `add` they must feed all {c_in} columns of layers[0]")
+    for g, name in ((add_group, "add_group"), (max_group, "max_group")):
+        if g is not None and (not isinstance(g, int) or isinstance(g, bool) or g < 1 or N % g):
+            raise ValueError(f"{name} must be an int >= 1 that divides N = {N}, got {g!r}")
+    if add is not None:
+        if not isinstance(add, torch.Tensor) or add.dtype != torch.float32:
+            raise TypeError("add must be a float32 torch.Tensor or None")
+        C1 = layers[0].conv.out_channels
+        if tuple(add.shape) != (B, C1, N // add_group) or add.device != dev:
+            raise ValueError(f"add must be [{B}, {C1}, {N // add_group}] (N / add_group columns) on {dev}")
+    if output not in ("activations", "max", "both"):
+        raise ValueError(f"output must be 'activations', 'max' or 'both', got {output!r}")
+    if (output != "activations") != (max_group is not None):
+        raise ValueError("max_group: output 'max' and 'both' need it, 'activations' takes none")
+    if max_group is not None and layers[-1].norm is None:
+        raise ValueError("max_group: the group max is taken after the last layer's BatchNorm + ReLU")
+    if any(layer.dropout is not None for layer in layers):
+        if not isinstance(drop_state, torch.Tensor) or drop_state.dtype != torch.int64 \
+                or tuple(drop_state.shape) != (2,) or drop_state.device != dev or not drop_state.is_contiguous():
+            raise ValueError("drop_state must be a contiguous int64 [2] (seed, offset) on the layers' device")
+    for i, layer in enumerate(layers):
+        norm = layer.norm
+        for t in list(layer.parameters()) + ([norm.running_mean, norm.running_var] if norm is not None else []):
+            if not t.is_cuda or t.dtype != torch.float32:
+                raise TypeError(f"layers[{i}]: every parameter and running statistic must be a float32 CUDA tensor")
+    return B, N
+
+
+def point_branch(sources, layers, drop_state=None, cols=None, add=None, add_group=1, max_group=None,
+                 output="activations"):
+    """point_chain in train mode, generalised to the point encoder's kNN module, final_pointnet and the decoder's
+    node-level PointNets (DESIGN.md 4.36): the same kernels, rules and determinism, plus
+
+    - 1x1 Conv2d + BatchNorm2d layers (the kNN module's): a [B,C,M,K] input is passed viewed as [B,C,M*K], and
+      BatchNorm2d's statistics over B*M*K are the chain's over its columns;
+    - layers up to BRANCH_MAX_WIDTH (1024) rows wide, run as row blocks into one pre-norm tensor;
+    - cols: layer 1's first column of each source (default: the sources in order from column 0); the columns no
+      source feeds stand for `add`, and layer 1's weight gradient is zero there;
+    - add [B, C_1, N / add_group]: added to layer 1 at column n from entry n // add_group (a projected per-node max
+      with add_group = K, a projected per-sample input with add_group = N); its gradient is layer 1's dY summed over
+      each group in column order in fp64;
+    - max_group: the max of the last layer's activations over groups of max_group consecutive columns by torch.max's
+      rule (first maximal index; a NaN propagates), [B, C, N / max_group], fused into the BN + ReLU pass; the backward
+      reads the compact gradient at the saved in-group index.  output "max" returns the max only (the activations are
+      never written), "both" returns (activations, max).
+
+    Train mode only; errors name the argument."""
+    if cols is None and isinstance(sources, (list, tuple)):
+        cols = [sum(s.shape[1] for s in sources[:i]) for i in range(len(sources))]
+    B, N = _check_branch_args(sources, layers, drop_state, cols, add, add_group, max_group, output)
+    flat = []
+    for layer in layers:
+        norm = layer.norm
+        flat += [layer.conv.weight, layer.conv.bias, None if norm is None else norm.weight,
+                 None if norm is None else norm.bias]
+    srcs = [s.contiguous() if (N > 1 and s.stride(2) != 1) or (s.shape[1] > 1 and s.stride(1) != N)
+            or (B > 1 and s.stride(0) < s.shape[1] * N) else s for s in sources]
+    return _PointChain.apply(list(layers), drop_state, len(srcs), list(cols),
+                             None if add is None else add.contiguous(), add_group, max_group, output, *srcs, *flat)
 
 
 class _ChannelProduct(torch.autograd.Function):

@@ -217,7 +217,7 @@ class Trainer:
         self.graph, self._eager_steps = None, 0
         self.sums = torch.zeros(5, dtype=torch.float64, device=self.device)
         self._consumed = torch.cuda.Event()
-        if model.point_layers == "fused":              # point_chain's dropout stream starts from the run's seed
+        if model.point_layers in ("fused", "fused_all"):   # point_chain's dropout stream starts from the run's seed
             model.point_chain_state.copy_(point_ops.new_dropout_state(self.seed, self.device))
 
     # -- state --------------------------------------------------------------------------------------------------------

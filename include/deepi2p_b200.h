@@ -1069,6 +1069,19 @@ int kitti_depth_records_f32(const double* xyz, const double* nrm, const float* i
  *   one-source operand of C rows, x an operand of K rows with n_src sources.  Split over the points, the splits
  *   summed in order in fp64.  workspace: 16-byte aligned, >= point_chain_dw_workspace_bytes.
  * point_chain_dropout_mask: out uint8 [B][C][N] = the keep bits of layer `layer` under drop_state (for tests).
+ *
+ * Grouped columns (DESIGN.md 4.36): G consecutive columns of a sample form a group (the K neighbours of a node, or
+ * all N nodes of a sample); G divides N.
+ * operand MODE DIB_PC_MODE_MAX_GRAD: a group max's gradient read back over the group, one source DATA f32
+ *   [B][CHANNELS][N / G] at batch stride BSTRIDE, Y = the max's int32 in-group indices in the same layout, LAYER = G:
+ *   row c, column n is DATA[b][c][n / G] where the index is n % G, else 0.
+ * point_chain_gemm_group_f32: point_chain_gemm_f32 with C <= DIB_PC_MAX_WIDTH (row blocks of 256 writing one [B][C][N]
+ *   and one partials table; packed holds all C rows) and add [B][C][N / add_group] added at column n from n / add_group.
+ * point_chain_group_max_f32: over a one-source operand of C rows: act [B][C][N] = its values (may be NULL) and max /
+ *   idx [B][C][N / G] = the max over each group and its in-group index by torch.max's rule (the first maximal value;
+ *   a NaN, the first one, over any number).
+ * point_chain_group_sum_f32: out [B][C][N / G] = the operand's sum over each group, in column order in fp64.
+ * point_chain_bn_f32 takes C <= DIB_PC_MAX_WIDTH.
  * ------------------------------------------------------------------------------------------ */
 #define DIB_PC_SRC 3
 #define DIB_PC_SRC_DATA 0
@@ -1087,6 +1100,8 @@ int kitti_depth_records_f32(const double* xyz, const double* nrm, const float* i
 #define DIB_PC_ACT_DROP_STATE 2
 #define DIB_PC_ACT_DROP_PPM 3
 #define DIB_PC_ACT_LAYER 4
+#define DIB_PC_MODE_MAX_GRAD 3
+#define DIB_PC_MAX_WIDTH 1024
 size_t point_chain_partial_bytes(int B, int N, int C);
 int point_chain_gemm_f32(const int64_t* operand, int n_src, const void* packed, const float* bias, const float* add,
                          int C, int B, int N, int epilogue, const int64_t* act, const float* act_y, float* out,
@@ -1099,6 +1114,13 @@ int point_chain_dw_f32(const int64_t* dy, const int64_t* x, int n_src, int B, in
                        void* workspace, size_t workspace_bytes, dib_stream_t stream);
 int point_chain_dropout_mask(const int64_t* drop_state, int layer, float p, int B, int C, int N, uint8_t* out,
                              dib_stream_t stream);
+int point_chain_gemm_group_f32(const int64_t* operand, int n_src, const void* packed, const float* bias,
+                               const float* add, int add_group, int C, int B, int N, int epilogue, const int64_t* act,
+                               const float* act_y, float* out, void* partials, size_t partial_bytes,
+                               dib_stream_t stream);
+int point_chain_group_max_f32(const int64_t* operand, int B, int N, int group, float* act, float* max, int32_t* idx,
+                              dib_stream_t stream);
+int point_chain_group_sum_f32(const int64_t* operand, int B, int N, int group, float* out, dib_stream_t stream);
 
 #ifdef __cplusplus
 }

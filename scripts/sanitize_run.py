@@ -123,5 +123,20 @@ if which in ("all", "accuracy"):
         a = classifier.prediction_accuracy(pc, P, K, 160, 512, cp, fp, return_labels=S != 3)
         print("accuracy", a["n_inside"].cpu().tolist(), a["coarse_correct"].cpu().tolist(),
               None if a["fine_correct"] is None else a["fine_correct"].cpu().tolist())
+if which in ("all", "point_branch"):
+    # a 300-row layer (two row blocks) with a group max over 7 of 77 x 7 columns, both outputs, then a 2-source chain
+    # on separate column ranges with a grouped additive term
+    from deepi2p_b200 import network
+    pn = network._PointNet(20, [300], True).cuda()
+    x = torch.randn(2, 20, 77 * 7, device="cuda", requires_grad=True)
+    act, mx = point_ops.point_branch([x], list(pn.layers), None, max_group=7, output="both")
+    (act.sum() + mx.sum()).backward()
+    pn2 = network._PointNet(40, [64, 16], True).cuda()
+    s1 = torch.randn(2, 10, 77, device="cuda", requires_grad=True)
+    s2 = torch.randn(2, 12, 77, device="cuda", requires_grad=True)
+    add = torch.randn(2, 64, 1, device="cuda", requires_grad=True)
+    y = point_ops.point_branch([s1, s2], list(pn2.layers), None, cols=[0, 28], add=add, add_group=77)
+    y.sum().backward()
+    print("point_branch", mx.abs().sum().item(), x.grad.abs().sum().item(), add.grad.abs().sum().item())
 torch.cuda.synchronize()
 print("done")

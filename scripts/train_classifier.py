@@ -39,7 +39,9 @@ def parse_args(argv=None):
     ap.add_argument("--store", default=None, choices=("cuda", "pinned"),
                     help="keep the scan records in one device or pinned store (KITTI, Oxford)")
     ap.add_argument("--point-layers", default="torch", choices=network.POINT_LAYERS,
-                    help="fused: the per-point chains as point_ops.point_chain (TF32, its own dropout stream)")
+                    help="fused: the per-point chains as point_ops.point_chain (TF32, its own dropout stream); "
+                         "fused_all: also the kNN module, final_pointnet and the node-level PointNets as "
+                         "point_ops.point_branch")
     a = ap.parse_args(argv)
     if a.epochs < 1:
         ap.error("--epochs must be >= 1")
