@@ -84,6 +84,28 @@ def _workspace(cache, need, device, stream=None, floor=1 << 20):
     return ws
 
 
+# dtypes of the feature operands of the ops that run under bfloat16 autocast (DESIGN.md 4.37), with the suffix of their
+# entry points
+FEATURE_DTYPES = {torch.float32: "f32", torch.bfloat16: "bf16"}
+
+
+def feature_dtype(named):
+    """The one dtype of an op's feature operands [(tensor or None, name)], float32 or bfloat16; returns (dtype, entry
+    point suffix).  Any other dtype raises RuntimeError "<name> must have dtype ...", operands of both dtypes raise
+    RuntimeError naming both."""
+    first = None
+    for t, name in named:
+        if t is None:
+            continue
+        if t.dtype not in FEATURE_DTYPES:
+            raise RuntimeError(f"{name} must have dtype {torch.float32} or {torch.bfloat16}")
+        if first is None:
+            first = (t.dtype, name)
+        elif t.dtype != first[0]:
+            raise RuntimeError(f"{first[1]} and {name} must have the same dtype, got {first[0]} and {t.dtype}")
+    return first[0], FEATURE_DTYPES[first[0]]
+
+
 def lib_path():
     return _build.LIB
 

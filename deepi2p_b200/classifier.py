@@ -13,7 +13,7 @@ import numbers
 import torch
 
 from . import _native
-from ._native import _ptr, _stream_ptr
+from ._native import _ptr, _stream_ptr, feature_dtype
 
 
 def fine_grid(H, W, fine_scale):
@@ -24,8 +24,7 @@ def fine_grid(H, W, fine_scale):
 def _check_scores(t, name, C=None):
     if not isinstance(t, torch.Tensor):
         raise TypeError(f"{name} must be a torch.Tensor")
-    if t.dtype != torch.float32:
-        raise RuntimeError(f"{name} must have dtype {torch.float32}")
+    feature_dtype(((t, name),))
     if t.dim() != 3 or (C is not None and t.shape[1] != C):
         raise RuntimeError(f"{name} must be [B,{C if C is not None else 'L'},N]")
 
@@ -41,6 +40,7 @@ def _check_args(coarse_scores, fine_scores, pc, P, K, H, W, fine_scale, focal_ga
         L = fine_scores.shape[1]
         if fine_scores.shape[0] != B or fine_scores.shape[2] != N:
             raise RuntimeError("fine_scores must be [B,L,N] with the B and N of coarse_scores")
+        feature_dtype(((coarse_scores, "coarse_scores"), (fine_scores, "fine_scores")))
     for t, name in ((pc, "pc"), (P, "P"), (K, "K")):
         if not isinstance(t, torch.Tensor):
             raise TypeError(f"{name} must be a torch.Tensor")
@@ -96,6 +96,7 @@ class _ClassifierLoss(torch.autograd.Function):
         lib = _native.load()
         dev = coarse_scores.device
         has_fine = fine_scores is not None
+        dtype, sfx = feature_dtype(((coarse_scores, "coarse_scores"), (fine_scores, "fine_scores")))
         coarse, cbs = _scores_view(coarse_scores)
         fine, fbs = _scores_view(fine_scores) if has_fine else (None, 0)
         with torch.cuda.device(dev):
@@ -112,14 +113,14 @@ class _ClassifierLoss(torch.autograd.Function):
             n_inside_total = torch.empty((1,), **i32)
             # per-CTA partials: from torch's allocator on every call, so that a captured graph owns its own
             ws = torch.empty((max(lib.classifier_loss_workspace_bytes(B, N), 8),), dtype=torch.uint8, device=dev)
-            rc = lib.classifier_loss_forward_f32(
+            rc = getattr(lib, f"classifier_loss_forward_{sfx}")(
                 coarse.data_ptr(), cbs, _ptr(fine), fbs, L, pc.data_ptr(), P12.data_ptr(), K9.data_ptr(), B, N,
                 float(H), float(W), float(s), H_f, W_f, float(coarse_alpha), float(focal_alpha), gamma, float(eps),
                 coarse_labels.data_ptr(), _ptr(fine_labels), coarse_pred.data_ptr(), _ptr(fine_pred), _ptr(lse),
                 loss.data_ptr(), coarse_loss.data_ptr(), fine_loss.data_ptr(), accuracy.data_ptr(),
                 n_inside.data_ptr(), coarse_correct.data_ptr(), _ptr(fine_correct), n_inside_total.data_ptr(),
                 ws.data_ptr(), ws.numel(), _stream_ptr())
-        _native.check(rc, "classifier_loss_forward_f32")
+        _native.check(rc, f"classifier_loss_forward_{sfx}")
         extras.update(coarse_labels=coarse_labels, fine_labels=fine_labels, coarse_predictions=coarse_pred,
                       fine_predictions=fine_pred, n_inside=n_inside, coarse_accuracy=accuracy[0],
                       fine_accuracy=accuracy[1] if has_fine else None, coarse_correct=coarse_correct,
@@ -127,6 +128,7 @@ class _ClassifierLoss(torch.autograd.Function):
         ctx.save_for_backward(coarse, fine, coarse_labels, fine_labels, lse, n_inside_total)
         ctx.cfg = cfg
         ctx.strides = (cbs, fbs)
+        ctx.dtype = (dtype, sfx)
         return loss, coarse_loss, fine_loss
 
     @staticmethod
@@ -137,17 +139,18 @@ class _ClassifierLoss(torch.autograd.Function):
         coarse, fine, coarse_labels, fine_labels, lse, n_inside_total = ctx.saved_tensors
         B, N, L, _, _, _, _, _, coarse_alpha, focal_alpha, gamma, eps = ctx.cfg
         cbs, fbs = ctx.strides
+        dtype, sfx = ctx.dtype
         dev = coarse.device
         g_loss, g_coarse, g_fine = (g.float().contiguous() for g in (g_loss, g_coarse, g_fine))
         lib = _native.load()
         with torch.cuda.device(dev):
-            gc = torch.empty((B, 2, N), dtype=torch.float32, device=dev) if want_c else None
-            gf = torch.empty((B, L, N), dtype=torch.float32, device=dev) if want_f else None
-            rc = lib.classifier_loss_backward_f32(
+            gc = torch.empty((B, 2, N), dtype=dtype, device=dev) if want_c else None
+            gf = torch.empty((B, L, N), dtype=dtype, device=dev) if want_f else None
+            rc = getattr(lib, f"classifier_loss_backward_{sfx}")(
                 coarse.data_ptr(), cbs, _ptr(fine), fbs, L, B, N, coarse_labels.data_ptr(), _ptr(fine_labels),
                 _ptr(lse), n_inside_total.data_ptr(), g_loss.data_ptr(), g_coarse.data_ptr(), g_fine.data_ptr(),
                 float(coarse_alpha), float(focal_alpha), gamma, float(eps), _ptr(gc), _ptr(gf), _stream_ptr())
-        _native.check(rc, "classifier_loss_backward_f32")
+        _native.check(rc, f"classifier_loss_backward_{sfx}")
         return gc, gf, None, None, None, None, None
 
 
@@ -156,8 +159,8 @@ def classifier_loss(coarse_scores, fine_scores, pc, P, K, H, W, fine_scale=32, c
     """Labels, losses, accuracies and predictions of one classifier step (models/multimodal_classifier.py:135-191;
     with fine_scores=None the coarse-only classifier, :482-508).
 
-    coarse_scores [B,2,N], fine_scores [B,L,N] or None, pc [B,3,N], all float32; P [B,3,4] or [B,4,4] and K [B,3,3]
-    float32 or float64 (read as fp64); all on one CUDA device.  Scores with (channel, point) strides (N, 1), such as
+    coarse_scores [B,2,N] and fine_scores [B,L,N] or None, both float32 or both bfloat16; pc [B,3,N] float32; P [B,3,4]
+    or [B,4,4] and K [B,3,3] float32 or float64 (read as fp64); all on one CUDA device.  Scores with (channel, point) strides (N, 1), such as
     the channel slices of the network's [B,2+L,N] output, are read without a copy.  L must be H_f * W_f with
     H_f = round(H / fine_scale), W_f = round(W / fine_scale).
 
@@ -175,7 +178,8 @@ def classifier_loss(coarse_scores, fine_scores, pc, P, K, H, W, fine_scale=32, c
       n_inside, coarse_correct, fine_correct   int32 [B] per sample (fine_correct counts inside points).
       coarse_accuracy, fine_accuracy           0-dim float32 from the integer counts (fine: NaN with no inside point).
     The fine_* entries are None for coarse-only.  No host synchronisation: the call is capturable in a CUDA graph.
-    pc, P and K must not require grad."""
+    pc, P and K must not require grad.  bfloat16 scores give every output of the float32 call on the widened scores,
+    and its score gradients rounded to bfloat16 (DESIGN.md 4.37)."""
     B, N, L, H_f, W_f = _check_args(coarse_scores, fine_scores, pc, P, K, H, W, fine_scale, focal_gamma)
     P12 = P[:, :3, :].to(torch.float64).reshape(B, 12).contiguous()
     K9 = K.to(torch.float64).reshape(B, 9).contiguous()

@@ -15,10 +15,13 @@
 //                        for evaluation, where the fused heads return predictions and no scores.
 // No atomics: every sum has an order fixed by the shape.  Per-point arithmetic is fp32, sums over points fp64.  The
 // file is compiled with --fmad=false (build.py NOFMA_SOURCES) so that the coarse label is inside_mask_kernel's
-// decision bit for bit.
+// decision bit for bit.  The forward and backward kernels are templated on the score type (float, or bf16 for the
+// *_bf16 entry points, feature_type.cuh): scores are widened at load and the score gradients rounded float -> bf16 at
+// store; everything else, losses, accuracies and predictions included, is computed as for float scores.
 #include <math.h>
 
 #include "common.cuh"
+#include "feature_type.cuh"
 #include "project.cuh"
 
 namespace dib {
@@ -100,8 +103,9 @@ __device__ __forceinline__ T warp_sum(T v) {
 
 // Partials [2][B][nblk] f64 (focal sum, cross-entropy sum over inside points) and [3][B][nblk] int32 (inside points,
 // correct coarse predictions, correct fine predictions of inside points).
+template <typename T>
 __global__ void __launch_bounds__(kClsThreads)
-    cls_forward_kernel(const float* __restrict__ coarse, long long cbs, const float* __restrict__ fine, long long fbs,
+    cls_forward_kernel(const T* __restrict__ coarse, long long cbs, const T* __restrict__ fine, long long fbs,
                        int L, const float* __restrict__ pc, const double* __restrict__ P12,
                        const double* __restrict__ K9, int B, int N, double H, double W, double s, int Wf, float alpha,
                        int gamma, float eps, int8_t* __restrict__ coarse_lab, int32_t* __restrict__ fine_lab,
@@ -116,8 +120,8 @@ __global__ void __launch_bounds__(kClsThreads)
     double u, v;
     const bool in = coarse_label(pc, P12, K9, b, n, N, H, W, &u, &v);
     const size_t bn = (size_t)b * N + n;
-    const float* zc = coarse + (size_t)b * cbs + n;
-    const float z0 = zc[0], z1 = zc[N];
+    const T* zc = coarse + (size_t)b * cbs + n;
+    const float z0 = load_f32(zc[0]), z1 = load_f32(zc[N]);
     const Focal2 f = focal2(z0, z1, in ? 1 : 0, alpha, gamma, eps);
     const int cp = (z0 == z0 && (z1 != z1 || z1 > z0)) ? 1 : 0;   // torch.max over two values
     coarse_lab[bn] = in ? 1 : 0;
@@ -127,17 +131,17 @@ __global__ void __launch_bounds__(kClsThreads)
     c_ok = cp == inside ? 1 : 0;
     if (fine) {
       const int label = fine_label(in, u, v, s, Wf);
-      const float* row = fine + (size_t)b * fbs + n;
+      const T* row = fine + (size_t)b * fbs + n;
       FineState st;
       int l = 0;
       for (; l + kClsChunk <= L; l += kClsChunk) {
         float z[kClsChunk];
 #pragma unroll
-        for (int j = 0; j < kClsChunk; ++j) z[j] = row[(size_t)(l + j) * N];
+        for (int j = 0; j < kClsChunk; ++j) z[j] = load_f32(row[(size_t)(l + j) * N]);
 #pragma unroll
         for (int j = 0; j < kClsChunk; ++j) st.step(z[j], l + j, label);
       }
-      for (; l < L; ++l) st.step(row[(size_t)l * N], l, label);
+      for (; l < L; ++l) st.step(load_f32(row[(size_t)l * N]), l, label);
       // the log-sum-exp kept in two parts, max and log of the shifted sum: z - m is exact near the top of the row, so
       // softmax = exp((z - m) - log_sum) keeps its digits when the logits are large
       const float ls = logf(st.sum);
@@ -226,46 +230,49 @@ __global__ void __launch_bounds__(kClsThreads)
   }
 }
 
+template <typename T>
 __global__ void __launch_bounds__(kClsThreads)
-    cls_backward_kernel(const float* __restrict__ coarse, long long cbs, const float* __restrict__ fine, long long fbs,
+    cls_backward_kernel(const T* __restrict__ coarse, long long cbs, const T* __restrict__ fine, long long fbs,
                         int L, int N, const int8_t* __restrict__ coarse_lab, const int32_t* __restrict__ fine_lab,
                         const float* __restrict__ lse, const int32_t* __restrict__ n_inside_total,
                         const float* __restrict__ g_loss, const float* __restrict__ g_coarse,
                         const float* __restrict__ g_fine, double coarse_scale, float alpha, int gamma, float eps,
-                        float* __restrict__ grad_coarse, float* __restrict__ grad_fine) {
+                        T* __restrict__ grad_coarse, T* __restrict__ grad_fine) {
   const int b = blockIdx.y, n = blockIdx.x * kClsThreads + threadIdx.x;
   if (n >= N) return;
   const size_t bn = (size_t)b * N + n;
   const float gl = *g_loss;
   if (grad_coarse) {
     const float sc = (float)(((double)gl + (double)*g_coarse) * coarse_scale);
-    const float* zc = coarse + (size_t)b * cbs + n;
-    const Focal2 f = focal2(zc[0], zc[N], coarse_lab[bn], alpha, gamma, eps);
+    const T* zc = coarse + (size_t)b * cbs + n;
+    const Focal2 f = focal2(load_f32(zc[0]), load_f32(zc[N]), coarse_lab[bn], alpha, gamma, eps);
     const float d = f.dz0 * sc;
-    float* gc = grad_coarse + (size_t)b * 2 * N + n;
-    gc[0] = d;
-    gc[N] = -d;
+    T* gc = grad_coarse + (size_t)b * 2 * N + n;
+    gc[0] = store_as<T>(d);
+    gc[N] = store_as<T>(-d);
   }
   if (grad_fine) {
-    float* gr = grad_fine + (size_t)b * L * N + n;
+    T* gr = grad_fine + (size_t)b * L * N + n;
     const int label = fine_lab[bn];
     if (label < 0) {
-      for (int l = 0; l < L; ++l) gr[(size_t)l * N] = 0.f;
+      for (int l = 0; l < L; ++l) gr[(size_t)l * N] = store_as<T>(0.f);
       return;
     }
     const float sf = (float)(((double)gl + (double)*g_fine) / (double)*n_inside_total);
     const float m = lse[bn], ls = lse[(size_t)gridDim.y * N + bn];
-    const float* row = fine + (size_t)b * fbs + n;
+    const T* row = fine + (size_t)b * fbs + n;
     int l = 0;
     for (; l + kClsChunk <= L; l += kClsChunk) {
       float z[kClsChunk];
 #pragma unroll
-      for (int j = 0; j < kClsChunk; ++j) z[j] = row[(size_t)(l + j) * N];
+      for (int j = 0; j < kClsChunk; ++j) z[j] = load_f32(row[(size_t)(l + j) * N]);
 #pragma unroll
       for (int j = 0; j < kClsChunk; ++j)
-        gr[(size_t)(l + j) * N] = (expf((z[j] - m) - ls) - (l + j == label ? 1.f : 0.f)) * sf;
+        gr[(size_t)(l + j) * N] = store_as<T>((expf((z[j] - m) - ls) - (l + j == label ? 1.f : 0.f)) * sf);
     }
-    for (; l < L; ++l) gr[(size_t)l * N] = (expf((row[(size_t)l * N] - m) - ls) - (l == label ? 1.f : 0.f)) * sf;
+    for (; l < L; ++l)
+      gr[(size_t)l * N] =
+          store_as<T>((expf((load_f32(row[(size_t)l * N]) - m) - ls) - (l == label ? 1.f : 0.f)) * sf);
   }
 }
 
@@ -329,7 +336,7 @@ size_t classifier_loss_workspace_bytes(int B, int N) {
 }
 
 // Shared host checks of both entry points.
-static int cls_check(const float* coarse, long long cbs, const float* fine, long long fbs, int L, int B, int N,
+static int cls_check(const void* coarse, long long cbs, const void* fine, long long fbs, int L, int B, int N,
                      int gamma, const char* what) {
   DIB_REQUIRE(B >= 1 && B <= 65535 && N >= 1, "%s: need 1 <= B <= 65535 and N >= 1", what);
   DIB_REQUIRE((long long)B * N < (1LL << 31), "%s: B * N must be below 2^31", what);
@@ -339,14 +346,16 @@ static int cls_check(const float* coarse, long long cbs, const float* fine, long
   return DIB_OK;
 }
 
-int classifier_loss_forward_f32(const float* coarse, int64_t coarse_batch_stride, const float* fine,
-                                int64_t fine_batch_stride, int L, const float* pc, const double* P12, const double* K9,
-                                int B, int N, double H, double W, double fine_scale, int H_f, int W_f,
-                                double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
-                                int8_t* coarse_labels, int32_t* fine_labels, int8_t* coarse_pred, int32_t* fine_pred,
-                                float* lse, float* loss, float* coarse_loss, float* fine_loss, float* accuracy,
-                                int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
-                                int32_t* n_inside_total, void* workspace, size_t workspace_bytes, dib_stream_t stream_) {
+}  // extern "C"
+
+template <typename T>
+static int cls_forward(const T* coarse, int64_t coarse_batch_stride, const T* fine, int64_t fine_batch_stride, int L,
+                       const float* pc, const double* P12, const double* K9, int B, int N, double H, double W,
+                       double fine_scale, int H_f, int W_f, double coarse_loss_alpha, double focal_alpha,
+                       int focal_gamma, double eps, int8_t* coarse_labels, int32_t* fine_labels, int8_t* coarse_pred,
+                       int32_t* fine_pred, float* lse, float* loss, float* coarse_loss, float* fine_loss,
+                       float* accuracy, int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
+                       int32_t* n_inside_total, void* workspace, size_t workspace_bytes, dib_stream_t stream_) {
   using namespace dib;
   cudaStream_t stream = (cudaStream_t)stream_;
   const int rc = cls_check(coarse, coarse_batch_stride, fine, fine_batch_stride, L, B, N, focal_gamma,
@@ -370,7 +379,7 @@ int classifier_loss_forward_f32(const float* coarse, int64_t coarse_batch_stride
   const int nblk = cls_blocks(N);
   double* part_d = (double*)workspace;
   int32_t* part_i = (int32_t*)(part_d + 2 * (size_t)B * nblk);
-  cls_forward_kernel<<<dim3(nblk, B), kClsThreads, 0, stream>>>(
+  cls_forward_kernel<T><<<dim3(nblk, B), kClsThreads, 0, stream>>>(
       coarse, coarse_batch_stride, fine, fine_batch_stride, L, pc, P12, K9, B, N, H, W, fine_scale, W_f,
       (float)focal_alpha, focal_gamma, (float)eps, coarse_labels, fine_labels, coarse_pred, fine_pred, lse, part_d,
       part_i);
@@ -380,6 +389,63 @@ int classifier_loss_forward_f32(const float* coarse, int64_t coarse_batch_stride
                                                    fine ? fine_correct : nullptr, n_inside_total);
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
+}
+
+template <typename T>
+static int cls_backward(const T* coarse, int64_t coarse_batch_stride, const T* fine, int64_t fine_batch_stride, int L,
+                        int B, int N, const int8_t* coarse_labels, const int32_t* fine_labels, const float* lse,
+                        const int32_t* n_inside_total, const float* grad_loss, const float* grad_coarse_loss,
+                        const float* grad_fine_loss, double coarse_loss_alpha, double focal_alpha, int focal_gamma,
+                        double eps, T* grad_coarse, T* grad_fine, dib_stream_t stream_) {
+  using namespace dib;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int rc = cls_check(coarse, coarse_batch_stride, fine, fine_batch_stride, L, B, N, focal_gamma,
+                           "classifier_loss_backward");
+  if (rc != DIB_OK) return rc;
+  DIB_REQUIRE(grad_loss && coarse_labels, "classifier_loss_backward: NULL argument");
+  DIB_REQUIRE(!grad_coarse || grad_coarse_loss, "classifier_loss_backward: NULL coarse upstream gradient");
+  DIB_REQUIRE(!grad_fine || (fine && fine_labels && lse && n_inside_total && grad_fine_loss),
+              "classifier_loss_backward: NULL fine argument");
+  if (!grad_coarse && !grad_fine) return DIB_OK;
+  const double coarse_scale = coarse_loss_alpha / ((double)B * (double)N);
+  cls_backward_kernel<T><<<dim3(cls_blocks(N), B), kClsThreads, 0, stream>>>(
+      coarse, coarse_batch_stride, fine, fine_batch_stride, L, N, coarse_labels, fine_labels, lse, n_inside_total,
+      grad_loss, grad_coarse_loss, grad_fine_loss, coarse_scale, (float)focal_alpha, focal_gamma, (float)eps,
+      grad_coarse, grad_fine);
+  DIB_CHECK_CUDA(cudaGetLastError());
+  return DIB_OK;
+}
+
+extern "C" {
+
+int classifier_loss_forward_f32(const float* coarse, int64_t coarse_batch_stride, const float* fine,
+                                int64_t fine_batch_stride, int L, const float* pc, const double* P12, const double* K9,
+                                int B, int N, double H, double W, double fine_scale, int H_f, int W_f,
+                                double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
+                                int8_t* coarse_labels, int32_t* fine_labels, int8_t* coarse_pred, int32_t* fine_pred,
+                                float* lse, float* loss, float* coarse_loss, float* fine_loss, float* accuracy,
+                                int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
+                                int32_t* n_inside_total, void* workspace, size_t workspace_bytes, dib_stream_t stream) {
+  return cls_forward(coarse, coarse_batch_stride, fine, fine_batch_stride, L, pc, P12, K9, B, N, H, W, fine_scale, H_f,
+                     W_f, coarse_loss_alpha, focal_alpha, focal_gamma, eps, coarse_labels, fine_labels, coarse_pred,
+                     fine_pred, lse, loss, coarse_loss, fine_loss, accuracy, n_inside, coarse_correct, fine_correct,
+                     n_inside_total, workspace, workspace_bytes, stream);
+}
+
+int classifier_loss_forward_bf16(const uint16_t* coarse, int64_t coarse_batch_stride, const uint16_t* fine,
+                                 int64_t fine_batch_stride, int L, const float* pc, const double* P12,
+                                 const double* K9, int B, int N, double H, double W, double fine_scale, int H_f,
+                                 int W_f, double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
+                                 int8_t* coarse_labels, int32_t* fine_labels, int8_t* coarse_pred, int32_t* fine_pred,
+                                 float* lse, float* loss, float* coarse_loss, float* fine_loss, float* accuracy,
+                                 int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
+                                 int32_t* n_inside_total, void* workspace, size_t workspace_bytes,
+                                 dib_stream_t stream) {
+  using dib::as_bf16;
+  return cls_forward(as_bf16(coarse), coarse_batch_stride, as_bf16(fine), fine_batch_stride, L, pc, P12, K9, B, N, H,
+                     W, fine_scale, H_f, W_f, coarse_loss_alpha, focal_alpha, focal_gamma, eps, coarse_labels,
+                     fine_labels, coarse_pred, fine_pred, lse, loss, coarse_loss, fine_loss, accuracy, n_inside,
+                     coarse_correct, fine_correct, n_inside_total, workspace, workspace_bytes, stream);
 }
 
 int classifier_prediction_accuracy_f32(const float* pc, const double* P12, const double* K9, const int8_t* coarse_pred,
@@ -413,24 +479,22 @@ int classifier_loss_backward_f32(const float* coarse, int64_t coarse_batch_strid
                                  const int32_t* fine_labels, const float* lse, const int32_t* n_inside_total,
                                  const float* grad_loss, const float* grad_coarse_loss, const float* grad_fine_loss,
                                  double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
-                                 float* grad_coarse, float* grad_fine, dib_stream_t stream_) {
-  using namespace dib;
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int rc = cls_check(coarse, coarse_batch_stride, fine, fine_batch_stride, L, B, N, focal_gamma,
-                           "classifier_loss_backward");
-  if (rc != DIB_OK) return rc;
-  DIB_REQUIRE(grad_loss && coarse_labels, "classifier_loss_backward: NULL argument");
-  DIB_REQUIRE(!grad_coarse || grad_coarse_loss, "classifier_loss_backward: NULL coarse upstream gradient");
-  DIB_REQUIRE(!grad_fine || (fine && fine_labels && lse && n_inside_total && grad_fine_loss),
-              "classifier_loss_backward: NULL fine argument");
-  if (!grad_coarse && !grad_fine) return DIB_OK;
-  const double coarse_scale = coarse_loss_alpha / ((double)B * (double)N);
-  cls_backward_kernel<<<dim3(cls_blocks(N), B), kClsThreads, 0, stream>>>(
-      coarse, coarse_batch_stride, fine, fine_batch_stride, L, N, coarse_labels, fine_labels, lse, n_inside_total,
-      grad_loss, grad_coarse_loss, grad_fine_loss, coarse_scale, (float)focal_alpha, focal_gamma, (float)eps,
-      grad_coarse, grad_fine);
-  DIB_CHECK_CUDA(cudaGetLastError());
-  return DIB_OK;
+                                 float* grad_coarse, float* grad_fine, dib_stream_t stream) {
+  return cls_backward(coarse, coarse_batch_stride, fine, fine_batch_stride, L, B, N, coarse_labels, fine_labels, lse,
+                      n_inside_total, grad_loss, grad_coarse_loss, grad_fine_loss, coarse_loss_alpha, focal_alpha,
+                      focal_gamma, eps, grad_coarse, grad_fine, stream);
+}
+
+int classifier_loss_backward_bf16(const uint16_t* coarse, int64_t coarse_batch_stride, const uint16_t* fine,
+                                  int64_t fine_batch_stride, int L, int B, int N, const int8_t* coarse_labels,
+                                  const int32_t* fine_labels, const float* lse, const int32_t* n_inside_total,
+                                  const float* grad_loss, const float* grad_coarse_loss, const float* grad_fine_loss,
+                                  double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
+                                  uint16_t* grad_coarse, uint16_t* grad_fine, dib_stream_t stream) {
+  using dib::as_bf16;
+  return cls_backward(as_bf16(coarse), coarse_batch_stride, as_bf16(fine), fine_batch_stride, L, B, N, coarse_labels,
+                      fine_labels, lse, n_inside_total, grad_loss, grad_coarse_loss, grad_fine_loss, coarse_loss_alpha,
+                      focal_alpha, focal_gamma, eps, as_bf16(grad_coarse), as_bf16(grad_fine), stream);
 }
 
 }  // extern "C"

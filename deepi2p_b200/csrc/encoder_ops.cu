@@ -27,9 +27,12 @@
 //     knn_reduce_kernel       gF[b][c][n] = float(((p_0 + p_1) + ...) + p_{S-1}) over the slice partials.
 // Each accumulator has one owner and a fixed order: no float atomics, bit-identical across runs and streams.
 // Single-precision arithmetic is written with explicit-rounding intrinsics, so FMA contraction cannot change it.
+// The feature kernels are templated on the feature type (float, or bf16 for the *_bf16 entry points, feature_type.cuh):
+// features, pooled / scattered / grouped and the gradients convert at load and store, the arithmetic is unchanged.
 #include <math.h>
 
 #include "common.cuh"
+#include "feature_type.cuh"
 #include "nearest_k.cuh"
 
 namespace dib {
@@ -47,6 +50,11 @@ constexpr int kSegRange = 128;                 // segments per segment-sum CTA (
 constexpr int kSegTargetCtas = 1024;           // slices are added until the grid has about this many CTAs ...
 constexpr int kSegMinTiles = 16;               // ... while every slice keeps at least this many tiles
 
+// point_ops.cu: index_max_forward's launch, for float and bf16 data
+template <typename T>
+int index_max_launch(const T* data, const int32_t* index, int32_t* out, int B, int C, int N, int K,
+                     dib_stream_t stream);
+
 __global__ void pool_mask_kernel(const int32_t* __restrict__ min_idx, int N, int M, float* __restrict__ mask) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
   if (n >= N) return;
@@ -55,29 +63,31 @@ __global__ void pool_mask_kernel(const int32_t* __restrict__ min_idx, int N, int
 }
 
 // one thread per (b, c, m)
-__global__ void pool_gather_kernel(const float* __restrict__ features, const int32_t* __restrict__ sel,
+template <typename T>
+__global__ void pool_gather_kernel(const T* __restrict__ features, const int32_t* __restrict__ sel,
                                    const float* __restrict__ mask, int C, int N, int M, size_t total,
-                                   float* __restrict__ pooled) {
+                                   T* __restrict__ pooled) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const size_t bc = i / M;
   const int m = (int)(i % M), b = (int)(bc / C);
-  pooled[i] = __fmul_rn(features[bc * N + sel[i]], mask[(size_t)b * M + m]);
+  pooled[i] = store_as<T>(__fmul_rn(load_f32(features[bc * N + sel[i]]), mask[(size_t)b * M + m]));
 }
 
 // grid (ceil(N / 256), ceil(C / 16), B)
+template <typename T>
 __global__ void __launch_bounds__(kScatterThreads)
-    pool_scatter_kernel(const float* __restrict__ pooled, const int32_t* __restrict__ min_idx, int C, int N, int M,
-                        float* __restrict__ scattered) {
+    pool_scatter_kernel(const T* __restrict__ pooled, const int32_t* __restrict__ min_idx, int C, int N, int M,
+                        T* __restrict__ scattered) {
   const int n = blockIdx.x * kScatterThreads + threadIdx.x, b = blockIdx.z, c0 = blockIdx.y * kScatterChannels;
   if (n >= N) return;
   const int nc = min(kScatterChannels, C - c0);
   const int m = min_idx[(size_t)b * N + n];
   const bool ok = m >= 0 && m < M;
-  const float* pr = pooled + ((size_t)b * C + c0) * M + (ok ? m : 0);
-  float* o = scattered + ((size_t)b * C + c0) * N + n;
+  const T* pr = pooled + ((size_t)b * C + c0) * M + (ok ? m : 0);
+  T* o = scattered + ((size_t)b * C + c0) * N + n;
 #pragma unroll 4
-  for (int c = 0; c < nc; ++c) o[(size_t)c * N] = ok ? pr[(size_t)c * M] : __int_as_float(0x7fc00000);
+  for (int c = 0; c < nc; ++c) o[(size_t)c * N] = ok ? pr[(size_t)c * M] : store_as<T>(__int_as_float(0x7fc00000));
 }
 
 template <int KK>
@@ -120,29 +130,31 @@ int knn_search_launch(const float* query, const float* database, int B, int M, i
 }
 
 // grid (ceil(M * K / 256), ceil((3 + C) / 16), B)
+template <typename T>
 __global__ void __launch_bounds__(kGroupThreads)
     knn_group_kernel(const float* __restrict__ query, const float* __restrict__ database,
-                     const float* __restrict__ features, const int32_t* __restrict__ knn_idx, int C, int M, int N,
-                     int K, float* __restrict__ grouped) {
+                     const T* __restrict__ features, const int32_t* __restrict__ knn_idx, int C, int M, int N,
+                     int K, T* __restrict__ grouped) {
   const int e = blockIdx.x * kGroupThreads + threadIdx.x, b = blockIdx.z;
   const size_t MK = (size_t)M * K;
   if ((size_t)e >= MK) return;
   const int n = knn_idx[b * MK + e], m = e / K;
   const int r0 = blockIdx.y * kGroupRows, r1 = min(3 + C, r0 + kGroupRows);
-  float* o = grouped + (size_t)b * (3 + C) * MK + e;
+  T* o = grouped + (size_t)b * (3 + C) * MK + e;
 #pragma unroll 4
   for (int r = r0; r < r1; ++r) {
     const float v = r < 3 ? __fsub_rn(database[((size_t)b * 3 + r) * N + n], query[((size_t)b * 3 + r) * M + m])
-                          : features[((size_t)b * C + (r - 3)) * N + n];
-    o[(size_t)r * MK] = v;
+                          : load_f32(features[((size_t)b * C + (r - 3)) * N + n]);
+    o[(size_t)r * MK] = store_as<T>(v);
   }
 }
 
 // grid (slices * ranges, ceil(C / 32), B), 32 threads.  g element (b, c, l) at b * g_batch_stride + c * L + l; seg
 // [B][L] int32, a value outside [0, S) joins no segment.  Partials [B][slices][C][S] f64.  The next tile's g and seg
 // are loaded into registers while the current one is accumulated.
+template <typename T>
 __global__ void __launch_bounds__(kSegChannels)
-    segment_sum_kernel(const float* __restrict__ g, int64_t g_batch_stride, const int32_t* __restrict__ seg, int C,
+    segment_sum_kernel(const T* __restrict__ g, int64_t g_batch_stride, const int32_t* __restrict__ seg, int C,
                        int L, int S, int slices, int slice_len, double* __restrict__ partial) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int ranges = (S + kSegRange - 1) / kSegRange;
@@ -156,7 +168,7 @@ __global__ void __launch_bounds__(kSegChannels)
   const int nc = min(kSegChannels, C - c0);
   for (int i = lane; i < kSegChannels * stride; i += 32) acc[i] = 0.0;
   const int l_begin = s * slice_len, l_end = min(L, l_begin + slice_len);
-  const float* gb = g + (size_t)b * g_batch_stride + (size_t)c0 * L;
+  const T* gb = g + (size_t)b * g_batch_stride + (size_t)c0 * L;
   const int32_t* sb = seg + (size_t)b * L;
   double* my = acc + lane * stride;
   float pg[kSegChannels];
@@ -164,7 +176,7 @@ __global__ void __launch_bounds__(kSegChannels)
   auto fetch = [&](int t0) {                                  // lane = element of the tile
     const int tn = min(kSegTile, l_end - t0);
 #pragma unroll
-    for (int c = 0; c < kSegChannels; ++c) pg[c] = (c < nc && lane < tn) ? gb[(size_t)c * L + t0 + lane] : 0.f;
+    for (int c = 0; c < kSegChannels; ++c) pg[c] = (c < nc && lane < tn) ? load_f32(gb[(size_t)c * L + t0 + lane]) : 0.f;
     pi = lane < tn ? sb[t0 + lane] : -1;
   };
   if (l_begin < l_end) fetch(l_begin);
@@ -191,16 +203,17 @@ __global__ void __launch_bounds__(kSegChannels)
 }
 
 // one warp per (b, c); gP [B][C][M] (may be NULL), partial [B][slices][C][M] (NULL: no scattered gradient).
-__global__ void pool_finish_kernel(const float* __restrict__ gP, const double* __restrict__ partial, int slices,
+template <typename T>
+__global__ void pool_finish_kernel(const T* __restrict__ gP, const double* __restrict__ partial, int slices,
                                    const int32_t* __restrict__ sel, const float* __restrict__ mask, int B, int C,
-                                   int N, int M, float* __restrict__ gF) {
+                                   int N, int M, T* __restrict__ gF) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= (long long)B * C) return;                           // warp-uniform
   const int b = (int)(w / C), c = (int)(w % C);
   const size_t row = (size_t)w * M;
   const size_t cm = (size_t)C * M;
-  float* out = gF + (size_t)w * N;
+  T* out = gF + (size_t)w * N;
   double z = 0.0;
   bool any0 = false;
   for (int mb = 0; mb < M; mb += 32) {
@@ -213,13 +226,13 @@ __global__ void pool_finish_kernel(const float* __restrict__ gP, const double* _
         const double* p = partial + (size_t)b * slices * cm + (size_t)c * M + m;
         sum = p[0];
         for (int s = 1; s < slices; ++s) sum += p[(size_t)s * cm];
-        if (gP) sum = (double)gP[row + m] + sum;
+        if (gP) sum = (double)load_f32(gP[row + m]) + sum;
       } else {
-        sum = (double)gP[row + m];
+        sum = (double)load_f32(gP[row + m]);
       }
       t = sum * (double)mask[(size_t)b * M + m];
       n = sel[row + m];
-      if (n != 0) out[n] = (float)t;                           // one segment per point: no other writer
+      if (n != 0) out[n] = store_as<T>((float)t);                           // one segment per point: no other writer
     }
     unsigned zm = __ballot_sync(0xffffffffu, m < M && n == 0);
     while (zm) {                                               // ascending m
@@ -230,19 +243,20 @@ __global__ void pool_finish_kernel(const float* __restrict__ gP, const double* _
       zm &= zm - 1;
     }
   }
-  if (lane == 0 && any0) out[0] = (float)z;
+  if (lane == 0 && any0) out[0] = store_as<T>((float)z);
 }
 
 // one thread per (b, c, n)
+template <typename T>
 __global__ void knn_reduce_kernel(const double* __restrict__ partial, int C, int N, int slices, size_t total,
-                                  float* __restrict__ gF) {
+                                  T* __restrict__ gF) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const size_t cn = (size_t)C * N, b = i / cn, r = i % cn;
   const double* p = partial + b * slices * cn + r;
   double sum = p[0];
   for (int s = 1; s < slices; ++s) sum += p[(size_t)s * cn];
-  gF[i] = (float)sum;
+  gF[i] = store_as<T>((float)sum);
 }
 
 // Slices of the segment sum: a function of the shape alone, so a given shape always sums in the same order.
@@ -273,7 +287,8 @@ inline size_t seg_workspace_bytes(int B, int C, int L, int S) {
 }
 
 // partial [B][slices][C][S] from g (element (b, c, l) at b * g_batch_stride + c * L + l) and seg [B][L]
-inline int launch_segment_sum(const float* g, int64_t g_batch_stride, const int32_t* seg, int B, int C, int L, int S,
+template <typename T>
+inline int launch_segment_sum(const T* g, int64_t g_batch_stride, const int32_t* seg, int B, int C, int L, int S,
                               double* partial, int* slices, cudaStream_t stream) {
   int slice_len;
   seg_slices(B, C, L, S, slices, &slice_len);
@@ -285,13 +300,9 @@ inline int launch_segment_sum(const float* g, int64_t g_batch_stride, const int3
   return DIB_OK;
 }
 
-}  // namespace dib
-
-extern "C" {
-
-int cluster_pool_forward_f32(const float* features, const int32_t* min_idx, int B, int C, int N, int M, int32_t* sel,
-                             float* mask, float* pooled, float* scattered, dib_stream_t stream_) {
-  using namespace dib;
+template <typename T>
+int cluster_pool_forward(const T* features, const int32_t* min_idx, int B, int C, int N, int M, int32_t* sel,
+                         float* mask, T* pooled, T* scattered, dib_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   DIB_REQUIRE(B >= 0 && C >= 0 && B <= 65535, "cluster_pool: need 0 <= B <= 65535, C >= 0");
   DIB_REQUIRE(N >= 1 && M >= 1, "cluster_pool: need N >= 1 and M >= 1");
@@ -303,7 +314,7 @@ int cluster_pool_forward_f32(const float* features, const int32_t* min_idx, int 
   if (C == 0) return DIB_OK;
   DIB_REQUIRE(features && sel && pooled, "cluster_pool: NULL argument");
   DIB_REQUIRE((C + kScatterChannels - 1) / kScatterChannels <= 65535, "cluster_pool: too many channels");
-  const int rc = index_max_forward(features, min_idx, sel, B, C, N, M, stream_);
+  const int rc = index_max_launch(features, min_idx, sel, B, C, N, M, stream_);
   if (rc != DIB_OK) return rc;
   const size_t total = (size_t)B * C * M;
   pool_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(features, sel, mask, C, N, M, total, pooled);
@@ -316,20 +327,16 @@ int cluster_pool_forward_f32(const float* features, const int32_t* min_idx, int 
   return DIB_OK;
 }
 
-size_t cluster_pool_backward_workspace_bytes(int B, int C, int N, int M) {
-  return dib::seg_workspace_bytes(B, C, N, M);
-}
-
-int cluster_pool_backward_f32(const float* grad_pooled, const float* grad_scattered, int64_t grad_scattered_batch_stride,
-                              const int32_t* min_idx, const int32_t* sel, const float* mask, int B, int C, int N, int M,
-                              float* grad_features, void* workspace, size_t workspace_bytes, dib_stream_t stream_) {
-  using namespace dib;
+template <typename T>
+int cluster_pool_backward(const T* grad_pooled, const T* grad_scattered, int64_t grad_scattered_batch_stride,
+                          const int32_t* min_idx, const int32_t* sel, const float* mask, int B, int C, int N, int M,
+                          T* grad_features, void* workspace, size_t workspace_bytes, dib_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   DIB_REQUIRE(B >= 0 && C >= 0 && B <= 65535, "cluster_pool_backward: need 0 <= B <= 65535, C >= 0");
   DIB_REQUIRE(N >= 1 && M >= 1, "cluster_pool_backward: need N >= 1 and M >= 1");
   if (B == 0 || C == 0) return DIB_OK;
   DIB_REQUIRE(grad_features && sel && mask, "cluster_pool_backward: NULL argument");
-  DIB_CHECK_CUDA(cudaMemsetAsync(grad_features, 0, (size_t)B * C * N * sizeof(float), stream));
+  DIB_CHECK_CUDA(cudaMemsetAsync(grad_features, 0, (size_t)B * C * N * sizeof(T), stream));
   if (!grad_pooled && !grad_scattered) return DIB_OK;
   double* partial = nullptr;
   int slices = 0;
@@ -337,7 +344,7 @@ int cluster_pool_backward_f32(const float* grad_pooled, const float* grad_scatte
     DIB_REQUIRE(min_idx, "cluster_pool_backward: NULL argument");
     DIB_REQUIRE(grad_scattered_batch_stride >= 0, "cluster_pool_backward: grad_scattered_batch_stride < 0");
     DIB_REQUIRE((C + kSegChannels - 1) / kSegChannels <= 65535, "cluster_pool_backward: too many channels");
-    const size_t need = cluster_pool_backward_workspace_bytes(B, C, N, M);
+    const size_t need = seg_workspace_bytes(B, C, N, M);
     DIB_REQUIRE(workspace && workspace_bytes >= need && ((uintptr_t)workspace & 7) == 0,
                 "cluster_pool_backward: workspace too small or misaligned");
     partial = (double*)workspace;
@@ -352,9 +359,9 @@ int cluster_pool_backward_f32(const float* grad_pooled, const float* grad_scatte
   return DIB_OK;
 }
 
-int knn_group_forward_f32(const float* query, const float* database, const float* features, int B, int C, int M,
-                          int N, int K, int32_t* knn_idx, float* grouped, dib_stream_t stream_) {
-  using namespace dib;
+template <typename T>
+int knn_group_forward(const float* query, const float* database, const T* features, int B, int C, int M, int N,
+                      int K, int32_t* knn_idx, T* grouped, dib_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   DIB_REQUIRE(B >= 0 && C >= 0 && M >= 0 && B <= 65535, "knn_group: need 0 <= B <= 65535, C, M >= 0");
   DIB_REQUIRE(N >= 1 && N <= kKnnMaxNodes, "knn_group: need 1 <= N <= 2048");
@@ -372,15 +379,9 @@ int knn_group_forward_f32(const float* query, const float* database, const float
   return DIB_OK;
 }
 
-size_t knn_group_backward_workspace_bytes(int B, int C, int M, int N, int K) {
-  if ((long long)M * K > 0x7fffffffLL) return 0;
-  return dib::seg_workspace_bytes(B, C, M * K, N);
-}
-
-int knn_group_backward_f32(const float* grad_grouped, int64_t grad_batch_stride, const int32_t* knn_idx, int B, int C,
-                           int M, int N, int K, float* grad_features, void* workspace, size_t workspace_bytes,
-                           dib_stream_t stream_) {
-  using namespace dib;
+template <typename T>
+int knn_group_backward(const T* grad_grouped, int64_t grad_batch_stride, const int32_t* knn_idx, int B, int C, int M,
+                       int N, int K, T* grad_features, void* workspace, size_t workspace_bytes, dib_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   DIB_REQUIRE(B >= 0 && C >= 0 && M >= 0 && B <= 65535, "knn_group_backward: need 0 <= B <= 65535, C, M >= 0");
   DIB_REQUIRE(N >= 1 && N <= kKnnMaxNodes, "knn_group_backward: need 1 <= N <= 2048");
@@ -389,13 +390,13 @@ int knn_group_backward_f32(const float* grad_grouped, int64_t grad_batch_stride,
   if (B == 0 || C == 0) return DIB_OK;
   DIB_REQUIRE(grad_features, "knn_group_backward: NULL argument");
   if (M == 0) {
-    DIB_CHECK_CUDA(cudaMemsetAsync(grad_features, 0, (size_t)B * C * N * sizeof(float), stream));
+    DIB_CHECK_CUDA(cudaMemsetAsync(grad_features, 0, (size_t)B * C * N * sizeof(T), stream));
     return DIB_OK;
   }
   DIB_REQUIRE(grad_grouped && knn_idx, "knn_group_backward: NULL argument");
   DIB_REQUIRE(grad_batch_stride >= 0, "knn_group_backward: grad_batch_stride < 0");
   DIB_REQUIRE((C + kSegChannels - 1) / kSegChannels <= 65535, "knn_group_backward: too many channels");
-  const size_t need = knn_group_backward_workspace_bytes(B, C, M, N, K);
+  const size_t need = seg_workspace_bytes(B, C, M * K, N);
   DIB_REQUIRE(workspace && workspace_bytes >= need && ((uintptr_t)workspace & 7) == 0,
               "knn_group_backward: workspace too small or misaligned");
   const int L = M * K;
@@ -408,6 +409,74 @@ int knn_group_backward_f32(const float* grad_grouped, int64_t grad_batch_stride,
   knn_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(partial, C, N, slices, total, grad_features);
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
+}
+
+}  // namespace dib
+
+extern "C" {
+
+int cluster_pool_forward_f32(const float* features, const int32_t* min_idx, int B, int C, int N, int M, int32_t* sel,
+                             float* mask, float* pooled, float* scattered, dib_stream_t stream) {
+  return dib::cluster_pool_forward(features, min_idx, B, C, N, M, sel, mask, pooled, scattered, stream);
+}
+
+int cluster_pool_forward_bf16(const uint16_t* features, const int32_t* min_idx, int B, int C, int N, int M,
+                              int32_t* sel, float* mask, uint16_t* pooled, uint16_t* scattered, dib_stream_t stream) {
+  using dib::as_bf16;
+  return dib::cluster_pool_forward(as_bf16(features), min_idx, B, C, N, M, sel, mask, as_bf16(pooled),
+                                   as_bf16(scattered), stream);
+}
+
+size_t cluster_pool_backward_workspace_bytes(int B, int C, int N, int M) {
+  return dib::seg_workspace_bytes(B, C, N, M);
+}
+
+int cluster_pool_backward_f32(const float* grad_pooled, const float* grad_scattered, int64_t grad_scattered_batch_stride,
+                              const int32_t* min_idx, const int32_t* sel, const float* mask, int B, int C, int N, int M,
+                              float* grad_features, void* workspace, size_t workspace_bytes, dib_stream_t stream) {
+  return dib::cluster_pool_backward(grad_pooled, grad_scattered, grad_scattered_batch_stride, min_idx, sel, mask, B, C,
+                                    N, M, grad_features, workspace, workspace_bytes, stream);
+}
+
+int cluster_pool_backward_bf16(const uint16_t* grad_pooled, const uint16_t* grad_scattered,
+                               int64_t grad_scattered_batch_stride, const int32_t* min_idx, const int32_t* sel,
+                               const float* mask, int B, int C, int N, int M, uint16_t* grad_features, void* workspace,
+                               size_t workspace_bytes, dib_stream_t stream) {
+  using dib::as_bf16;
+  return dib::cluster_pool_backward(as_bf16(grad_pooled), as_bf16(grad_scattered), grad_scattered_batch_stride,
+                                    min_idx, sel, mask, B, C, N, M, as_bf16(grad_features), workspace,
+                                    workspace_bytes, stream);
+}
+
+int knn_group_forward_f32(const float* query, const float* database, const float* features, int B, int C, int M,
+                          int N, int K, int32_t* knn_idx, float* grouped, dib_stream_t stream) {
+  return dib::knn_group_forward(query, database, features, B, C, M, N, K, knn_idx, grouped, stream);
+}
+
+int knn_group_forward_bf16(const float* query, const float* database, const uint16_t* features, int B, int C, int M,
+                           int N, int K, int32_t* knn_idx, uint16_t* grouped, dib_stream_t stream) {
+  using dib::as_bf16;
+  return dib::knn_group_forward(query, database, as_bf16(features), B, C, M, N, K, knn_idx, as_bf16(grouped), stream);
+}
+
+size_t knn_group_backward_workspace_bytes(int B, int C, int M, int N, int K) {
+  if ((long long)M * K > 0x7fffffffLL) return 0;
+  return dib::seg_workspace_bytes(B, C, M * K, N);
+}
+
+int knn_group_backward_f32(const float* grad_grouped, int64_t grad_batch_stride, const int32_t* knn_idx, int B, int C,
+                           int M, int N, int K, float* grad_features, void* workspace, size_t workspace_bytes,
+                           dib_stream_t stream) {
+  return dib::knn_group_backward(grad_grouped, grad_batch_stride, knn_idx, B, C, M, N, K, grad_features, workspace,
+                                 workspace_bytes, stream);
+}
+
+int knn_group_backward_bf16(const uint16_t* grad_grouped, int64_t grad_batch_stride, const int32_t* knn_idx, int B,
+                            int C, int M, int N, int K, uint16_t* grad_features, void* workspace,
+                            size_t workspace_bytes, dib_stream_t stream) {
+  using dib::as_bf16;
+  return dib::knn_group_backward(as_bf16(grad_grouped), grad_batch_stride, knn_idx, B, C, M, N, K,
+                                 as_bf16(grad_features), workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -18,7 +18,11 @@
 // loop reproduces bit for bit whatever the tile size.  k past the end is zero in both operands, and fma(0, 0, s) == s
 // for every s the sum can hold (never -0.0: it starts at +0.0 and an exact cancellation rounds to +0.0).  No atomics
 // and no workspace: bit-identical across runs, streams and batch compositions.
+//
+// The kernel is templated on the operand type T (float, or bf16 for the *_bf16 entry points, feature_type.cuh): the
+// operands are widened at load, the result rounded float -> T at store; the fp64 accumulation is the same.
 #include "common.cuh"
+#include "feature_type.cuh"
 
 namespace dib {
 
@@ -26,10 +30,10 @@ constexpr int kFusionBK = 16;                  // k per shared-memory chunk
 constexpr int kFusionMaxRowTiles = 65535;      // grid y: row tiles of the 32-row kernel
 constexpr long long kFusionBigTiles = 264;     // 64 x 64 tiles from two per SM of a 132-SM H100 up, else 32 x 32
 
-template <int BM, int BN, bool XK, bool YK>
+template <int BM, int BN, bool XK, bool YK, typename T>
 __global__ void __launch_bounds__((BM / 4) * (BN / 4))
-    fusion_tile_kernel(const float* __restrict__ x, int64_t xb, int64_t xi, int64_t xk, const float* __restrict__ y,
-                       int64_t yb, int64_t yk, int64_t yj, int I, int J, int K, double div, float* __restrict__ out) {
+    fusion_tile_kernel(const T* __restrict__ x, int64_t xb, int64_t xi, int64_t xk, const T* __restrict__ y,
+                       int64_t yb, int64_t yk, int64_t yj, int I, int J, int K, double div, T* __restrict__ out) {
   constexpr int TX = BN / 4, TY = BM / 4, NT = TX * TY, BK = kFusionBK;
   constexpr int XL = BK * BM / NT, YL = BK * BN / NT;         // elements each thread stages per chunk
   // rows padded by one double: the k-fastest stores of a k-contiguous operand fall in distinct banks
@@ -46,14 +50,14 @@ __global__ void __launch_bounds__((BM / 4) * (BN / 4))
       const int t = tid + e * NT;
       const int kk = XK ? t % BK : t / BM, ii = XK ? t / BK : t % BM;
       const int i = i0 + ii, k = k0 + kk;
-      rx[e] = (i < I && k < K) ? x[i * xi + k * xk] : 0.f;
+      rx[e] = (i < I && k < K) ? load_f32(x[i * xi + k * xk]) : 0.f;
     }
 #pragma unroll
     for (int e = 0; e < YL; ++e) {
       const int t = tid + e * NT;
       const int kk = YK ? t % BK : t / BN, jj = YK ? t / BK : t % BN;
       const int j = j0 + jj, k = k0 + kk;
-      ry[e] = (j < J && k < K) ? y[k * yk + j * yj] : 0.f;
+      ry[e] = (j < J && k < K) ? load_f32(y[k * yk + j * yj]) : 0.f;
     }
   };
   auto stage = [&](int buf) {
@@ -96,7 +100,7 @@ __global__ void __launch_bounds__((BM / 4) * (BN / 4))
     if (t + 1 < chunks) stage(buf ^ 1);
     __syncthreads();
   }
-  float* ob = out + (int64_t)b * I * J;
+  T* ob = out + (int64_t)b * I * J;
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
     const int i = i0 + ty + TY * r;
@@ -104,23 +108,23 @@ __global__ void __launch_bounds__((BM / 4) * (BN / 4))
 #pragma unroll
     for (int s = 0; s < 4; ++s) {
       const int j = j0 + tx + TX * s;
-      if (j < J) ob[(int64_t)i * J + j] = __double2float_rn(__ddiv_rn(acc[r][s], div));
+      if (j < J) ob[(int64_t)i * J + j] = store_as<T>(__double2float_rn(__ddiv_rn(acc[r][s], div)));
     }
   }
 }
 
 // out [B][I][J] contiguous; X element (b, i, k) at x + b xb + i xi + k xk, Y element (b, k, j) at y + b yb + k yk + j yj.
 // The tile size follows from the shape and never changes a result.
-template <bool XK, bool YK>
-int launch_fusion(const float* x, int64_t xb, int64_t xi, int64_t xk, const float* y, int64_t yb, int64_t yk,
-                  int64_t yj, int B, int I, int J, int K, int P, float* out, cudaStream_t stream) {
+template <bool XK, bool YK, typename T>
+int launch_fusion(const T* x, int64_t xb, int64_t xi, int64_t xk, const T* y, int64_t yb, int64_t yk, int64_t yj,
+                  int B, int I, int J, int K, int P, T* out, cudaStream_t stream) {
   const long long tiles64 = (long long)B * ((I + 63) / 64) * ((J + 63) / 64);
   if (tiles64 >= kFusionBigTiles) {
     dim3 grid((J + 63) / 64, (I + 63) / 64, B);
-    fusion_tile_kernel<64, 64, XK, YK><<<grid, 256, 0, stream>>>(x, xb, xi, xk, y, yb, yk, yj, I, J, K, (double)P, out);
+    fusion_tile_kernel<64, 64, XK, YK, T><<<grid, 256, 0, stream>>>(x, xb, xi, xk, y, yb, yk, yj, I, J, K, (double)P, out);
   } else {
     dim3 grid((J + 31) / 32, (I + 31) / 32, B);
-    fusion_tile_kernel<32, 32, XK, YK><<<grid, 64, 0, stream>>>(x, xb, xi, xk, y, yb, yk, yj, I, J, K, (double)P, out);
+    fusion_tile_kernel<32, 32, XK, YK, T><<<grid, 64, 0, stream>>>(x, xb, xi, xk, y, yb, yk, yj, I, J, K, (double)P, out);
   }
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
@@ -134,13 +138,9 @@ static int check_fusion_shape(int B, int C, int P, int M, const char* what) {
   return DIB_OK;
 }
 
-}  // namespace dib
-
-extern "C" {
-
-int attn_fusion_forward_f32(const float* img_features, const float* attention, int B, int C, int P, int M, float* out,
-                            dib_stream_t stream_) {
-  using namespace dib;
+template <typename T>
+int attn_fusion_forward(const T* img_features, const T* attention, int B, int C, int P, int M, T* out,
+                        dib_stream_t stream_) {
   const int rc = check_fusion_shape(B, C, P, M, "attn_fusion_forward");
   if (rc != DIB_OK) return rc;
   DIB_REQUIRE(img_features && attention && out, "attn_fusion_forward: NULL argument");
@@ -149,10 +149,9 @@ int attn_fusion_forward_f32(const float* img_features, const float* attention, i
                                     out, (cudaStream_t)stream_);
 }
 
-int attn_fusion_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* img_features,
-                             const float* attention, int B, int C, int P, int M, float* grad_img_features,
-                             float* grad_attention, dib_stream_t stream_) {
-  using namespace dib;
+template <typename T>
+int attn_fusion_backward(const T* grad_out, int64_t grad_batch_stride, const T* img_features, const T* attention,
+                         int B, int C, int P, int M, T* grad_img_features, T* grad_attention, dib_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   int rc = check_fusion_shape(B, C, P, M, "attn_fusion_backward");
   if (rc != DIB_OK) return rc;
@@ -174,6 +173,36 @@ int attn_fusion_backward_f32(const float* grad_out, int64_t grad_batch_stride, c
     if (rc != DIB_OK) return rc;
   }
   return DIB_OK;
+}
+
+}  // namespace dib
+
+extern "C" {
+
+int attn_fusion_forward_f32(const float* img_features, const float* attention, int B, int C, int P, int M, float* out,
+                            dib_stream_t stream) {
+  return dib::attn_fusion_forward(img_features, attention, B, C, P, M, out, stream);
+}
+
+int attn_fusion_forward_bf16(const uint16_t* img_features, const uint16_t* attention, int B, int C, int P, int M,
+                             uint16_t* out, dib_stream_t stream) {
+  using dib::as_bf16;
+  return dib::attn_fusion_forward(as_bf16(img_features), as_bf16(attention), B, C, P, M, as_bf16(out), stream);
+}
+
+int attn_fusion_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* img_features,
+                             const float* attention, int B, int C, int P, int M, float* grad_img_features,
+                             float* grad_attention, dib_stream_t stream) {
+  return dib::attn_fusion_backward(grad_out, grad_batch_stride, img_features, attention, B, C, P, M,
+                                   grad_img_features, grad_attention, stream);
+}
+
+int attn_fusion_backward_bf16(const uint16_t* grad_out, int64_t grad_batch_stride, const uint16_t* img_features,
+                              const uint16_t* attention, int B, int C, int P, int M, uint16_t* grad_img_features,
+                              uint16_t* grad_attention, dib_stream_t stream) {
+  using dib::as_bf16;
+  return dib::attn_fusion_backward(as_bf16(grad_out), grad_batch_stride, as_bf16(img_features), as_bf16(attention), B,
+                                   C, P, M, as_bf16(grad_img_features), as_bf16(grad_attention), stream);
 }
 
 }  // extern "C"

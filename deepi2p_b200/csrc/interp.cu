@@ -15,10 +15,13 @@
 //   interp_reduce_kernel    gF[b][c][m] = float(((p_0 + p_1) + ...) + p_{S-1}) over the slice partials, in slice order.
 //
 // All arithmetic is IEEE single precision without contraction (this file is compiled with --fmad=false; the
-// intrinsics below make the rounding explicit anyway).  oracle_interp restates it.
+// intrinsics below make the rounding explicit anyway).  oracle_interp restates it.  The forward and backward are
+// templated on the feature type (float, or bf16 for the *_bf16 entry points, feature_type.cuh): the features (staged
+// in shared memory as they are), the output and the gradients convert at load and store; the weights stay f32.
 #include <math.h>
 
 #include "common.cuh"
+#include "feature_type.cuh"
 
 namespace dib {
 
@@ -77,14 +80,15 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-template <int K>
+template <int K, typename T>
 __global__ void __launch_bounds__(kFwdThreads)
-    interp_forward_kernel(const float* __restrict__ features, const float* __restrict__ w,
-                          const int32_t* __restrict__ idx, int C, int Nq, int M, int cc, float* __restrict__ out) {
-  extern __shared__ __align__(16) float s_f[];         // [cc][M]
+    interp_forward_kernel(const T* __restrict__ features, const float* __restrict__ w,
+                          const int32_t* __restrict__ idx, int C, int Nq, int M, int cc, T* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char s_raw[];
+  T* s_f = reinterpret_cast<T*>(s_raw);                     // [cc][M]
   const int b = blockIdx.z, c0 = blockIdx.y * cc, tid = threadIdx.x;
   const int nc = min(cc, C - c0);
-  const float* fb = features + ((size_t)b * C + c0) * M;    // the chunk's rows are contiguous
+  const T* fb = features + ((size_t)b * C + c0) * M;        // the chunk's rows are contiguous
   for (int i = tid; i < nc * M; i += kFwdThreads) s_f[i] = fb[i];
   __syncthreads();
   const int n = blockIdx.x * kFwdThreads + tid;
@@ -94,26 +98,26 @@ __global__ void __launch_bounds__(kFwdThreads)
   int ij[K];
 #pragma unroll
   for (int j = 0; j < K; ++j) { wj[j] = w[row + j]; ij[j] = idx[row + j]; }
-  float* ob = out + ((size_t)b * C + c0) * Nq + n;
+  T* ob = out + ((size_t)b * C + c0) * Nq + n;
   if (ij[0] < 0) {                                           // an index was out of range: the whole column is NaN
-    for (int c = 0; c < nc; ++c) ob[(size_t)c * Nq] = __int_as_float(0x7fc00000);
+    for (int c = 0; c < nc; ++c) ob[(size_t)c * Nq] = store_as<T>(__int_as_float(0x7fc00000));
     return;
   }
 #pragma unroll 4
   for (int c = 0; c < nc; ++c) {
-    const float* f = s_f + c * M;
-    float acc = __fmul_rn(wj[0], f[ij[0]]);
+    const T* f = s_f + c * M;
+    float acc = __fmul_rn(wj[0], load_f32(f[ij[0]]));
 #pragma unroll
-    for (int j = 1; j < K; ++j) acc = __fadd_rn(acc, __fmul_rn(wj[j], f[ij[j]]));
-    ob[(size_t)c * Nq] = acc;
+    for (int j = 1; j < K; ++j) acc = __fadd_rn(acc, __fmul_rn(wj[j], load_f32(f[ij[j]])));
+    ob[(size_t)c * Nq] = store_as<T>(acc);
   }
 }
 
 // grid (slices * ranges, ceil(C / 32), B), 32 threads.  Partials [B][slices][C][M] f64.  The next tile's g, w and
 // idx are loaded into registers while the current one is accumulated.
-template <int K>
+template <int K, typename T>
 __global__ void __launch_bounds__(kBwdChannels)
-    interp_backward_kernel(const float* __restrict__ g, int64_t g_batch_stride, const float* __restrict__ w,
+    interp_backward_kernel(const T* __restrict__ g, int64_t g_batch_stride, const float* __restrict__ w,
                            const int32_t* __restrict__ idx, int C, int Nq, int M, int slices, int slice_len,
                            double* __restrict__ partial) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -129,7 +133,7 @@ __global__ void __launch_bounds__(kBwdChannels)
   const int nc = min(kBwdChannels, C - c0);
   for (int i = lane; i < kBwdChannels * stride; i += 32) acc[i] = 0.0;
   const int n_begin = s * slice_len, n_end = min(Nq, n_begin + slice_len);
-  const float* gb = g + (size_t)b * g_batch_stride + (size_t)c0 * Nq;
+  const T* gb = g + (size_t)b * g_batch_stride + (size_t)c0 * Nq;
   const size_t wb = (size_t)b * Nq * K;
   double* my = acc + lane * stride;
   float pg[kBwdChannels], pw[K];
@@ -137,7 +141,7 @@ __global__ void __launch_bounds__(kBwdChannels)
   auto fetch = [&](int t0) {                                  // lane = point of the tile for g, flat (point, j) for w
     const int tn = min(kBwdTile, n_end - t0);
 #pragma unroll
-    for (int c = 0; c < kBwdChannels; ++c) pg[c] = (c < nc && lane < tn) ? gb[(size_t)c * Nq + t0 + lane] : 0.f;
+    for (int c = 0; c < kBwdChannels; ++c) pg[c] = (c < nc && lane < tn) ? load_f32(gb[(size_t)c * Nq + t0 + lane]) : 0.f;
 #pragma unroll
     for (int q = 0; q < K; ++q) {
       const int i = q * 32 + lane;
@@ -193,15 +197,16 @@ __global__ void __launch_bounds__(kBwdChannels)
 }
 
 // one thread per (b, c, m)
+template <typename T>
 __global__ void interp_reduce_kernel(const double* __restrict__ partial, int C, int M, int slices, size_t total,
-                                     float* __restrict__ gF) {
+                                     T* __restrict__ gF) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const size_t cm = (size_t)C * M, b = i / cm, r = i % cm;
   const double* p = partial + b * slices * cm + r;
   double sum = p[0];
   for (int s = 1; s < slices; ++s) sum += p[(size_t)s * cm];
-  gF[i] = (float)sum;
+  gF[i] = store_as<T>((float)sum);
 }
 
 // Slices of the backward: a function of the shape alone, so a given shape always sums in the same order.
@@ -257,9 +262,13 @@ int interp_weights_f32(const void* topk_idx, int idx_bytes, const float* query, 
   return DIB_OK;
 }
 
-int interp_forward_f32(const float* features, const float* w, const int32_t* idx, int B, int C, int Nq, int M, int k,
-                       float* out, dib_stream_t stream_) {
-  using namespace dib;
+}  // extern "C"
+
+namespace dib {
+
+template <typename T>
+int interp_forward(const T* features, const float* w, const int32_t* idx, int B, int C, int Nq, int M, int k, T* out,
+                   dib_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   DIB_REQUIRE(B >= 0 && C >= 0 && Nq >= 0 && B <= 65535, "interp_forward: need 0 <= B <= 65535, C, Nq >= 0");
   DIB_REQUIRE(M >= 1 && M <= kInterpMaxNodes, "interp_forward: need 1 <= M <= 2048");
@@ -268,14 +277,15 @@ int interp_forward_f32(const float* features, const float* w, const int32_t* idx
   DIB_REQUIRE(features && w && idx && out, "interp_forward: NULL argument");
   const int cc = fwd_chunk(M);
   DIB_REQUIRE((C + cc - 1) / cc <= 65535, "interp_forward: too many channels");
-  const size_t smem = (size_t)cc * M * sizeof(float);
+  const size_t smem = (size_t)cc * M * sizeof(T);
   dim3 grid((Nq + kFwdThreads - 1) / kFwdThreads, (C + cc - 1) / cc, B);
 #define DIB_IF_LAUNCH(KK)                                                                                      \
   case KK:                                                                                                     \
     if (smem > 48 * 1024)                                                                                      \
-      DIB_CHECK_CUDA(cudaFuncSetAttribute(interp_forward_kernel<KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                          kFwdSmemFloats * (int)sizeof(float)));                               \
-    interp_forward_kernel<KK><<<grid, kFwdThreads, smem, stream>>>(features, w, idx, C, Nq, M, cc, out);       \
+      DIB_CHECK_CUDA(cudaFuncSetAttribute(interp_forward_kernel<KK, T>,                                        \
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize,                         \
+                                          kFwdSmemFloats * (int)sizeof(T)));                                   \
+    interp_forward_kernel<KK, T><<<grid, kFwdThreads, smem, stream>>>(features, w, idx, C, Nq, M, cc, out);    \
     break;
   switch (k) {
     DIB_IF_LAUNCH(1) DIB_IF_LAUNCH(2) DIB_IF_LAUNCH(3) DIB_IF_LAUNCH(4)
@@ -286,17 +296,17 @@ int interp_forward_f32(const float* features, const float* w, const int32_t* idx
   return DIB_OK;
 }
 
-size_t interp_backward_workspace_bytes(int B, int C, int Nq, int M) {
+inline size_t bwd_workspace_bytes(int B, int C, int Nq, int M) {
   if (B <= 0 || C <= 0 || Nq <= 0 || M <= 0) return 0;
   int slices, slice_len;
-  dib::bwd_slices(B, C, Nq, M, &slices, &slice_len);
+  bwd_slices(B, C, Nq, M, &slices, &slice_len);
   return (size_t)B * slices * (size_t)C * M * sizeof(double);
 }
 
-int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* w, const int32_t* idx, int B,
-                        int C, int Nq, int M, int k, float* grad_features, void* workspace, size_t workspace_bytes,
-                        dib_stream_t stream_) {
-  using namespace dib;
+template <typename T>
+int interp_backward(const T* grad_out, int64_t grad_batch_stride, const float* w, const int32_t* idx, int B, int C,
+                    int Nq, int M, int k, T* grad_features, void* workspace, size_t workspace_bytes,
+                    dib_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   DIB_REQUIRE(B >= 0 && C >= 0 && Nq >= 0 && B <= 65535, "interp_backward: need 0 <= B <= 65535, C, Nq >= 0");
   DIB_REQUIRE(M >= 1 && M <= kInterpMaxNodes, "interp_backward: need 1 <= M <= 2048");
@@ -304,13 +314,13 @@ int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const 
   if (B == 0 || C == 0) return DIB_OK;
   DIB_REQUIRE(grad_features, "interp_backward: NULL argument");
   if (Nq == 0) {
-    DIB_CHECK_CUDA(cudaMemsetAsync(grad_features, 0, (size_t)B * C * M * sizeof(float), stream));
+    DIB_CHECK_CUDA(cudaMemsetAsync(grad_features, 0, (size_t)B * C * M * sizeof(T), stream));
     return DIB_OK;
   }
   DIB_REQUIRE(grad_out && w && idx, "interp_backward: NULL argument");
   DIB_REQUIRE(grad_batch_stride >= 0, "interp_backward: grad_batch_stride < 0");
   DIB_REQUIRE((C + kBwdChannels - 1) / kBwdChannels <= 65535, "interp_backward: too many channels");
-  const size_t need = interp_backward_workspace_bytes(B, C, Nq, M);
+  const size_t need = bwd_workspace_bytes(B, C, Nq, M);
   DIB_REQUIRE(workspace && workspace_bytes >= need && ((uintptr_t)workspace & 7) == 0,
               "interp_backward: workspace too small or misaligned");
   int slices, slice_len;
@@ -321,8 +331,8 @@ int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const 
   double* partial = (double*)workspace;
 #define DIB_IB_LAUNCH(KK)                                                                                    \
   case KK:                                                                                                   \
-    interp_backward_kernel<KK><<<grid, kBwdChannels, smem, stream>>>(grad_out, grad_batch_stride, w, idx, C, Nq, M, \
-                                                                     slices, slice_len, partial);              \
+    interp_backward_kernel<KK, T><<<grid, kBwdChannels, smem, stream>>>(grad_out, grad_batch_stride, w, idx, C, Nq,  \
+                                                                        M, slices, slice_len, partial);          \
     break;
   switch (k) {
     DIB_IB_LAUNCH(1) DIB_IB_LAUNCH(2) DIB_IB_LAUNCH(3) DIB_IB_LAUNCH(4)
@@ -335,6 +345,36 @@ int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const 
                                                                              grad_features);
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
+}
+
+}  // namespace dib
+
+extern "C" {
+
+int interp_forward_f32(const float* features, const float* w, const int32_t* idx, int B, int C, int Nq, int M, int k,
+                       float* out, dib_stream_t stream) {
+  return dib::interp_forward(features, w, idx, B, C, Nq, M, k, out, stream);
+}
+
+int interp_forward_bf16(const uint16_t* features, const float* w, const int32_t* idx, int B, int C, int Nq, int M,
+                        int k, uint16_t* out, dib_stream_t stream) {
+  return dib::interp_forward(dib::as_bf16(features), w, idx, B, C, Nq, M, k, dib::as_bf16(out), stream);
+}
+
+size_t interp_backward_workspace_bytes(int B, int C, int Nq, int M) { return dib::bwd_workspace_bytes(B, C, Nq, M); }
+
+int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* w, const int32_t* idx, int B,
+                        int C, int Nq, int M, int k, float* grad_features, void* workspace, size_t workspace_bytes,
+                        dib_stream_t stream) {
+  return dib::interp_backward(grad_out, grad_batch_stride, w, idx, B, C, Nq, M, k, grad_features, workspace,
+                              workspace_bytes, stream);
+}
+
+int interp_backward_bf16(const uint16_t* grad_out, int64_t grad_batch_stride, const float* w, const int32_t* idx,
+                         int B, int C, int Nq, int M, int k, uint16_t* grad_features, void* workspace,
+                         size_t workspace_bytes, dib_stream_t stream) {
+  return dib::interp_backward(dib::as_bf16(grad_out), grad_batch_stride, w, idx, B, C, Nq, M, k,
+                              dib::as_bf16(grad_features), workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -13,6 +13,7 @@
 // Here a warp owns a row: coalesced loads, ballot + popc ordered compaction, early exit once K
 // hits are found, then the reference's padding rule (none -> 0, fewer -> cyclic repeat).
 #include "common.cuh"
+#include "feature_type.cuh"
 
 namespace dib {
 
@@ -39,9 +40,25 @@ __device__ __forceinline__ void im_consider(float* bestf, unsigned long long* be
   }
 }
 
-// grid = (ceil(C / CPB), B); dynamic smem = CPB * K * 12 bytes
-template <int CPB, bool VEC>
-__global__ void __launch_bounds__(kImThreads) index_max_kernel(const float* __restrict__ data,
+// Four consecutive elements of a row as floats: one 128-bit load of float, one 64-bit load of bf16 (widened exactly).
+__device__ __forceinline__ float4 ldg4(const float* row, int i) { return __ldg(reinterpret_cast<const float4*>(row) + i); }
+__device__ __forceinline__ float4 ldcs4(const float* row, int i) {
+  return __ldcs(reinterpret_cast<const float4*>(row) + i);
+}
+__device__ __forceinline__ float4 widen4(uint2 u) {
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xFFFF0000u));
+}
+__device__ __forceinline__ float4 ldg4(const bf16* row, int i) {
+  return widen4(__ldg(reinterpret_cast<const uint2*>(row) + i));
+}
+__device__ __forceinline__ float4 ldcs4(const bf16* row, int i) {
+  return widen4(__ldcs(reinterpret_cast<const uint2*>(row) + i));
+}
+
+// grid = (ceil(C / CPB), B); dynamic smem = CPB * K * 12 bytes.  T = float or bf16: the values are compared as floats.
+template <int CPB, bool VEC, typename T>
+__global__ void __launch_bounds__(kImThreads) index_max_kernel(const T* __restrict__ data,
                                                                const int32_t* __restrict__ index,
                                                                int32_t* __restrict__ out, int B, int C, int N, int K) {
   extern __shared__ __align__(16) unsigned char im_smem[];
@@ -53,7 +70,7 @@ __global__ void __launch_bounds__(kImThreads) index_max_kernel(const float* __re
   for (int i = threadIdx.x; i < CPB * K; i += kImThreads) { bestk[i] = 0ull; bestv[i] = -1000.0f; }
   __syncthreads();
   const int32_t* idx = index + (size_t)b * N;
-  const float* rows = data + ((size_t)b * C + c0) * N;
+  const T* rows = data + ((size_t)b * C + c0) * N;
 
   if (VEC) {
     const int n4 = N >> 2;
@@ -70,7 +87,7 @@ __global__ void __launch_bounds__(kImThreads) index_max_kernel(const float* __re
 #pragma unroll
         for (int c = 0; c < CPB; ++c) {
           if (c < nc) {
-            const float4 v = __ldg(reinterpret_cast<const float4*>(rows + (size_t)c * N) + i);
+            const float4 v = ldg4(rows + (size_t)c * N, i);
             const float v4[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
@@ -92,7 +109,7 @@ __global__ void __launch_bounds__(kImThreads) index_max_kernel(const float* __re
       kk = __ldg(reinterpret_cast<const int4*>(idx) + i);
 #pragma unroll
       for (int c = 0; c < CPB; ++c)
-        if (c < nc) vv[c] = __ldcs(reinterpret_cast<const float4*>(rows + (size_t)c * N) + i);
+        if (c < nc) vv[c] = ldcs4(rows + (size_t)c * N, i);
     }
     while (i < n4) {
       const int inext = i + kImThreads;
@@ -102,7 +119,7 @@ __global__ void __launch_bounds__(kImThreads) index_max_kernel(const float* __re
         kn = __ldg(reinterpret_cast<const int4*>(idx) + inext);
 #pragma unroll
         for (int c = 0; c < CPB; ++c)
-          if (c < nc) vn[c] = __ldcs(reinterpret_cast<const float4*>(rows + (size_t)c * N) + inext);
+          if (c < nc) vn[c] = ldcs4(rows + (size_t)c * N, inext);
       }
       const uint32_t n = (uint32_t)i << 2;
 #pragma unroll
@@ -125,7 +142,7 @@ __global__ void __launch_bounds__(kImThreads) index_max_kernel(const float* __re
       if ((unsigned)k >= (unsigned)K) continue;
 #pragma unroll
       for (int c = 0; c < CPB; ++c)
-        if (c < nc) im_consider<CPB>(bestv, bestk, K, c, k, __ldcs(rows + (size_t)c * N + i), (uint32_t)i);
+        if (c < nc) im_consider<CPB>(bestv, bestk, K, c, k, load_f32(__ldcs(rows + (size_t)c * N + i)), (uint32_t)i);
     }
   }
   __syncthreads();
@@ -288,19 +305,16 @@ __global__ void __launch_bounds__(kBqSplit * 32) ball_query_split_kernel(const f
   }
 }
 
-}  // namespace dib
-
-extern "C" {
-
-int index_max_forward(const float* data, const int32_t* index, int32_t* out, int B, int C, int N, int K,
-                      dib_stream_t stream) {
-  using namespace dib;
+// index_max_forward's launch for float or bf16 data (cluster_pool_forward_* launch it too)
+template <typename T>
+int index_max_launch(const T* data, const int32_t* index, int32_t* out, int B, int C, int N, int K,
+                     dib_stream_t stream) {
   DIB_REQUIRE(data && index && out, "NULL argument");
   DIB_REQUIRE(B >= 0 && C >= 0 && N >= 0 && K >= 1, "bad shape B=%d C=%d N=%d K=%d", B, C, N, K);
   DIB_REQUIRE(B <= 65535, "B too large for grid.y");
   if (B == 0 || C == 0) return DIB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const bool vec = (N % 4 == 0) && ((uintptr_t)data % 16 == 0) && ((uintptr_t)index % 16 == 0);
+  const bool vec = (N % 4 == 0) && ((uintptr_t)data % (4 * sizeof(T)) == 0) && ((uintptr_t)index % 16 == 0);
   const size_t per_c = (size_t)K * 12;
   const size_t limit = 227 * 1024;
   int cpb = 4;
@@ -310,9 +324,9 @@ int index_max_forward(const float* data, const int32_t* index, int32_t* out, int
   dim3 grid((C + cpb - 1) / cpb, B);
 #define DIB_IM_LAUNCH(CPB, VEC)                                                                              \
   do {                                                                                                       \
-    auto kern = dib::index_max_kernel<CPB, VEC>;                                                             \
+    auto kern = index_max_kernel<CPB, VEC, T>;                                                               \
     DIB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      \
-    kern<<<grid, dib::kImThreads, smem, st>>>(data, index, out, B, C, N, K);                                 \
+    kern<<<grid, kImThreads, smem, st>>>(data, index, out, B, C, N, K);                                      \
   } while (0)
   if (cpb == 4) { if (vec) DIB_IM_LAUNCH(4, true); else DIB_IM_LAUNCH(4, false); }
   else if (cpb == 2) { if (vec) DIB_IM_LAUNCH(2, true); else DIB_IM_LAUNCH(2, false); }
@@ -320,6 +334,17 @@ int index_max_forward(const float* data, const int32_t* index, int32_t* out, int
 #undef DIB_IM_LAUNCH
   DIB_CHECK_CUDA(cudaGetLastError());
   return DIB_OK;
+}
+template int index_max_launch<float>(const float*, const int32_t*, int32_t*, int, int, int, int, dib_stream_t);
+template int index_max_launch<bf16>(const bf16*, const int32_t*, int32_t*, int, int, int, int, dib_stream_t);
+
+}  // namespace dib
+
+extern "C" {
+
+int index_max_forward(const float* data, const int32_t* index, int32_t* out, int B, int C, int N, int K,
+                      dib_stream_t stream) {
+  return dib::index_max_launch(data, index, out, B, C, N, K, stream);
 }
 
 int ball_query_forward(const float* dist, float radius, int32_t* out, int B, int M, int N, int K,

@@ -207,7 +207,9 @@ class KeypointDetector(nn.Module):
 
     The stride-32 map must have H_f x W_f = round(H / fine_scale) x round(W / fine_scale) pixels and the stride-16 map
     four times as many, because the attention PointNets give one weight per pixel; the shipped sizes do.  Only
-    normalization='batch' and activation='relu' are supported.  resnet_weights: optional path of a torchvision-layout
+    normalization='batch' and activation='relu' are supported.  With point_layers="torch" the forward and its backward
+    also run under torch.autocast("cuda", dtype=torch.bfloat16): the project's ops then take and return bfloat16
+    features (DESIGN.md 4.37); the fused modes and float16 autocast raise ValueError.  resnet_weights: optional path of a torchvision-layout
     ResNet-34 state_dict (e.g. resnet34-333f7ec4.pth) for the image backbone; without it the backbone starts from the
     reference's initialisation.  Construction runs on the CPU and reads nothing but that file."""
 
@@ -320,6 +322,8 @@ class KeypointDetector(nn.Module):
         return scores[:, 0:2, :]
 
     def forward(self, pc, intensity, sn, node_a, node_b, img):
+        if torch.is_autocast_enabled("cuda"):
+            check_autocast(self.point_layers)
         if self.point_layers == "fused_all" and not self.training:
             return self._fused_all_eval(pc, intensity, sn, node_a, node_b, img)
         B, Ma, Mb = pc.shape[0], node_a.shape[2], node_b.shape[2]
@@ -402,6 +406,18 @@ class KeypointDetector(nn.Module):
         if self.fine:
             return scores[:, 0:2, :], scores[:, 2:, :]
         return scores[:, 0:2, :]
+
+
+def check_autocast(point_layers):
+    """The forward's rule under torch.autocast (DESIGN.md 4.37): bfloat16 autocast with point_layers="torch" only.  The
+    fused modes keep their TF32 contract and take float32 only; float16 autocast is not supported.  ValueError
+    otherwise, before any kernel runs."""
+    dtype = torch.get_autocast_dtype("cuda")
+    if dtype != torch.bfloat16:
+        raise ValueError(f"KeypointDetector supports torch.autocast with dtype torch.bfloat16 only, got {dtype}")
+    if point_layers != "torch":
+        raise ValueError(f"KeypointDetector(point_layers={point_layers!r}) runs float32 TF32 kernels: under "
+                         f"torch.autocast use point_layers='torch'")
 
 
 def load_checkpoint(model, path_or_dict):

@@ -9,7 +9,7 @@ stream (SURVEY.md 8b).
 import torch
 
 from . import _native
-from ._native import _stream_ptr, _workspace
+from ._native import _stream_ptr, _workspace, feature_dtype
 
 
 def _check_input(t, name, dtype):
@@ -141,9 +141,10 @@ def _check_interp_args(topk_idx, query, node, features):
             raise RuntimeError(f"{name} must have 3 dimensions")
     if topk_idx.dtype not in (torch.int32, torch.int64):
         raise RuntimeError("topk_idx must have dtype torch.int32 or torch.int64")
-    for t, name in ((query, "query"), (node, "node"), (features, "features")):
+    for t, name in ((query, "query"), (node, "node")):
         if t.dtype != torch.float32:
             raise RuntimeError(f"{name} must have dtype {torch.float32}")
+    feature_dtype(((features, "features"),))
     B, Nq, k = topk_idx.shape
     M = node.shape[2]
     if (query.shape[0] != B or query.shape[1] != 3 or query.shape[2] != Nq or node.shape[0] != B or node.shape[1] != 3
@@ -171,20 +172,22 @@ class _Interpolation(torch.autograd.Function):
         B, Nq, k = topk_idx.shape
         C, M = features.shape[1], features.shape[2]
         dev = features.device
+        dtype, sfx = feature_dtype(((features, "features"),))
         with torch.cuda.device(dev):
             w = torch.empty((B, Nq, k), dtype=torch.float32, device=dev)
             idx = torch.empty((B, Nq, k), dtype=torch.int32, device=dev)
-            out = torch.empty((B, C, Nq), dtype=torch.float32, device=dev)
+            out = torch.empty((B, C, Nq), dtype=dtype, device=dev)
             if out.numel():
                 stream = _stream_ptr()
                 rc = lib.interp_weights_f32(topk_idx.data_ptr(), topk_idx.element_size(), query.data_ptr(),
                                             node.data_ptr(), B, Nq, M, k, w.data_ptr(), idx.data_ptr(), stream)
                 _native.check(rc, "interp_weights_f32")
-                rc = lib.interp_forward_f32(features.data_ptr(), w.data_ptr(), idx.data_ptr(), B, C, Nq, M, k,
-                                            out.data_ptr(), stream)
-                _native.check(rc, "interp_forward_f32")
+                rc = getattr(lib, f"interp_forward_{sfx}")(features.data_ptr(), w.data_ptr(), idx.data_ptr(), B, C,
+                                                           Nq, M, k, out.data_ptr(), stream)
+                _native.check(rc, f"interp_forward_{sfx}")
         ctx.save_for_backward(w, idx)
         ctx.shape = (B, C, Nq, M, k)
+        ctx.dtype = (dtype, sfx)
         return out
 
     @staticmethod
@@ -193,22 +196,24 @@ class _Interpolation(torch.autograd.Function):
             return None, None, None, None
         w, idx = ctx.saved_tensors
         B, C, Nq, M, k = ctx.shape
+        dtype, sfx = ctx.dtype
         dev = w.device
         # the kernel takes any batch stride with (channel, point) strides (Nq, 1): a channel slice of a torch.cat
         # gradient needs no copy
-        grad_out = grad_out.float()
+        grad_out = grad_out.to(dtype)
         if (C > 1 and grad_out.stride(1) != Nq) or (Nq > 1 and grad_out.stride(2) != 1):
             grad_out = grad_out.contiguous()
         lib = _native.load()
         with torch.cuda.device(dev):
-            gF = torch.empty((B, C, M), dtype=torch.float32, device=dev)
+            gF = torch.empty((B, C, M), dtype=dtype, device=dev)
             if gF.numel():
                 stream = _stream_ptr()
                 ws = _backward_workspace(dev, lib.interp_backward_workspace_bytes(B, C, Nq, M))
                 bstride = grad_out.stride(0) if B > 1 else 0
-                rc = lib.interp_backward_f32(grad_out.data_ptr(), bstride, w.data_ptr(), idx.data_ptr(), B, C, Nq, M,
-                                             k, gF.data_ptr(), ws.data_ptr(), ws.numel(), stream)
-                _native.check(rc, "interp_backward_f32")
+                rc = getattr(lib, f"interp_backward_{sfx}")(grad_out.data_ptr(), bstride, w.data_ptr(), idx.data_ptr(),
+                                                            B, C, Nq, M, k, gF.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                            stream)
+                _native.check(rc, f"interp_backward_{sfx}")
         return None, None, None, gF
 
 
@@ -217,12 +222,14 @@ def upsample_by_interpolation(topk_idx, query, node, features):
     (models/networks_united.py:90-103, the same argument order without `self`) without its B x C x Nq x k tensors.
 
     topk_idx [B,Nq,k] int32 / int64 (e.g. cluster_assign_forward(...)["min_k_idx"] or a torch.topk result), query
-    [B,3,Nq], node [B,3,M], features [B,C,M] float32 CUDA; 1 <= k <= 8, 1 <= M <= 2048.  Returns out [B,C,Nq] with
+    [B,3,Nq], node [B,3,M] float32 and features [B,C,M] float32 or bfloat16 CUDA; 1 <= k <= 8, 1 <= M <= 2048.
+    Returns out [B,C,Nq] of the features' dtype with
     out[b,c,n] = sum_j w_j features[b,c,idx_j], d_j = |query_n - node_{idx_j}|, w_j = 1 - d_j / sum_j d_j (DESIGN.md
     4.12).  As in the reference the weights sum to k - 1, k = 1 gives weight 0 and a zero distance sum gives NaN; a
     query point with any index outside [0, M) gets NaN in all C channels and no share of the feature gradient.
     Differentiable with respect to `features` only, with a deterministic gradient; query and node must not require
-    grad."""
+    grad.  bfloat16 features give the float32 result on the widened features, rounded to bfloat16, and the same rule
+    for the gradient (DESIGN.md 4.37)."""
     _check_interp_args(topk_idx, query, node, features)
     return _Interpolation.apply(topk_idx, query, node, features)
 
@@ -246,8 +253,7 @@ def _check_pool_args(features, min_idx, M):
     for t, name in ((features, "features"), (min_idx, "min_idx")):
         if not isinstance(t, torch.Tensor):
             raise TypeError(f"{name} must be a torch.Tensor")
-    if features.dtype != torch.float32:
-        raise RuntimeError(f"features must have dtype {torch.float32}")
+    feature_dtype(((features, "features"),))
     if min_idx.dtype != torch.int32:
         raise RuntimeError(f"min_idx must have dtype {torch.int32}")
     if features.dim() != 3 or min_idx.dim() != 2 or min_idx.shape[0] != features.shape[0] \
@@ -266,20 +272,22 @@ class _ClusterMaxPool(torch.autograd.Function):
         lib = _native.load()
         B, C, N = features.shape
         dev = features.device
+        dtype, sfx = feature_dtype(((features, "features"),))
         with torch.cuda.device(dev):
             sel = torch.empty((B, C, M), dtype=torch.int32, device=dev)
             mask = torch.empty((B, M), dtype=torch.float32, device=dev)
-            pooled = torch.empty((B, C, M), dtype=torch.float32, device=dev)
-            scattered = torch.empty((B, C, N), dtype=torch.float32, device=dev) if broadcast else None
+            pooled = torch.empty((B, C, M), dtype=dtype, device=dev)
+            scattered = torch.empty((B, C, N), dtype=dtype, device=dev) if broadcast else None
             if B:
-                rc = lib.cluster_pool_forward_f32(features.data_ptr(), min_idx.data_ptr(), B, C, N, M, sel.data_ptr(),
-                                                  mask.data_ptr(), pooled.data_ptr(),
-                                                  scattered.data_ptr() if broadcast and scattered.numel() else None,
-                                                  _stream_ptr())
-                _native.check(rc, "cluster_pool_forward_f32")
+                rc = getattr(lib, f"cluster_pool_forward_{sfx}")(
+                    features.data_ptr(), min_idx.data_ptr(), B, C, N, M, sel.data_ptr(), mask.data_ptr(),
+                    pooled.data_ptr(), scattered.data_ptr() if broadcast and scattered.numel() else None,
+                    _stream_ptr())
+                _native.check(rc, f"cluster_pool_forward_{sfx}")
         ctx.set_materialize_grads(False)           # a missing pooled or scattered gradient stays None
         ctx.save_for_backward(min_idx, sel, mask)
         ctx.shape = (B, C, N, M)
+        ctx.dtype = (dtype, sfx)
         return (pooled, scattered) if broadcast else pooled
 
     @staticmethod
@@ -288,18 +296,19 @@ class _ClusterMaxPool(torch.autograd.Function):
             return None, None, None, None
         min_idx, sel, mask = ctx.saved_tensors
         B, C, N, M = ctx.shape
+        dtype, sfx = ctx.dtype
         dev = sel.device
         if grad_pooled is not None:
-            grad_pooled = grad_pooled.float().contiguous()
+            grad_pooled = grad_pooled.to(dtype).contiguous()
         if grad_scattered is not None:
             # any batch stride with (channel, point) strides (N, 1): a channel slice of a torch.cat gradient needs
             # no copy
-            grad_scattered = grad_scattered.float()
+            grad_scattered = grad_scattered.to(dtype)
             if (C > 1 and grad_scattered.stride(1) != N) or (N > 1 and grad_scattered.stride(2) != 1):
                 grad_scattered = grad_scattered.contiguous()
         lib = _native.load()
         with torch.cuda.device(dev):
-            gF = torch.empty((B, C, N), dtype=torch.float32, device=dev)
+            gF = torch.empty((B, C, N), dtype=dtype, device=dev)
             if gF.numel():
                 stream = _stream_ptr()
                 ws, ws_bytes = None, 0
@@ -308,11 +317,11 @@ class _ClusterMaxPool(torch.autograd.Function):
                     ws_bytes = ws.numel()
                 gs_ptr = grad_scattered.data_ptr() if grad_scattered is not None else None
                 bstride = grad_scattered.stride(0) if grad_scattered is not None and B > 1 else 0
-                rc = lib.cluster_pool_backward_f32(grad_pooled.data_ptr() if grad_pooled is not None else None, gs_ptr,
-                                                   bstride, min_idx.data_ptr(), sel.data_ptr(), mask.data_ptr(), B, C,
-                                                   N, M, gF.data_ptr(), ws.data_ptr() if ws is not None else None,
-                                                   ws_bytes, stream)
-                _native.check(rc, "cluster_pool_backward_f32")
+                rc = getattr(lib, f"cluster_pool_backward_{sfx}")(
+                    grad_pooled.data_ptr() if grad_pooled is not None else None, gs_ptr, bstride, min_idx.data_ptr(),
+                    sel.data_ptr(), mask.data_ptr(), B, C, N, M, gF.data_ptr(),
+                    ws.data_ptr() if ws is not None else None, ws_bytes, stream)
+                _native.check(rc, f"cluster_pool_backward_{sfx}")
         return gF, None, None, None
 
 
@@ -320,12 +329,14 @@ def cluster_max_pool(features, min_idx, M, broadcast=False):
     """SO-Net masked max-pool of PCEncoder.forward (models/networks_pc.py:88-104) in one op, with a deterministic
     feature gradient (DESIGN.md 4.16).
 
-    features [B,C,N] float32 and min_idx [B,N] int32 (cluster_assign_forward's) CUDA, M >= 1 segments.  Returns pooled
-    [B,C,M] = features[b,c,sel] * mask[b,m], sel = index_max_forward(features, min_idx, M) and mask[b,m] = 1.0 where
+    features [B,C,N] float32 or bfloat16 and min_idx [B,N] int32 (cluster_assign_forward's) CUDA, M >= 1 segments.
+    Returns pooled [B,C,M] (of the features' dtype, as scattered) = features[b,c,sel] * mask[b,m], sel = index_max_forward(features, min_idx, M) and mask[b,m] = 1.0 where
     some point has min_idx == m (else 0.0: an empty segment gives features[b,c,0] * 0.0, -0.0 or NaN included).  With
     broadcast=True returns (pooled, scattered), scattered [B,C,N] = pooled[b,c,min_idx[b,n]].  A point whose min_idx
     is outside [0, M) joins no segment, gets NaN in every channel of scattered and no share of the gradient.
-    Differentiable with respect to `features`: fp64 sums in an order fixed by the shape, no float atomics."""
+    Differentiable with respect to `features`: fp64 sums in an order fixed by the shape, no float atomics.  bfloat16
+    features give the float32 results on the widened features, rounded to bfloat16, and the same rule for the gradient
+    (DESIGN.md 4.37)."""
     _check_pool_args(features, min_idx, M)
     return _ClusterMaxPool.apply(features, min_idx, int(M), bool(broadcast))
 
@@ -335,7 +346,9 @@ def _check_knn_args(query, database, features, K):
     for t, name in ((query, "query"), (database, "database"), (features, "features")):
         if not isinstance(t, torch.Tensor):
             raise TypeError(f"{name} must be a torch.Tensor")
-        if t.dtype != torch.float32:
+        if t is features:
+            feature_dtype(((features, "features"),))
+        elif t.dtype != torch.float32:
             raise RuntimeError(f"{name} must have dtype {torch.float32}")
         if t.dim() != 3:
             raise RuntimeError(f"{name} must have 3 dimensions")
@@ -361,17 +374,20 @@ class _KnnGroup(torch.autograd.Function):
         B, C, N = features.shape
         M = query.shape[2]
         dev = features.device
+        dtype, sfx = feature_dtype(((features, "features"),))
         with torch.cuda.device(dev):
             idx = torch.empty((B, M, K), dtype=torch.int32, device=dev)
-            grouped = torch.empty((B, 3 + C, M, K), dtype=torch.float32, device=dev)
+            grouped = torch.empty((B, 3 + C, M, K), dtype=dtype, device=dev)
             if idx.numel():
-                rc = lib.knn_group_forward_f32(query.data_ptr(), database.data_ptr(), features.data_ptr(), B, C, M, N,
-                                               K, idx.data_ptr(), grouped.data_ptr(), _stream_ptr())
-                _native.check(rc, "knn_group_forward_f32")
+                rc = getattr(lib, f"knn_group_forward_{sfx}")(query.data_ptr(), database.data_ptr(),
+                                                              features.data_ptr(), B, C, M, N, K, idx.data_ptr(),
+                                                              grouped.data_ptr(), _stream_ptr())
+                _native.check(rc, f"knn_group_forward_{sfx}")
         ctx.mark_non_differentiable(idx)
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(idx)
         ctx.shape = (B, C, M, N, K)
+        ctx.dtype = (dtype, sfx)
         return idx, grouped
 
     @staticmethod
@@ -380,25 +396,27 @@ class _KnnGroup(torch.autograd.Function):
             return None, None, None, None
         idx, = ctx.saved_tensors
         B, C, M, N, K = ctx.shape
+        dtype, sfx = ctx.dtype
         dev = idx.device
         if grad_grouped is None:                   # grouped took no part in the loss: a zero gradient, not materialised
             return None, None, None, None
         # any batch stride with (row, query, neighbour) strides (M * K, K, 1).  There are always 3 + C >= 3 rows, so the
         # row stride is checked whatever M and K are (at M = K = 1 a slice of a cat along dim 3 has row stride != 1)
-        grad_grouped = grad_grouped.float()
+        grad_grouped = grad_grouped.to(dtype)
         if grad_grouped.stride(1) != M * K or (M > 1 and grad_grouped.stride(2) != K) \
                 or (K > 1 and grad_grouped.stride(3) != 1):
             grad_grouped = grad_grouped.contiguous()
         lib = _native.load()
         with torch.cuda.device(dev):
-            gF = torch.empty((B, C, N), dtype=torch.float32, device=dev)
+            gF = torch.empty((B, C, N), dtype=dtype, device=dev)
             if gF.numel():
                 stream = _stream_ptr()
                 ws = _backward_workspace(dev, lib.knn_group_backward_workspace_bytes(B, C, M, N, K))
                 bstride = grad_grouped.stride(0) if B > 1 else 0
-                rc = lib.knn_group_backward_f32(grad_grouped.data_ptr() if M else None, bstride, idx.data_ptr(), B, C,
-                                                M, N, K, gF.data_ptr(), ws.data_ptr(), ws.numel(), stream)
-                _native.check(rc, "knn_group_backward_f32")
+                rc = getattr(lib, f"knn_group_backward_{sfx}")(grad_grouped.data_ptr() if M else None, bstride,
+                                                               idx.data_ptr(), B, C, M, N, K, gF.data_ptr(),
+                                                               ws.data_ptr(), ws.numel(), stream)
+                _native.check(rc, f"knn_group_backward_{sfx}")
         return None, None, gF, None
 
 
@@ -406,12 +424,14 @@ def knn_group(query, database, features, K):
     """Node kNN grouping of GeneralKNNFusionModule.forward (models/layers_pc.py:793-807) in one op, with a
     deterministic feature gradient (DESIGN.md 4.16).
 
-    query [B,3,M], database [B,3,N], features [B,C,N] float32 CUDA; 1 <= K <= 32, K <= N <= 2048.  Returns (knn_idx
-    [B,M,K] int32, grouped [B,3+C,M,K]): knn_idx holds the K nearest database nodes of each query, nearest first, by
+    query [B,3,M], database [B,3,N] float32 and features [B,C,N] float32 or bfloat16 CUDA; 1 <= K <= 32, K <= N <=
+    2048.  Returns (knn_idx [B,M,K] int32, grouped [B,3+C,M,K] of the features' dtype): knn_idx holds the K nearest database nodes of each query, nearest first, by
     cluster_assign's key (f32 ((dx*dx + dy*dy) + dz*dz) without fma, ties -> lower index, +inf after finite keys, NaN
     after +inf); grouped rows 0-2 are database[idx] - query and rows 3 onward features[idx], the tensor
     layers_pc.py:807 concatenates.  Differentiable with respect to `features` only (fp64 sums in an order fixed by the
-    shape, no float atomics); query and database must not require grad, as the reference detaches both."""
+    shape, no float atomics); query and database must not require grad, as the reference detaches both.  bfloat16
+    features give the float32 result on the widened features rounded to bfloat16 (the coordinate rows too), and the
+    same rule for the gradient (DESIGN.md 4.37)."""
     _check_knn_args(query, database, features, K)
     return _KnnGroup.apply(query, database, features, int(K))
 
@@ -427,8 +447,7 @@ def _check_fusion_args(img_features, attention):
             raise TypeError(f"{name} must be a torch.Tensor")
         if t.dim() != 3:
             raise RuntimeError(f"{name} must have 3 dimensions")
-        if t.dtype != torch.float32:
-            raise RuntimeError(f"{name} must have dtype {torch.float32}")
+    feature_dtype(((img_features, "img_features"), (attention, "attention")))
     B, C, P = img_features.shape
     M = attention.shape[2]
     if attention.shape[0] != B or attention.shape[1] != P:
@@ -449,13 +468,15 @@ class _AttentionFusion(torch.autograd.Function):
         B, C, P = img_features.shape
         M = attention.shape[2]
         dev = img_features.device
+        dtype, sfx = feature_dtype(((img_features, "img_features"), (attention, "attention")))
         with torch.cuda.device(dev):
-            out = torch.empty((B, C, M), dtype=torch.float32, device=dev)
-            rc = lib.attn_fusion_forward_f32(img_features.data_ptr(), attention.data_ptr(), B, C, P, M, out.data_ptr(),
-                                             _stream_ptr())
-        _native.check(rc, "attn_fusion_forward_f32")
+            out = torch.empty((B, C, M), dtype=dtype, device=dev)
+            rc = getattr(lib, f"attn_fusion_forward_{sfx}")(img_features.data_ptr(), attention.data_ptr(), B, C, P, M,
+                                                            out.data_ptr(), _stream_ptr())
+        _native.check(rc, f"attn_fusion_forward_{sfx}")
         ctx.set_materialize_grads(False)           # a missing output gradient stays None
         ctx.save_for_backward(img_features, attention)
+        ctx.dtype = (dtype, sfx)
         return out
 
     @staticmethod
@@ -466,20 +487,21 @@ class _AttentionFusion(torch.autograd.Function):
         F, A = ctx.saved_tensors
         B, C, P = F.shape
         M = A.shape[2]
+        dtype, sfx = ctx.dtype
         dev = F.device
         # any batch stride with (channel, node) strides (M, 1): a channel slice of a torch.cat gradient needs no copy
-        grad_out = grad_out.float()
+        grad_out = grad_out.to(dtype)
         if (C > 1 and grad_out.stride(1) != M) or (M > 1 and grad_out.stride(2) != 1):
             grad_out = grad_out.contiguous()
         lib = _native.load()
         with torch.cuda.device(dev):
-            gF = torch.empty((B, C, P), dtype=torch.float32, device=dev) if need_F else None
-            gA = torch.empty((B, P, M), dtype=torch.float32, device=dev) if need_A else None
+            gF = torch.empty((B, C, P), dtype=dtype, device=dev) if need_F else None
+            gA = torch.empty((B, P, M), dtype=dtype, device=dev) if need_A else None
             bstride = grad_out.stride(0) if B > 1 else 0
-            rc = lib.attn_fusion_backward_f32(grad_out.data_ptr(), bstride, F.data_ptr(), A.data_ptr(), B, C, P, M,
-                                              gF.data_ptr() if need_F else None, gA.data_ptr() if need_A else None,
-                                              _stream_ptr())
-        _native.check(rc, "attn_fusion_backward_f32")
+            rc = getattr(lib, f"attn_fusion_backward_{sfx}")(grad_out.data_ptr(), bstride, F.data_ptr(), A.data_ptr(),
+                                                             B, C, P, M, gF.data_ptr() if need_F else None,
+                                                             gA.data_ptr() if need_A else None, _stream_ptr())
+        _native.check(rc, f"attn_fusion_backward_{sfx}")
         return gF, gA
 
 
@@ -488,11 +510,12 @@ def attention_fusion(img_features, attention):
     torch.mean(img_features.unsqueeze(3) * attention.unsqueeze(1), dim=2)) without its B x C x P x M product
     (DESIGN.md 4.17).
 
-    img_features [B,C,P] (the feature map's .view(B, C, -1)) and attention [B,P,M] float32 CUDA, contiguous, on one
-    device.  Returns out [B,C,M], out[b,c,m] = float((sum over p ascending of F[b,c,p] * A[b,p,m]) / P), one fp64
+    img_features [B,C,P] (the feature map's .view(B, C, -1)) and attention [B,P,M] CUDA, contiguous, on one device,
+    both float32 or both bfloat16.  Returns out [B,C,M] of their dtype, out[b,c,m] = float((sum over p ascending of F[b,c,p] * A[b,p,m]) / P), one fp64
     accumulator per output over the exact products, so the result does not depend on tiling, batch composition or the
     TF32 flags.  Differentiable with respect to both inputs with the same rule (sums over m for img_features, over c
-    for attention); an input that needs no gradient costs nothing in the backward."""
+    for attention); an input that needs no gradient costs nothing in the backward.  bfloat16 inputs give the float32
+    result on the widened inputs, rounded to bfloat16, and the same rule for the gradients (DESIGN.md 4.37)."""
     _check_fusion_args(img_features, attention)
     return _AttentionFusion.apply(img_features, attention)
 

@@ -15,6 +15,7 @@ rule; then the epoch's checkpoint and the resume file.  While step k runs, batch
 so the assembly's host reads wait on that stream only.  Losses and accuracies are summed on the device and read at
 the print interval and at the end of the epoch: the loop itself never synchronises with the device.
 """
+import contextlib
 import os
 import time
 
@@ -41,6 +42,9 @@ INPUT_FIELDS = ("pc", "intensity", "sn", "node_a", "node_b", "P", "img", "K")
 LOSS_KEYS = ("loss", "coarse", "fine")
 ACCURACY_KEYS = ("coarse_accuracy", "fine_accuracy")
 WARMUP_STEPS = 3            # eager steps before the capture: Adam's state and every lazy initialisation exist by then
+# Trainer(precision=...): "fp32" is the reference's float32 step; "bf16" runs the forward and the loss under bfloat16
+# autocast (DESIGN.md 4.37)
+PRECISIONS = ("fp32", "bf16")
 
 
 def coarse_loss_alpha(fine):
@@ -162,14 +166,32 @@ def make_optimizer(model, lr=LR):
                             betas=BETAS, weight_decay=WEIGHT_DECAY, capturable=True)
 
 
-def train_step(model, optimizer, inputs):
+def autocast(precision):
+    """The context the forward and the loss run in: nothing for "fp32"; for "bf16" torch.autocast("cuda",
+    dtype=torch.bfloat16) with the weight-cast cache off, so that a captured step casts the weights it reads at replay
+    time.  No GradScaler is needed: bfloat16 has float32's exponent range."""
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
+    if precision == "fp32":
+        return contextlib.nullcontext()
+    return torch.autocast("cuda", dtype=torch.bfloat16, cache_enabled=False)
+
+
+def _forward_loss(model, inputs, precision):
+    with autocast(precision):
+        scores = model(*(inputs[k] for k in ("pc", "intensity", "sn", "node_a", "node_b", "img")))
+        coarse, fine = scores if model.fine else (scores, None)
+        return classifier.classifier_loss(coarse, fine, inputs["pc"], inputs["P"], inputs["K"], model.img_H,
+                                          model.img_W, model.fine_scale, coarse_loss_alpha=coarse_loss_alpha(model.fine))
+
+
+def train_step(model, optimizer, inputs, precision="fp32"):
     """MMClassifer.optimize on one batch (INTEGRATION.md 4d): train mode, forward, classifier_loss, zero_grad,
-    backward, optimizer step.  inputs: INPUT_FIELDS -> device tensors.  Returns classifier_loss's dict."""
+    backward, optimizer step.  inputs: INPUT_FIELDS -> device tensors.  precision "bf16" runs the forward and the loss
+    under autocast(precision); the backward and Adam run outside it, on the float32 parameters.  Returns
+    classifier_loss's dict."""
     model.train()
-    scores = model(*(inputs[k] for k in ("pc", "intensity", "sn", "node_a", "node_b", "img")))
-    coarse, fine = scores if model.fine else (scores, None)
-    out = classifier.classifier_loss(coarse, fine, inputs["pc"], inputs["P"], inputs["K"], model.img_H, model.img_W,
-                                     model.fine_scale, coarse_loss_alpha=coarse_loss_alpha(model.fine))
+    out = _forward_loss(model, inputs, precision)
     optimizer.zero_grad(set_to_none=True)
     out["loss"].backward()
     optimizer.step()
@@ -191,12 +213,20 @@ class Trainer:
     eager steps (forward, loss, backward, Adam, BatchNorm statistics and dropout with torch's graph-safe RNG) and
     replayed from one static input set; the assembled batch goes through a staging buffer filled on a side stream
     while the previous step runs.  Checkpoints and the resume file go to out_dir.  gpu: the number in the checkpoint
-    names (the device index by default)."""
+    names (the device index by default).  precision: "fp32" (the reference's) or "bf16" (the step and the test pass
+    under bfloat16 autocast, point_layers="torch" only; parameters, Adam's state, BatchNorm's buffers and the
+    checkpoints stay float32)."""
 
     def __init__(self, model, train_source, test_source, dataset, out_dir, batch_size=None, seed=0, epochs=EPOCHS,
-                 version=None, gpu=None, log=print):
+                 version=None, gpu=None, log=print, precision="fp32"):
         if not isinstance(model, network.KeypointDetector):
             raise TypeError("Trainer trains a network.KeypointDetector")
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
+        if precision == "bf16" and model.point_layers != "torch":
+            raise ValueError(f"precision='bf16' needs point_layers='torch', the model has {model.point_layers!r}: the "
+                             f"fused point layers are float32 TF32 kernels")
+        self.precision = precision
         d = DEFAULTS[dataset]
         self.model, self.dataset, self.out_dir, self.log = model, dataset, out_dir, log
         self.batch_size = int(batch_size or d["batch_size"])
@@ -270,7 +300,7 @@ class Trainer:
 
     # -- the step ------------------------------------------------------------------------------------------------------
     def _body(self):
-        self.sums += _stats(train_step(self.model, self.optimizer, self.inputs)).double()
+        self.sums += _stats(train_step(self.model, self.optimizer, self.inputs, self.precision)).double()
 
     def _step(self):
         if self.graph is not None:
@@ -330,11 +360,7 @@ class Trainer:
                     seed, rng = batch_draws(self.seed, epoch, b, test=True)
                     t = self.make_test(items, seed, rng, None)
                     inp = dict(zip(INPUT_FIELDS, (v.to(self.device, torch.float32) for v in t[:8])))
-                    scores = model(*(inp[k] for k in ("pc", "intensity", "sn", "node_a", "node_b", "img")))
-                    coarse, fine = scores if model.fine else (scores, None)
-                    out = classifier.classifier_loss(coarse, fine, inp["pc"], inp["P"], inp["K"], model.img_H,
-                                                     model.img_W, model.fine_scale,
-                                                     coarse_loss_alpha=coarse_loss_alpha(model.fine))
+                    out = _forward_loss(model, inp, self.precision)
                     sums += len(items) * _stats(out).double()
                     n += len(items)
         finally:

@@ -472,6 +472,13 @@ size_t interp_backward_workspace_bytes(int B, int C, int Nq, int M);
 int interp_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* w, const int32_t* idx, int B,
                         int C, int Nq, int M, int k, float* grad_features, void* workspace, size_t workspace_bytes,
                         dib_stream_t stream);
+/* bfloat16 features, output and gradients, passed as uint16_t bit patterns (DESIGN.md 4.37): the f32 call's result on
+ * the widened inputs, rounded to nearest even at each store.  The weights and the workspace are the f32 calls'. */
+int interp_forward_bf16(const uint16_t* features, const float* w, const int32_t* idx, int B, int C, int Nq, int M,
+                        int k, uint16_t* out, dib_stream_t stream);
+int interp_backward_bf16(const uint16_t* grad_out, int64_t grad_batch_stride, const float* w, const int32_t* idx,
+                         int B, int C, int Nq, int M, int k, uint16_t* grad_features, void* workspace,
+                         size_t workspace_bytes, dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * The point encoder's SO-Net cluster max-pool and node kNN grouping (models/networks_pc.py:88-111,
@@ -510,6 +517,20 @@ size_t knn_group_backward_workspace_bytes(int B, int C, int M, int N, int K);
 int knn_group_backward_f32(const float* grad_grouped, int64_t grad_batch_stride, const int32_t* knn_idx, int B, int C,
                            int M, int N, int K, float* grad_features, void* workspace, size_t workspace_bytes,
                            dib_stream_t stream);
+/* bfloat16 features, pooled, scattered, grouped and gradients, passed as uint16_t bit patterns (DESIGN.md 4.37): the
+ * f32 call's result on the widened inputs, rounded to nearest even at each store (grouped's coordinate rows too).  The
+ * arg-max, mask, indices, coordinates and workspaces are the f32 calls'. */
+int cluster_pool_forward_bf16(const uint16_t* features, const int32_t* min_idx, int B, int C, int N, int M,
+                              int32_t* sel, float* mask, uint16_t* pooled, uint16_t* scattered, dib_stream_t stream);
+int cluster_pool_backward_bf16(const uint16_t* grad_pooled, const uint16_t* grad_scattered,
+                               int64_t grad_scattered_batch_stride, const int32_t* min_idx, const int32_t* sel,
+                               const float* mask, int B, int C, int N, int M, uint16_t* grad_features, void* workspace,
+                               size_t workspace_bytes, dib_stream_t stream);
+int knn_group_forward_bf16(const float* query, const float* database, const uint16_t* features, int B, int C, int M,
+                           int N, int K, int32_t* knn_idx, uint16_t* grouped, dib_stream_t stream);
+int knn_group_backward_bf16(const uint16_t* grad_grouped, int64_t grad_batch_stride, const int32_t* knn_idx, int B,
+                            int C, int M, int N, int K, uint16_t* grad_features, void* workspace,
+                            size_t workspace_bytes, dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * The classifier's attention-weighted image-feature fusion (models/networks_united.py:149-150,172-174,
@@ -531,6 +552,13 @@ int attn_fusion_forward_f32(const float* img_features, const float* attention, i
 int attn_fusion_backward_f32(const float* grad_out, int64_t grad_batch_stride, const float* img_features,
                              const float* attention, int B, int C, int P, int M, float* grad_img_features,
                              float* grad_attention, dib_stream_t stream);
+/* bfloat16 operands, output and gradients, passed as uint16_t bit patterns (DESIGN.md 4.37): the f32 call's result on
+ * the widened inputs, rounded to nearest even at each store. */
+int attn_fusion_forward_bf16(const uint16_t* img_features, const uint16_t* attention, int B, int C, int P, int M,
+                             uint16_t* out, dib_stream_t stream);
+int attn_fusion_backward_bf16(const uint16_t* grad_out, int64_t grad_batch_stride, const uint16_t* img_features,
+                              const uint16_t* attention, int B, int C, int P, int M, uint16_t* grad_img_features,
+                              uint16_t* grad_attention, dib_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * The image side of classifier batches (data/kitti_pc_img_pose_loader.py:326-349,360-362,439-440,
@@ -608,6 +636,23 @@ int classifier_loss_backward_f32(const float* coarse, int64_t coarse_batch_strid
                                  const float* grad_loss, const float* grad_coarse_loss, const float* grad_fine_loss,
                                  double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
                                  float* grad_coarse, float* grad_fine, dib_stream_t stream);
+/* bfloat16 scores and score gradients, passed as uint16_t bit patterns (DESIGN.md 4.37): the f32 call on the widened
+ * scores, its score gradients rounded to nearest even; every other output keeps the f32 call's type and value. */
+int classifier_loss_forward_bf16(const uint16_t* coarse, int64_t coarse_batch_stride, const uint16_t* fine,
+                                 int64_t fine_batch_stride, int L, const float* pc, const double* P12,
+                                 const double* K9, int B, int N, double H, double W, double fine_scale, int H_f,
+                                 int W_f, double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
+                                 int8_t* coarse_labels, int32_t* fine_labels, int8_t* coarse_pred, int32_t* fine_pred,
+                                 float* lse, float* loss, float* coarse_loss, float* fine_loss, float* accuracy,
+                                 int32_t* n_inside, int32_t* coarse_correct, int32_t* fine_correct,
+                                 int32_t* n_inside_total, void* workspace, size_t workspace_bytes,
+                                 dib_stream_t stream);
+int classifier_loss_backward_bf16(const uint16_t* coarse, int64_t coarse_batch_stride, const uint16_t* fine,
+                                  int64_t fine_batch_stride, int L, int B, int N, const int8_t* coarse_labels,
+                                  const int32_t* fine_labels, const float* lse, const int32_t* n_inside_total,
+                                  const float* grad_loss, const float* grad_coarse_loss, const float* grad_fine_loss,
+                                  double coarse_loss_alpha, double focal_alpha, int focal_gamma, double eps,
+                                  uint16_t* grad_coarse, uint16_t* grad_fine, dib_stream_t stream);
 int classifier_prediction_accuracy_f32(const float* pc, const double* P12, const double* K9, const int8_t* coarse_pred,
                                        const int32_t* fine_pred, int B, int N, double H, double W, double fine_scale,
                                        int H_f, int W_f, int8_t* coarse_labels, int32_t* fine_labels,

@@ -4,7 +4,7 @@ GPU, with the reference's schedule, test pass, loss lines and checkpoint names (
     python scripts/train_classifier.py --dataset {kitti,oxford,nuscenes} --root R --out DIR
         [--epochs 101] [--batch B] [--seed 0] [--version V] [--coarse-only] [--resnet-weights FILE]
         [--record-dir NAME] [--nuscenes-version V] [--resume DIR/resume.pth] [--store {cuda,pinned}]
-        [--point-layers {torch,fused}]
+        [--point-layers {torch,fused,fused_all}] [--precision {fp32,bf16}]
 
 Every epoch writes DIR/v{version}-gpu{gpu}-epoch{epoch}-{test coarse accuracy}.pth (the detector's state_dict, which
 network.load_checkpoint and the reference's load_model read) and DIR/resume.pth (model, optimiser, epoch, step
@@ -42,6 +42,9 @@ def parse_args(argv=None):
                     help="fused: the per-point chains as point_ops.point_chain (TF32, its own dropout stream); "
                          "fused_all: also the kNN module, final_pointnet and the node-level PointNets as "
                          "point_ops.point_branch")
+    ap.add_argument("--precision", default="fp32", choices=train.PRECISIONS,
+                    help="bf16: the forward and the loss under bfloat16 autocast (with --point-layers torch only); "
+                         "parameters, optimiser state and checkpoints stay float32")
     a = ap.parse_args(argv)
     if a.epochs < 1:
         ap.error("--epochs must be >= 1")
@@ -53,6 +56,8 @@ def parse_args(argv=None):
         ap.error("--nuscenes-version is a nuScenes setting")
     if a.store is not None and a.dataset == "nuscenes":
         ap.error("--store: nuScenes batches read their sweeps from the files")
+    if a.precision == "bf16" and a.point_layers != "torch":
+        ap.error("--precision bf16 needs --point-layers torch")
     return a
 
 
@@ -68,7 +73,7 @@ def main(argv=None):
     print("#training point clouds = %d" % trainset[0])
     print("#testing point clouds = %d" % testset[0])
     trainer = train.Trainer(model, trainset, testset, a.dataset, a.out, batch_size=a.batch, seed=a.seed,
-                            epochs=a.epochs, version=a.version)
+                            epochs=a.epochs, version=a.version, precision=a.precision)
     if a.resume:
         trainer.resume(a.resume)
     return trainer.run()
